@@ -117,7 +117,7 @@ struct vxb_context
 	DevBuf<uint8_t> lattice1;
 	uint8_t* latticePtr = nullptr;  // lattice1.p, or the cube's fourth channel
 	bool haveLattice1 = false, latticeOff = false;
-	int gridBlock[3] = { 0, 0, 0 }, gridBlock0Small = 0, level0Threads = 256, gridDecideBig = 0, gridTransition = 0;
+	int gridBlock[3] = { 0, 0, 0 }, gridDecideBig = 0, gridTransition = 0;
 	DevBuf<unsigned char> mixInfo, coarseDone;
 	DevBuf<unsigned short> mixCount;
 	// lattices of the coarse levels (VxbDev::coarseLattice): own buffer, or - sharded runs - an area of the buffer the peers map
@@ -653,10 +653,8 @@ int vxb_create(int device, vxb_context** out)
 
 	ctx->graphDisabled = getenv("VXB200_NO_GRAPH") != nullptr; // plain launches (debugging, A/B timing)
 	struct KernelSetup { const void* fn; size_t smem; int* grid; const char* name; int threads; };
-	ctx->level0Threads = getenv("VXB200_L0_THREADS") ? atoi(getenv("VXB200_L0_THREADS")) : 256; // A/B switch: 256 (default: measured faster) or 128
-	const KernelSetup setups[6] = {
+	const KernelSetup setups[5] = {
 		{ (const void*)vxb_block_kernel<0, 256>, sizeof(VxbBlockSmem<0, 256>), &ctx->gridBlock[0], "vxb_block_kernel<0, 256>", 256 },
-		{ (const void*)vxb_block_kernel<0, 128>, sizeof(VxbBlockSmem<0, 128>), &ctx->gridBlock0Small, "vxb_block_kernel<0, 128>", 128 },
 		{ (const void*)vxb_block_kernel<1, 256>, sizeof(VxbBlockSmem<1, 256>), &ctx->gridBlock[1], "vxb_block_kernel<1>", VXB_THREADS },
 		{ (const void*)vxb_block_kernel<2, 256>, sizeof(VxbBlockSmem<2, 256>), &ctx->gridBlock[2], "vxb_block_kernel<2>", VXB_THREADS },
 		{ (const void*)vxb_decide_kernel<4096, 1>, sizeof(VxbDecideSmemBig), &ctx->gridDecideBig, "vxb_decide_kernel<4096>", VXB_THREADS },
@@ -1388,8 +1386,7 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 			if (selectLevel(0))
 			{
 				timer.begin(3);
-				if (ctx->level0Threads == 256) vxb_block_kernel<0, 256><<<ctx->gridBlock[0], 256, sizeof(VxbBlockSmem<0, 256>), st>>>(ctx->tmapDist19, ctx->tmapDist19, dev, 0);
-				else vxb_block_kernel<0, 128><<<ctx->gridBlock0Small, 128, sizeof(VxbBlockSmem<0, 128>), st>>>(ctx->tmapDist19, ctx->tmapDist19, dev, 0);
+				vxb_block_kernel<0, 256><<<ctx->gridBlock[0], 256, sizeof(VxbBlockSmem<0, 256>), st>>>(ctx->tmapDist19, ctx->tmapDist19, dev, 0);
 				timer.end(); ++launches; ++ctx->kindLaunches[3];
 			}
 			vxb_mark_split_kernel<<<1, 1, 0, st>>>(dev); ++launches; // level 0 is complete: the flat kernels work on [split, end)

@@ -78,15 +78,14 @@ struct VxbTileView
 	const unsigned char* blend;
 	int ox, oy, oz;              // block origin (grid coordinates of its first voxel)
 	int sx, sy, sz;              // first coordinate held by the distance tile: (origin.x - 16, origin.y - 1, origin.z - 1)
-	                             // - TMA needs a 16-byte aligned innermost start -, or 0 on the low grid edge
+	                             // - TMA needs a 16-byte aligned innermost start -, also on the low grid edge
 	int n;                       // grid edge
 };
 
-// low edge: coordinate -1 clamps to 0 = the tile's first sample; the far edge is replicated when the tile is filled
+// every tap of a level-0 vertex lies in [origin - 1, origin + 17]: the tile holds it, clamped values included
 VXB_FN int vxb_dist(const VxbTileView& g, int x, int y, int z)
 {
-	const int xi = (x < g.sx ? g.sx : x) - g.sx, yi = (y < g.sy ? g.sy : y) - g.sy, zi = (z < g.sz ? g.sz : z) - g.sz;
-	return g.dist[(zi * 19 + yi) * 48 + xi];
+	return g.dist[((z - g.sz) * 19 + (y - g.sy)) * 48 + (x - g.sx)];
 }
 VXB_FN size_t vxb_tile_mat_index(const VxbTileView& g, int x, int y, int z)
 {

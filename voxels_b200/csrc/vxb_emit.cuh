@@ -19,13 +19,10 @@
 // Bit-exactness notes are in vxb_kernels.cuh / vxb_cell.h; the formulation is identical, only the schedule differs.
 #pragma once
 #ifndef VXB_OCC
-#define VXB_OCC 5 // resident CTAs per SM the per-block kernels are compiled for (register cap 65536 / (256 * VXB_OCC))
+#define VXB_OCC 4 // resident CTAs per SM the per-block kernels are compiled for (register cap 65536 / (256 * VXB_OCC))
 #endif
 #ifndef VXB_FLAT_OCC
 #define VXB_FLAT_OCC 4 // same for the flat per-vertex kernels
-#endif
-#ifndef VXB_VB_OCC
-#define VXB_VB_OCC 8 // and for the 128-thread level-0 vertex kernel
 #endif
 
 // Non-trivial bits of all 4096 cells from the tile, 16 cells per thread-step instead of one:
@@ -81,9 +78,7 @@ __device__ __forceinline__ unsigned vxb_rank_of(const unsigned int* nt32, const 
 #define VXB_DTILE_BYTES (19 * 19 * VXB_DTILE_PITCH)
 // Capacities of the shared-memory path of vxb_block_kernel<MODE, T>: non-trivial cells of a block (larger blocks go to
 // vxb_decide_kernel<4096, 1>) and new vertices of a level-0 block generated inside the CTA (more => the flat kernels).
-// The 128-thread level-0 variant trades capacity and the second tile buffer for twice as many resident CTAs.
 template <int MODE, int T> struct VxbBlockCaps { static constexpr int CAP = 1024, VL = (MODE == 0 ? 2048 : 8), NBUF = (MODE == 0 ? 1 : 2); }; // level 0: one tile buffer => 4 CTAs per SM
-template <> struct VxbBlockCaps<0, 128> { static constexpr int CAP = 512, VL = 1024, NBUF = 1; };
 
 // ------------------------------------------------------------------------------------------------
 // vxb_block_kernel<MODE>: everything that needs the block as a unit, in ONE pass over its sample tile
@@ -114,7 +109,7 @@ struct __align__(128) VxbBlockSmem
 	unsigned int hist[16];
 	unsigned int used[8];
 	unsigned long long mbar[2];
-	unsigned int item, hasChild, pageReady, emitIdx, voff, ioff, cellBase, slot, take, removed;
+	unsigned int item, ahead, hasChild, pageReady, emitIdx, voff, ioff, cellBase, slot, take, removed;
 	unsigned int levelEnd[VXB_MAX_LEVELS + 1];
 	unsigned int recA[Caps::CAP];     // matId | matBlend<<8 | slotK<<16
 	unsigned int recB[Caps::CAP];     // newMask | quirkMask<<12 | reuse mask << 24
@@ -133,7 +128,7 @@ __device__ __forceinline__ bool vxb_overflowed(const VxbDev& d)
 }
 
 template <int MODE, int T>
-__global__ void __launch_bounds__(T, (MODE == 0 ? (T == 128 ? 5 : 4) : (MODE == 2 ? 4 : VXB_OCC))) vxb_block_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB, const VxbDev d, const int levelArg)
+__global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB, const VxbDev d, const int levelArg)
 {
 	constexpr int PITCH = (MODE == 0) ? VXB_DTILE_PITCH : VXB_TILE_PITCH;
 	constexpr int ROWS = (MODE == 0) ? 19 : 17;
@@ -207,28 +202,32 @@ __global__ void __launch_bounds__(T, (MODE == 0 ? (T == 128 ? 5 : 4) : (MODE == 
 		{
 			if (tid == 0)
 			{
-				// the tile starts one sample before the block, except on the low grid edge (all TMA coordinates stay >= 0)
-				const int sx = bx ? bx * 16 - 16 : 0, sy = by ? by * 16 - 1 : 0, sz = bz ? bz * 16 - 1 : 0; // x start 16-byte aligned
+				// the tile starts one sample before the block (x: 16 samples, a 16-byte aligned start); on the low grid edge
+				// the box starts at a negative coordinate and TMA zero-fills what lies outside the volume
 				vxb_fence_proxy_async();
 				vxb_mbar_expect_tx(&s.mbar[buf], VXB_DTILE_BYTES);
-				vxb_tma_load_3d(s.tiles[buf], &tmapA, sx, sy, sz, &s.mbar[buf]);
+				vxb_tma_load_3d(s.tiles[buf], &tmapA, bx * 16 - 16, by * 16 - 1, bz * 16 - 1, &s.mbar[buf]);
 			}
 		}
 		else if (MODE == 1) vxb_tile_issue(s.tiles[buf], &s.mbar[buf], &tmapA, &tmapB, d, level, bx, by, bz);
 	};
 
-	if (tid == 0) s.item = atomicAdd(cursor, 1u);
+	// MODE 0 takes its items two ahead: the cursor's round trip for the item after next overlaps a whole block (the other
+	// modes keep the register it costs)
+	constexpr bool AHEAD = MODE == 0;
+	if (tid == 0) { s.item = atomicAdd(cursor, 1u); if (AHEAD) s.ahead = atomicAdd(cursor, 1u); }
 	__syncthreads();
-	unsigned item = s.item;
+	unsigned item = s.item, aheadItem = AHEAD ? s.ahead : 0u;
 	int buf = 0;
 	if (item < workCount) { int l, x, y, z; decode(item, l, x, y, z); issue(0, l, x, y, z); }
 	__syncthreads();
 
 	while (item < workCount)
 	{
-		if (tid == 0) { s.item = atomicAdd(cursor, 1u); s.hasChild = 0; s.pageReady = 0; s.take = 1; s.removed = 0; }
+		unsigned ahead = 0; // thread 0: the item after next, published in s.ahead at the end of this block
+		if (tid == 0) { if (AHEAD) ahead = atomicAdd(cursor, 1u); else s.item = atomicAdd(cursor, 1u); s.hasChild = 0; s.pageReady = 0; s.take = 1; s.removed = 0; }
 		__syncthreads();
-		const unsigned nextItem = s.item;
+		const unsigned nextItem = AHEAD ? aheadItem : s.item;
 		bool nextIssued = false; // NBUF == 1: the next tile is requested as soon as this one is not read any more
 		if (nextItem < workCount && MODE != 2 && NBUF == 2) { int l, x, y, z; decode(nextItem, l, x, y, z); issue(buf ^ 1, l, x, y, z); nextIssued = true; }
 		int level, bx, by, bz;
@@ -293,44 +292,47 @@ __global__ void __launch_bounds__(T, (MODE == 0 ? (T == 128 ? 5 : 4) : (MODE == 
 
 		// ---- tile ----
 		const signed char* tile; // sample (0, 0, 0) of the block
-		int hsx = 0, hsy = 0, hsz = 0; // MODE 0: first coordinate held by the halo tile
+		const int hsx = bx * 16 - 16, hsy = by * 16 - 1, hsz = bz * 16 - 1; // MODE 0: first coordinate held by the halo tile
 		if (MODE == 0)
 		{
-			hsx = bx ? bx * 16 - 16 : 0; hsy = by ? by * 16 - 1 : 0; hsz = bz ? bz * 16 - 1 : 0;
 			vxb_mbar_wait(&s.mbar[buf], (phaseBits >> buf) & 1u);
 			phaseBits ^= 1u << buf;
-			// far grid edge: TMA zero-fills outside the volume, the reference clamps the coordinate to n-1 (:1037-1047, :1198)
+			// grid edges: TMA zero-fills outside the volume, the reference clamps the coordinate to [0, n-1] (:1037-1047, :1198).
+			// One axis after the other, so that edge and corner entries copy values already fixed on the earlier axes.
 			const int lastX = d.n - 1 - hsx, lastY = d.n - 1 - hsy, lastZ = d.n - 1 - hsz; // tile index of coordinate n-1
-			if (bx == nb - 1)
+			if (bx == 0 || bx == nb - 1)
 			{
 				__syncthreads();
 				for (int i = tid; i < 19 * 19; i += T)
 				{
 					signed char* r = tileRaw + i * VXB_DTILE_PITCH;
-					r[lastX + 1] = r[lastX]; r[lastX + 2] = r[lastX];
+					if (bx == 0) r[15] = r[16];
+					if (bx == nb - 1) { r[lastX + 1] = r[lastX]; r[lastX + 2] = r[lastX]; }
 				}
 			}
-			if (by == nb - 1)
+			if (by == 0 || by == nb - 1)
 			{
 				__syncthreads();
 				for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += T)
 				{
 					const int z = i / VXB_DTILE_PITCH, x = i % VXB_DTILE_PITCH;
 					signed char* p = tileRaw + z * 19 * VXB_DTILE_PITCH + x;
-					for (int q = lastY + 1; q < 19; ++q) p[q * VXB_DTILE_PITCH] = p[lastY * VXB_DTILE_PITCH];
+					if (by == 0) p[0] = p[VXB_DTILE_PITCH];
+					if (by == nb - 1) for (int q = lastY + 1; q < 19; ++q) p[q * VXB_DTILE_PITCH] = p[lastY * VXB_DTILE_PITCH];
 				}
 			}
-			if (bz == nb - 1)
+			if (bz == 0 || bz == nb - 1)
 			{
 				__syncthreads();
 				for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += T)
 				{
 					const int y = i / VXB_DTILE_PITCH, x = i % VXB_DTILE_PITCH;
 					signed char* p = tileRaw + y * VXB_DTILE_PITCH + x;
-					for (int q = lastZ + 1; q < 19; ++q) p[q * 19 * VXB_DTILE_PITCH] = p[lastZ * 19 * VXB_DTILE_PITCH];
+					if (bz == 0) p[0] = p[19 * VXB_DTILE_PITCH];
+					if (bz == nb - 1) for (int q = lastZ + 1; q < 19; ++q) p[q * 19 * VXB_DTILE_PITCH] = p[lastZ * 19 * VXB_DTILE_PITCH];
 				}
 			}
-			tile = tileRaw + ((bz * 16 - hsz) * 19 + (by * 16 - hsy)) * VXB_DTILE_PITCH + (bx * 16 - hsx);
+			tile = tileRaw + (19 + 1) * VXB_DTILE_PITCH + 16;
 		}
 		else if (MODE == 2)
 		{
@@ -367,7 +369,8 @@ __global__ void __launch_bounds__(T, (MODE == 0 ? (T == 128 ? 5 : 4) : (MODE == 
 				if (tid < 128)
 				{
 					unsigned* page = d.consPages + (size_t)coordId * 128;
-					page[tid] = d.consValid[coordId] ? (page[tid] | s.nt32[tid]) : s.nt32[tid]; // bits are only ever set (:757)
+					// bits are only ever set (:757); a full run has cleared consValid, and this block is the only one that sets its flag
+					page[tid] = (d.incremental && d.consValid[coordId]) ? (page[tid] | s.nt32[tid]) : s.nt32[tid];
 				}
 			}
 			else if (!d.cacheValid[level][coordId]) vxb_init_cache_page(d, level, coordId);
@@ -718,9 +721,11 @@ __global__ void __launch_bounds__(T, (MODE == 0 ? (T == 128 ? 5 : 4) : (MODE == 
 				}
 			}
 		}
+		if (AHEAD && tid == 0) s.ahead = ahead;
 		__syncthreads();
 		if (NBUF == 1 && MODE != 2 && !nextIssued && nextItem < workCount) { int l2, x2, y2, z2; decode(nextItem, l2, x2, y2, z2); issue(0, l2, x2, y2, z2); }
 		item = nextItem;
+		if (AHEAD) aheadItem = s.ahead;
 		if (NBUF == 2) buf ^= 1;
 	}
 
@@ -1007,128 +1012,6 @@ __global__ void __launch_bounds__(VXB_THREADS, VXB_FLAT_OCC) vxb_vertex_kernel(c
 	}
 	__syncthreads();
 	if (threadIdx.x < 8 && sUsed[threadIdx.x]) atomicOr(&d.counters->usedMaterials[threadIdx.x], sUsed[threadIdx.x]);
-}
-
-// Level-0 vertices, one emitted block per CTA iteration: the block's distance neighbourhood (19^3) is staged by one TMA
-// load, so the twelve distance taps of a vertex come from shared memory instead of separate 32-byte DRAM sectors.
-// Grid-edge clamping (:1198) is baked into the tile.  (Staging the material / blend samples too was slower: the extra
-// 18 KB per CTA halve the occupancy.)
-#define VXB_VB_CELLS 512   // blocks with more non-trivial cells read their records from global memory
-#define VXB_VB_THREADS 128 // a block has ~350 new vertices: 128-thread CTAs waste fewer lanes in the last round and more of them fit an SM
-struct __align__(128) VxbVertexBlockSmem
-{
-	signed char dist[VXB_DTILE_BYTES + 80];
-	unsigned long long mbar;
-	unsigned int item;
-	unsigned int used[8];
-	uint4 cells[VXB_VB_CELLS]; // the block's cell records, staged while the TMA load is in flight
-};
-
-__global__ void __launch_bounds__(VXB_VB_THREADS, VXB_VB_OCC) vxb_vertex_block_kernel(const __grid_constant__ CUtensorMap tmapDist19, const VxbDev d)
-{
-	extern __shared__ __align__(128) unsigned char smemRaw[];
-	VxbVertexBlockSmem& s = *reinterpret_cast<VxbVertexBlockSmem*>(smemRaw);
-	const int tid = threadIdx.x;
-	if (tid == 0) vxb_mbar_init(&s.mbar, 1);
-	if (tid < 8) s.used[tid] = 0;
-	__syncthreads();
-	unsigned phase = 0;
-	const bool live = !vxb_overflowed(d);
-	const unsigned count = live ? d.counters->splitRecords : 0u; // level-0 blocks own the first directory slots
-	const int nb = d.n / 16;
-	for (;;)
-	{
-		if (tid == 0) s.item = atomicAdd(&d.counters->vertexBlockCursor, 1u);
-		__syncthreads();
-		const unsigned slot = s.item;
-		if (slot >= count) break;
-		const VxbBlockRec* br = &d.blockRecs[slot];
-		const unsigned coordId = br->packed & 0x0FFFFFFFu;
-		const unsigned voff = br->voff, nverts = br->nverts, cellBase = br->cellBase, ntc = br->ntc;
-		const bool staged = ntc <= VXB_VB_CELLS;
-		const int bx = coordId % nb, by = (coordId / nb) % nb, bz = coordId / (nb * nb);
-		// the distance tile starts one sample before the block, except on the low grid edge (all TMA coordinates stay >= 0)
-		const int sx = bx ? bx * 16 - 16 : 0, sy = by ? by * 16 - 1 : 0, sz = bz ? bz * 16 - 1 : 0; // x start 16-byte aligned
-		if (tid == 0)
-		{
-			vxb_fence_proxy_async();
-			vxb_mbar_expect_tx(&s.mbar, VXB_DTILE_BYTES);
-			vxb_tma_load_3d(s.dist, &tmapDist19, sx, sy, sz, &s.mbar);
-		}
-		if (staged)
-			for (unsigned i = tid; i < ntc; i += VXB_VB_THREADS) s.cells[i] = *reinterpret_cast<const uint4*>(&d.cellRecs[cellBase + i]);
-		unsigned e = (tid < nverts) ? d.vlist[voff + tid] : 0u;
-		vxb_mbar_wait(&s.mbar, phase);
-		phase ^= 1;
-		// far grid edge: TMA zero-fills outside the volume, the reference clamps the coordinate to n-1
-		const int lastX = d.n - 1 - sx, lastY = d.n - 1 - sy, lastZ = d.n - 1 - sz; // tile index of coordinate n-1
-		if (bx == nb - 1)
-		{
-			__syncthreads();
-			for (int i = tid; i < 19 * 19; i += VXB_VB_THREADS)
-			{
-				signed char* r = s.dist + i * VXB_DTILE_PITCH;
-				r[lastX + 1] = r[lastX]; r[lastX + 2] = r[lastX];
-			}
-		}
-		if (by == nb - 1)
-		{
-			__syncthreads();
-			for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += VXB_VB_THREADS)
-			{
-				const int z = i / VXB_DTILE_PITCH, x = i % VXB_DTILE_PITCH;
-				signed char* p = s.dist + z * 19 * VXB_DTILE_PITCH + x;
-				for (int q = lastY + 1; q < 19; ++q) p[q * VXB_DTILE_PITCH] = p[lastY * VXB_DTILE_PITCH];
-			}
-		}
-		if (bz == nb - 1)
-		{
-			__syncthreads();
-			for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += VXB_VB_THREADS)
-			{
-				const int y = i / VXB_DTILE_PITCH, x = i % VXB_DTILE_PITCH;
-				signed char* p = s.dist + y * VXB_DTILE_PITCH + x;
-				for (int q = lastZ + 1; q < 19; ++q) p[q * 19 * VXB_DTILE_PITCH] = p[lastZ * 19 * VXB_DTILE_PITCH];
-			}
-		}
-		__syncthreads();
-		VxbTileView g;
-		g.dist = s.dist; g.ox = bx * 16; g.oy = by * 16; g.oz = bz * 16; g.sx = sx; g.sy = sy; g.sz = sz;
-		g.mat = d.grid.mat; g.blend = d.grid.blend; g.n = d.n; // the two material / blend taps of a vertex stay global loads
-		for (unsigned j = tid; j < nverts; j += VXB_VB_THREADS)
-		{
-			const unsigned ci = e >> 4; const int k = e & 15;
-			if (j + VXB_VB_THREADS < nverts) e = d.vlist[voff + j + VXB_VB_THREADS]; // next round's entry, in flight during this one
-			const uint4 crv = staged ? s.cells[ci - cellBase] : *reinterpret_cast<const uint4*>(&d.cellRecs[ci]);
-			const int c = crv.x & 0xFFF;
-			const unsigned code = (crv.x >> 12) & 0xFF, zm = (crv.x >> 20) & 0xFF;
-			const int local[3] = { c & 15, (c >> 4) & 15, c >> 8 };
-			const int base[3] = { bx * 16 + local[0], by * 16 + local[1], bz * 16 + local[2] };
-			const unsigned matId = crv.y & 0xFF, matBlend = (crv.y >> 8) & 0xFF;
-			VxbVertexDesc vd = vxb_regular_vertex_desc_lite(vxbGRegularVertexData[code * 12 + k], zm);
-			VxbRawVertex rv;
-			if (vd.endpoint)
-			{
-				const bool quirk = (crv.z >> (12 + k)) & 1u;
-				vxb_corner_vertex(g, 0, base, local, quirk ? vd.v0 : ((vd.t == 0) ? vd.v1 : vd.v0), matId, matBlend, rv);
-			}
-			else
-			{
-				const int a = vxb_dist(g, base[0] + (vd.v0 & 1), base[1] + ((vd.v0 >> 1) & 1), base[2] + (vd.v0 >> 2));
-				const int b = vxb_dist(g, base[0] + (vd.v1 & 1), base[1] + ((vd.v1 >> 1) & 1), base[2] + (vd.v1 >> 2));
-				vd.t = vxb_fixed_t(a, b); // :1591
-				vxb_edge_vertex(g, 0, base, local, vd, matId, matBlend, rv);
-			}
-			vxb_regular_secondary(0, rv);
-			VxbVertex ov;
-			vxb_finish_vertex(rv, *d.lut, ov);
-			vxb_store_vertex(d.verts + voff + j, ov);
-			atomicOr(&s.used[matId >> 5], 1u << (matId & 31));
-		}
-		__syncthreads();
-	}
-	__syncthreads();
-	if (tid < 8 && s.used[tid]) atomicOr(&d.counters->usedMaterials[tid], s.used[tid]);
 }
 
 __global__ void __launch_bounds__(VXB_THREADS) vxb_triangle_kernel(const VxbDev d, const int part)

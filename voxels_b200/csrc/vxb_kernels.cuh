@@ -43,7 +43,6 @@ struct VxbCounters
 	unsigned int bigCount[2], bigCursor[2]; // blocks with > 1024 non-trivial cells (second tier of vxb_decide_kernel)
 	unsigned int cells;                     // cursor of the cell-record arena
 	unsigned int splitVertices, splitCells, splitRecords; // cursors after group 0 (level 0): later kernels split their ranges there
-	unsigned int vertexBlockCursor;
 	unsigned int transBlocks, transCursor;  // emitted mid-level blocks (vxb_transition_kernel work list)
 	unsigned int finishCursor;
 	unsigned int coarseCursor;              // item cursor of the single launch that handles the coarse levels
@@ -937,9 +936,10 @@ __device__ __forceinline__ bool vxb_vote_candidate(const VxbVoteSource& d, const
 	return valid != 0u && (all & 0x00FF00FFu) != 0x00FF00FFu;
 }
 
-// returns id | blend << 8, or -1 when no child carries a material (results in a register: a noinline callee would
-// write reference outputs through local memory)
-__device__ __noinline__ int vxb_vote_cell(const VxbVoteSource d, const int bx0, const int by0, const int bz0)
+// returns id | blend << 8, or -1 when no child carries a material (results in a register: reference outputs would go
+// through local memory).  Inlined: as a call, the callee-saved registers of vxb_block_kernel<1> went to the stack around
+// every vote.
+__device__ __forceinline__ int vxb_vote_cell(const VxbVoteSource d, const int bx0, const int by0, const int bz0)
 {
 	const int level = d.level;
 	const int base[3] = { bx0, by0, bz0 };
