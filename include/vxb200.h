@@ -315,7 +315,7 @@ int vxb_set_capacity(vxb_context* ctx, uint64_t vertices, uint64_t indices, uint
 
 /* Per-kernel device time of the last vxb_polygonize run with VXB_FLAG_KERNEL_TIMES, for bench.py's roofline line:
  * which = 0: vxb_scan_kernel (streams the level-0 distance volume once), 1: block info, sign-mix pyramid + selection kernels,
- * 2: vxb_block_kernel<1>/<2> (levels >= 1: classification, votes, decisions) + vxb_decide_kernel<4096>, 3: vxb_block_kernel<0>
+ * 2: vxb_block_kernel<1>/<2> (levels >= 1: classification, votes, decisions) + vxb_big_block_kernel, 3: vxb_block_kernel<0>
  * (level 0: classification, decisions, vertices and triangles in one pass), 4: vxb_vertex_kernel (levels >= 1),
  * 5: vxb_triangle_kernel (levels >= 1), 6: vxb_transition_kernel + vertices, 7: vxb_finish_kernel; sharded runs (phase 3) also
  * 8: exchange 0 (lattice publication + ncclAllGather of the block info), 9: exchange 1 (page publication + the ordering all-gather).

@@ -10,7 +10,7 @@ import sys
 
 KINDS = [("vxb_scan", "scan"), ("vxb_block_info", "select"), ("vxb_pyramid", "select"), ("vxb_select", "select"), ("vxb_plan", "select"),
          ("vxb_block_kernel<0", "block_level0"), ("vxb_block_kernel<1", "block_levels1plus"), ("vxb_block_kernel<2", "block_levels1plus"),
-         ("vxb_classify", "classify"), ("vxb_decide", "block_levels1plus"), ("vxb_mark_split", "select"), ("vxb_vertex", "vertex"),
+         ("vxb_classify", "classify"), ("vxb_big_block", "block_levels1plus"), ("vxb_mark_split", "select"), ("vxb_vertex", "vertex"),
          ("vxb_triangle", "triangle"), ("vxb_transition", "transition"), ("vxb_finish", "finish"), ("vxb_publish", "exchange")]
 COLS = {"us": "gpu__time_duration.sum", "rd": "dram__bytes_read.sum", "wr": "dram__bytes_write.sum", "regs": "launch__registers_per_thread",
         "warps": "sm__warps_active.avg.pct_of_peak_sustained_active", "inst": "smsp__inst_executed.sum", "grid": "launch__grid_size",

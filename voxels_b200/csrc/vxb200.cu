@@ -30,8 +30,6 @@
 #include "vxb_grid.cuh"
 #include "vxb_draw.cuh"
 
-typedef VxbDecideSmem<4096> VxbDecideSmemBig;
-
 static_assert(sizeof(VxbVertex) == 48, "PolygonVertex layout");
 static_assert(sizeof(vxb_block_record) == 128, "record layout");
 
@@ -113,11 +111,10 @@ struct vxb_context
 	DevBuf<VxbMaterialLut> lut;
 	uint64_t capV = 0, capI = 0, capTV = 0, capTI = 0;
 	CUtensorMap tmap, tmap1, tmapDist19;
-	int gridVertexBlock = 0;
 	DevBuf<uint8_t> lattice1;
 	uint8_t* latticePtr = nullptr;  // lattice1.p, or the cube's fourth channel
 	bool haveLattice1 = false, latticeOff = false;
-	int gridBlock[3] = { 0, 0, 0 }, gridDecideBig = 0, gridTransition = 0;
+	int gridBlock[3] = { 0, 0, 0 }, gridBigBlock = 0, gridTransition = 0;
 	DevBuf<unsigned char> mixInfo, coarseDone;
 	DevBuf<unsigned short> mixCount;
 	// lattices of the coarse levels (VxbDev::coarseLattice): own buffer, or - sharded runs - an area of the buffer the peers map
@@ -654,10 +651,10 @@ int vxb_create(int device, vxb_context** out)
 	ctx->graphDisabled = getenv("VXB200_NO_GRAPH") != nullptr; // plain launches (debugging, A/B timing)
 	struct KernelSetup { const void* fn; size_t smem; int* grid; const char* name; int threads; };
 	const KernelSetup setups[5] = {
-		{ (const void*)vxb_block_kernel<0, 256>, sizeof(VxbBlockSmem<0, 256>), &ctx->gridBlock[0], "vxb_block_kernel<0, 256>", 256 },
-		{ (const void*)vxb_block_kernel<1, 256>, sizeof(VxbBlockSmem<1, 256>), &ctx->gridBlock[1], "vxb_block_kernel<1>", VXB_THREADS },
-		{ (const void*)vxb_block_kernel<2, 256>, sizeof(VxbBlockSmem<2, 256>), &ctx->gridBlock[2], "vxb_block_kernel<2>", VXB_THREADS },
-		{ (const void*)vxb_decide_kernel<4096, 1>, sizeof(VxbDecideSmemBig), &ctx->gridDecideBig, "vxb_decide_kernel<4096>", VXB_THREADS },
+		{ (const void*)vxb_block_kernel<0>, sizeof(VxbBlockSmem<0>), &ctx->gridBlock[0], "vxb_block_kernel<0>", VXB_THREADS },
+		{ (const void*)vxb_block_kernel<1>, sizeof(VxbBlockSmem<1>), &ctx->gridBlock[1], "vxb_block_kernel<1>", VXB_THREADS },
+		{ (const void*)vxb_block_kernel<2>, sizeof(VxbBlockSmem<2>), &ctx->gridBlock[2], "vxb_block_kernel<2>", VXB_THREADS },
+		{ (const void*)vxb_big_block_kernel, sizeof(VxbBigBlockSmem), &ctx->gridBigBlock, "vxb_big_block_kernel", VXB_THREADS },
 		{ (const void*)vxb_transition_kernel, 0, &ctx->gridTransition, "vxb_transition_kernel", VXB_TR_THREADS },
 	};
 	for (const KernelSetup& k : setups)
@@ -1386,16 +1383,16 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 			if (selectLevel(0))
 			{
 				timer.begin(3);
-				vxb_block_kernel<0, 256><<<ctx->gridBlock[0], 256, sizeof(VxbBlockSmem<0, 256>), st>>>(ctx->tmapDist19, ctx->tmapDist19, dev, 0);
+				vxb_block_kernel<0><<<ctx->gridBlock[0], VXB_THREADS, sizeof(VxbBlockSmem<0>), st>>>(ctx->tmapDist19, ctx->tmapDist19, dev, 0);
 				timer.end(); ++launches; ++ctx->kindLaunches[3];
 			}
-			vxb_mark_split_kernel<<<1, 1, 0, st>>>(dev); ++launches; // level 0 is complete: the flat kernels work on [split, end)
+			vxb_mark_split_kernel<<<1, 1, 0, st>>>(dev); ++launches; // level 0 is complete: the flat kernels work behind the split
 			for (int l = 1; l < coarseLo && l < computed; ++l)
 			{
 				if (!selectLevel(l)) continue;
 				if (l >= VXB_LATTICE_LO) joinLattice();
 				timer.begin(2);
-				vxb_block_kernel<1, 256><<<ctx->gridBlock[1], VXB_THREADS, sizeof(VxbBlockSmem<1, 256>), st>>>(ctx->tmap, ctx->tmap1, dev, l);
+				vxb_block_kernel<1><<<ctx->gridBlock[1], VXB_THREADS, sizeof(VxbBlockSmem<1>), st>>>(ctx->tmap, ctx->tmap1, dev, l);
 				timer.end(); ++launches; ++ctx->kindLaunches[2];
 			}
 			if (sharded && peers.count) { timer.begin(9); vxb_publish_kernel<<<(unsigned)ctx->smCount * 4, VXB_THREADS, 0, st>>>(dev, peers); timer.end(); ++launches; ++ctx->kindLaunches[9]; }
@@ -1408,12 +1405,12 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 			{
 				joinLattice(); // the lattices are complete
 				timer.begin(2);
-				vxb_block_kernel<2, 256><<<ctx->gridBlock[2], VXB_THREADS, sizeof(VxbBlockSmem<2, 256>), st>>>(ctx->tmap, ctx->tmap1, dev, coarseLo);
+				vxb_block_kernel<2><<<ctx->gridBlock[2], VXB_THREADS, sizeof(VxbBlockSmem<2>), st>>>(ctx->tmap, ctx->tmap1, dev, coarseLo);
 				timer.end(); ++launches; ++ctx->kindLaunches[2];
 			}
 			// blocks too large for the shared-memory path of vxb_block_kernel (> 1024 non-trivial cells / > 2048 level-0 vertices)
 			timer.begin(2);
-			vxb_decide_kernel<4096, 1><<<ctx->gridDecideBig, VXB_THREADS, sizeof(VxbDecideSmemBig), st>>>(ctx->tmap, ctx->tmap1, dev, 2);
+			vxb_big_block_kernel<<<ctx->gridBigBlock, VXB_THREADS, sizeof(VxbBigBlockSmem), st>>>(ctx->tmap, ctx->tmap1, dev);
 			timer.end(); ++launches; ++ctx->kindLaunches[2];
 			// vertices + triangles of everything but the level-0 blocks done inside vxb_block_kernel<0>, next to the transition
 			// cells (which need the block records and the material pages only)
@@ -1424,10 +1421,10 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 				VXB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->evFork, 0));
 			}
 			timer.begin(4);
-			vxb_vertex_kernel<<<flatGrid, VXB_THREADS, 0, st>>>(dev, 1);
+			vxb_vertex_kernel<<<flatGrid, VXB_THREADS, 0, st>>>(dev);
 			timer.end(); ++launches; ++ctx->kindLaunches[4];
 			timer.begin(5);
-			vxb_triangle_kernel<<<flatGrid, VXB_THREADS, 0, st>>>(dev, 1);
+			vxb_triangle_kernel<<<flatGrid, VXB_THREADS, 0, st>>>(dev);
 			timer.end(); ++launches; ++ctx->kindLaunches[5];
 			if (dev.transitions && computed > 1)
 			{

@@ -1,22 +1,14 @@
-// Fast path of the polygonizer (included by vxb200.cu after vxb_kernels.cuh).
+// Per-block and flat kernels of the polygonizer (included by vxb200.cu after vxb_kernels.cuh).
 //
-//   vxb_classify_kernel   per LOD level (levels depend on each other ONLY through this step):
-//                         tile -> case codes -> non-trivial bits; consistency page (level 0) or majority votes of
-//                         the non-trivial cells and of every transition-face cell into the level's material page
-//                         (CalculateMaterialForCellCache :753-838, called from :1568 and :1859); statistics;
-//                         appends blocks that have non-trivial cells to the emit list together with their bit mask.
-//   then ONE launch each for the blocks of ALL levels:
-//   vxb_decide_kernel<C>  per block (largest first): ordered compaction of the non-trivial cells, materials, owned reuse
-//                         slots, new-vs-reuse decisions, block scans -> vertex / triangle bases; reserves the output
-//                         ranges and writes one 16-byte record per cell + the vertex work list.  C = 1024 (34 KB smem),
-//                         larger blocks go to a second launch with C = 4096.
-//   vxb_vertex_kernel     flat, one thread per NEW VERTEX of the whole grid: position, normal, material, secondary.
-//   vxb_triangle_kernel   flat, one thread per non-trivial CELL: vertex ids (own + reused) and triangles with the
-//                         degenerate-triangle test of PushBlocksToResult (:1300-1321).
-//   vxb_transition_kernel per emitted mid-level block: the six transition faces (:1754-2131).
-//   vxb_finish_kernel     per emitted block: order-preserving compaction where triangles were removed + directory.
+//   vxb_block_kernel<MODE>  one pass per block: tile -> non-trivial cells, consistency page or material votes, statistics,
+//                           then the decide passes (vxb_decide_cells) and the arena reservation.  Level 0 makes the block's
+//                           vertices and triangles itself; levels >= 1 write cell records + the vertex work list.
+//   vxb_big_block_kernel    the decide passes of the blocks too large for the shared-memory path of vxb_block_kernel.
+//   vxb_vertex_kernel, vxb_triangle_kernel   flat, one thread per new vertex / per cell of the blocks with cell records.
+//   vxb_transition_kernel   per face of an emitted mid-level block: the transition cells (:1754-2131).
+//   vxb_finish_kernel       per emitted block: order-preserving compaction where triangles were removed + directory.
 //
-// Bit-exactness notes are in vxb_kernels.cuh / vxb_cell.h; the formulation is identical, only the schedule differs.
+// Launch order, occupancy and costs: DESIGN.md §4.  Bit-exactness notes are in vxb_kernels.cuh / vxb_cell.h.
 #pragma once
 #ifndef VXB_OCC
 #define VXB_OCC 4 // resident CTAs per SM the per-block kernels are compiled for (register cap 65536 / (256 * VXB_OCC))
@@ -76,9 +68,9 @@ __device__ __forceinline__ unsigned vxb_rank_of(const unsigned int* nt32, const 
 // axis, as 19 x 19 rows of 48 bytes (the TMA box starts on a 16-byte boundary one 16-byte group before the block).
 #define VXB_DTILE_PITCH 48
 #define VXB_DTILE_BYTES (19 * 19 * VXB_DTILE_PITCH)
-// Capacities of the shared-memory path of vxb_block_kernel<MODE, T>: non-trivial cells of a block (larger blocks go to
-// vxb_decide_kernel<4096, 1>) and new vertices of a level-0 block generated inside the CTA (more => the flat kernels).
-template <int MODE, int T> struct VxbBlockCaps { static constexpr int CAP = 1024, VL = (MODE == 0 ? 2048 : 8), NBUF = (MODE == 0 ? 1 : 2); }; // level 0: one tile buffer => 4 CTAs per SM
+// Capacities of the shared-memory path of vxb_block_kernel<MODE>: non-trivial cells of a block (larger blocks go to
+// vxb_big_block_kernel) and new vertices of a level-0 block generated inside the CTA (more => the flat kernels).
+template <int MODE> struct VxbBlockCaps { static constexpr int CAP = 1024, VL = (MODE == 0 ? 2048 : 8), NBUF = (MODE == 0 ? 1 : 2); }; // level 0: one tile buffer => 4 CTAs per SM
 
 // ------------------------------------------------------------------------------------------------
 // vxb_block_kernel<MODE>: everything that needs the block as a unit, in ONE pass over its sample tile
@@ -86,7 +78,7 @@ template <int MODE, int T> struct VxbBlockCaps { static constexpr int CAP = 1024
 //   every transition-face cell into the level's material page (CalculateMaterialForCellCache :753-838, called from :1568
 //   and :1859) - the only cross-level dependency; statistics; then, for blocks with non-trivial cells: ordered compaction,
 //   materials, owned reuse slots, new-vs-reuse decisions, block scans -> vertex / triangle bases, arena reservation.
-//   MODE 0  level 0 from its work list: halo tile by one TMA load (double buffered); the new vertices and the triangles
+//   MODE 0  level 0 from its work list: halo tile by one TMA load into one tile buffer; the new vertices and the triangles
 //           are produced right here from shared memory (no per-cell records in global memory).
 //   MODE 1  one level from its work list (17^3 tile: TMA for level 0 / the even lattice of level 1, strided gather else);
 //           writes 16-byte cell records + the vertex work list for the flat per-vertex / per-cell kernels.
@@ -94,10 +86,10 @@ template <int MODE, int T> struct VxbBlockCaps { static constexpr int CAP = 1024
 //           the done flags of its eight children (they were taken earlier from the same cursor, so they are running or
 //           done: no deadlock), applies the block-walk test itself, then works like MODE 1.
 // ------------------------------------------------------------------------------------------------
-template <int MODE, int T>
+template <int MODE>
 struct __align__(128) VxbBlockSmem
 {
-	typedef VxbBlockCaps<MODE, T> Caps;
+	typedef VxbBlockCaps<MODE> Caps;
 	signed char tiles[Caps::NBUF][MODE == 0 ? (VXB_DTILE_BYTES + 80) : (VXB_TILE_BYTES + 96)]; // NBUF = 2: the next block's tile lands while this one is worked on
 	unsigned int rowSign[17 * 17 + 3]; // bit x = sample (x, y, z) of the tile is negative
 	unsigned int nt32[128];
@@ -127,14 +119,157 @@ __device__ __forceinline__ bool vxb_overflowed(const VxbDev& d)
 	return c->vertices > d.vcap || c->indices > d.icap || c->cells > d.ccap || c->records > d.rcap;
 }
 
-template <int MODE, int T>
-__global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB, const VxbDev d, const int levelArg)
+// ---- the steps both per-block kernels (vxb_block_kernel, vxb_big_block_kernel) take over a block's non-trivial cells;
+// their shared memory has the arrays nt32, wpre, list, cz, recA, recB, vbase, tbase, the three tables and warpSums ----
+
+// ordered compact list of the non-trivial cells: thread = cell row (z, y), 16 bits each (VXB_THREADS = 256 rows)
+__device__ __forceinline__ void vxb_compact_cells(const unsigned int* nt32, const unsigned int* wpre, unsigned short* list)
+{
+	const int r = threadIdx.x;
+	unsigned bits = reinterpret_cast<const unsigned short*>(nt32)[r];
+	unsigned pos = wpre[r >> 1] + ((r & 1) ? __popc(nt32[r >> 1] & 0xFFFFu) : 0u);
+	while (bits) { const int x = __ffs(bits) - 1; bits &= bits - 1; list[pos++] = (unsigned short)(r * 16 + x); }
+}
+
+// The decide passes over the ntc cells of the compact list: pass A, pass B and the block scans; nverts / ntris = the block's
+// totals.  HIST: pass A takes the level-0 case histogram (PerCaseCellsCount :1574) into s.hist.  Ends without a barrier.
+template <int PITCH, int ROWS, bool HIST, class Smem>
+__device__ __forceinline__ void vxb_decide_cells(Smem& s, const signed char* tile, const VxbDev& d, int level, unsigned coordId,
+	int bx, int by, int bz, unsigned ntc, unsigned& nverts, unsigned& ntris)
+{
+	const int tid = threadIdx.x;
+	const VxbGrid g = d.grid;
+	// ---- pass A: material, case code, zero mask, owned slots ----
+	for (unsigned i = tid; i < ntc; i += VXB_THREADS)
+	{
+		const int c = s.list[i];
+		signed char v[8];
+		vxb_tile_samples<PITCH, ROWS>(tile, c, v);
+		const unsigned code = vxb_case_code(v);
+		const unsigned zm = vxb_zero_mask(v);
+		unsigned matId, matBlend;
+		if (level == 0)
+		{
+			if constexpr (HIST) atomicAdd(&s.hist[s.tabClass[code]], 1u);
+			const size_t gi = ((size_t)((bz * 16 + (c >> 8))) * d.n + (by * 16 + ((c >> 4) & 15))) * d.n + (bx * 16 + (c & 15));
+			matId = g.mat[gi]; matBlend = g.blend[gi];
+		}
+		else
+		{
+			const unsigned e = d.cachePages[level][(size_t)coordId * 4096 + c]; // the vote of vxb_block_kernel
+			matId = e & 0xFF; matBlend = e >> 8;
+		}
+		unsigned slotK = 0xFFFFu;
+		const int nv = s.tabCell[s.tabClass[code] * 16] >> 4;
+		for (int k = 0; k < nv; ++k)
+		{
+			const VxbVertexDesc vd = vxb_regular_vertex_desc_lite(s.tabVert[code * 12 + k], zm);
+			const int sl = vxb_regular_owned_slot(vd);
+			if (sl >= 0) slotK = (slotK & ~(0xFu << (4 * sl))) | ((unsigned)k << (4 * sl));
+		}
+		s.cz[i] = (unsigned short)(code | (zm << 8));
+		s.recA[i] = matId | (matBlend << 8) | (slotK << 16);
+	}
+	__syncthreads();
+
+	// ---- pass B: new-vs-reuse decisions ----
+	for (unsigned i = tid; i < ntc; i += VXB_THREADS)
+	{
+		const int c = s.list[i];
+		const unsigned code = s.cz[i] & 0xFF, zm = s.cz[i] >> 8;
+		const unsigned geo = s.tabCell[s.tabClass[code] * 16];
+		const unsigned rowStart = vxb_rank_of(s.nt32, s.wpre, c & ~15), sliceStart = s.wpre[(c >> 8) * 8];
+		const int mask = (i > rowStart ? 1 : 0) | (rowStart > sliceStart ? 2 : 0) | (sliceStart > 0 ? 4 : 0);
+		const unsigned myMat = s.recA[i] & 0xFF;
+		unsigned newMask = 0, quirkMask = 0;
+		for (int k = 0; k < (int)(geo >> 4); ++k)
+		{
+			// new-vs-reuse decision (:1610-1644) from the owner cell's record
+			const VxbVertexDesc vd = vxb_regular_vertex_desc_lite(s.tabVert[code * 12 + k], zm);
+			bool isNew = true;
+			if (!vd.atC7 && (vd.dir & mask) == vd.dir) // dir == 8 never passes: mask < 8
+			{
+				const int oc = c - (vd.dir & 1) - ((vd.dir >> 1) & 1) * 16 - ((vd.dir >> 2) & 1) * 256;
+				int ok = VXB_NO_SLOT; unsigned oa = 0;
+				if ((s.nt32[oc >> 5] >> (oc & 31)) & 1u)
+				{
+					oa = s.recA[vxb_rank_of(s.nt32, s.wpre, oc)];
+					ok = (oa >> (16 + 4 * vd.slot)) & 0xF;
+				}
+				if (ok != VXB_NO_SLOT) { if ((oa & 0xFF) == myMat) isNew = false; } // else: material split, new at its natural place
+				else if (vd.endpoint) quirkMask |= 1u << k;                            // :1633-1640 creates the vertex at v0
+			}
+			if (isNew) newMask |= 1u << k;
+		}
+		s.recB[i] = newMask | (quirkMask << 12) | ((unsigned)mask << 24);
+		s.vbase[i] = (unsigned short)__popc(newMask);
+		s.tbase[i] = (unsigned short)(geo & 0xF);
+	}
+	__syncthreads();
+
+	// ---- exclusive scans in serial cell order (contiguous chunk per thread) ----
+	const unsigned per = (ntc + VXB_THREADS - 1) / VXB_THREADS;
+	const unsigned i0 = min(tid * per, ntc), i1 = min(i0 + per, ntc);
+	unsigned sv = 0, st = 0;
+	for (unsigned i = i0; i < i1; ++i) { sv += s.vbase[i]; st += s.tbase[i]; }
+	unsigned total;
+	const unsigned base = vxb_block_scan(sv | (st << 16), s.warpSums, total);
+	nverts = total & 0xFFFF; ntris = total >> 16;
+	unsigned bv = base & 0xFFFF, bt = base >> 16;
+	for (unsigned i = i0; i < i1; ++i)
+	{
+		const unsigned cv = s.vbase[i], ct = s.tbase[i];
+		s.vbase[i] = (unsigned short)bv; s.tbase[i] = (unsigned short)bt;
+		bv += cv; bt += ct;
+	}
+}
+
+// the block's non-trivial bits and their prefix, read back by vxb_big_block_kernel and vxb_triangle_kernel
+__device__ __forceinline__ void vxb_save_nt(const VxbDev& d, unsigned emitIdx, const unsigned int* nt32, const unsigned int* wpre)
+{
+	const int tid = threadIdx.x;
+	if (tid < 128) { d.ntScratch[(size_t)emitIdx * 256 + tid] = nt32[tid]; d.ntScratch[(size_t)emitIdx * 256 + 128 + tid] = wpre[tid]; }
+}
+
+// one 16-byte record per cell + the vertex work list entries of its new vertices, for the flat kernels
+template <class Smem>
+__device__ __forceinline__ void vxb_write_cell_records(const Smem& s, const VxbDev& d, unsigned ntc, unsigned voff, unsigned cellBase, unsigned slot)
+{
+	for (unsigned i = threadIdx.x; i < ntc; i += VXB_THREADS)
+	{
+		const unsigned rb = s.recB[i];
+		VxbCellRec cr;
+		cr.a = (unsigned)s.list[i] | ((unsigned)s.cz[i] << 12) | ((rb >> 24) << 28);
+		cr.b = s.recA[i];
+		cr.c = rb & 0x00FFFFFFu;
+		cr.d = (unsigned)s.vbase[i] | ((unsigned)s.tbase[i] << 16);
+		*reinterpret_cast<uint4*>(&d.cellRecs[cellBase + i]) = *reinterpret_cast<const uint4*>(&cr);
+		d.cellBlock[cellBase + i] = slot;
+		unsigned nm = rb & 0xFFFu, j = voff + s.vbase[i];
+		while (nm) { const int k = __ffs(nm) - 1; nm &= nm - 1; d.vlist[j++] = ((cellBase + i) << 4) | (unsigned)k; }
+	}
+}
+
+// the block's record in directory slot `slot` (one thread); a mid-level block also joins the transition work list
+__device__ __forceinline__ void vxb_write_block_rec(const VxbDev& d, unsigned slot, int level, unsigned coordId, unsigned emitIdx,
+	unsigned voff, unsigned ioff, unsigned cellBase, unsigned ntc, unsigned nverts, unsigned ntris, unsigned removed)
+{
+	VxbBlockRec br;
+	br.packed = ((unsigned)level << 28) | coordId; br.emitIdx = emitIdx; br.voff = voff; br.ioff = ioff; br.cellBase = cellBase;
+	br.ntc = ntc; br.nverts = nverts; br.ntris = ntris; br.removed = removed;
+	for (int f = 0; f < 6; ++f) { br.tvoff[f] = 0; br.tioff[f] = 0; br.tvcount[f] = 0; br.ticount[f] = 0; }
+	br.pad[0] = br.pad[1] = br.pad[2] = 0;
+	d.blockRecs[slot] = br;
+	if (level > 0 && level != d.lastLevel && d.transitions) d.transList[atomicAdd(&d.counters->transBlocks, 1u)] = slot;
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(VXB_THREADS, VXB_OCC) vxb_block_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB, const VxbDev d, const int levelArg)
 {
 	constexpr int PITCH = (MODE == 0) ? VXB_DTILE_PITCH : VXB_TILE_PITCH;
 	constexpr int ROWS = (MODE == 0) ? 19 : 17;
-	typedef VxbBlockSmem<MODE, T> Smem;
+	typedef VxbBlockSmem<MODE> Smem;
 	constexpr int CAP_C = Smem::Caps::CAP, VL_CAP = Smem::Caps::VL, NBUF = Smem::Caps::NBUF;
-	static_assert(T == 128 || T == 256, "the per-word steps assume 128 or 256 threads");
 	extern __shared__ __align__(128) unsigned char smemRaw[];
 	Smem& s = *reinterpret_cast<Smem*>(smemRaw);
 	const int tid = threadIdx.x;
@@ -143,8 +278,8 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 	if (tid == 0) { vxb_mbar_init(&s.mbar[0], 1); vxb_mbar_init(&s.mbar[1], 1); }
 	if (tid < 16) s.hist[tid] = 0;
 	if (tid < 8) s.used[tid] = 0;
-	for (int i = tid; i < 256; i += T) { s.tabClass[i] = vxbGRegularCellClass[i]; s.tabCell[i] = vxbGRegularCellData[i]; }
-	for (int i = tid; i < 3072; i += T) s.tabVert[i] = vxbGRegularVertexData[i];
+	for (int i = tid; i < 256; i += VXB_THREADS) { s.tabClass[i] = vxbGRegularCellClass[i]; s.tabCell[i] = vxbGRegularCellData[i]; }
+	for (int i = tid; i < 3072; i += VXB_THREADS) s.tabVert[i] = vxbGRegularVertexData[i];
 	unsigned statNonTrivial = 0;
 
 	// ---- work source ----
@@ -303,7 +438,7 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 			if (bx == 0 || bx == nb - 1)
 			{
 				__syncthreads();
-				for (int i = tid; i < 19 * 19; i += T)
+				for (int i = tid; i < 19 * 19; i += VXB_THREADS)
 				{
 					signed char* r = tileRaw + i * VXB_DTILE_PITCH;
 					if (bx == 0) r[15] = r[16];
@@ -313,7 +448,7 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 			if (by == 0 || by == nb - 1)
 			{
 				__syncthreads();
-				for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += T)
+				for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += VXB_THREADS)
 				{
 					const int z = i / VXB_DTILE_PITCH, x = i % VXB_DTILE_PITCH;
 					signed char* p = tileRaw + z * 19 * VXB_DTILE_PITCH + x;
@@ -324,7 +459,7 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 			if (bz == 0 || bz == nb - 1)
 			{
 				__syncthreads();
-				for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += T)
+				for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += VXB_THREADS)
 				{
 					const int y = i / VXB_DTILE_PITCH, x = i % VXB_DTILE_PITCH;
 					signed char* p = tileRaw + y * VXB_DTILE_PITCH + x;
@@ -353,7 +488,7 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 		__syncthreads();
 		unsigned ntc;
 		{
-			const unsigned cnt = (tid < 128) ? __popc(s.nt32[tid]) : 0u; // T >= 128: one word per thread
+			const unsigned cnt = (tid < 128) ? __popc(s.nt32[tid]) : 0u; // one word per thread
 			const unsigned ex = vxb_block_scan(cnt, s.warpSums, ntc);
 			if (tid < 128) s.wpre[tid] = ex;
 		}
@@ -374,16 +509,7 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 				}
 			}
 			else if (!d.cacheValid[level][coordId]) vxb_init_cache_page(d, level, coordId);
-			if (inCap)
-			{
-				// ordered compact list: one cell row (z, y) = 16 bits at a time
-				for (int r = tid; r < 256; r += T)
-				{
-					unsigned bits = reinterpret_cast<const unsigned short*>(s.nt32)[r];
-					unsigned pos = s.wpre[r >> 1] + ((r & 1) ? __popc(s.nt32[r >> 1] & 0xFFFFu) : 0u);
-					while (bits) { const int x = __ffs(bits) - 1; bits &= bits - 1; s.list[pos++] = (unsigned short)(r * 16 + x); }
-				}
-			}
+			if (inCap) vxb_compact_cells(s.nt32, s.wpre, s.list);
 			__syncthreads();
 			if (tid == 0)
 			{
@@ -410,17 +536,17 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 					if (vote >= 0) d.cachePages[level][(size_t)coordId * 4096 + c] = (unsigned short)vote;
 				}
 			};
-			if (inCap) { if (level > 0) for (unsigned i = tid; i < ntc; i += T) cellWork(s.list[i]); } // level 0: the histogram is taken in pass A
+			if (inCap) { if (level > 0) for (unsigned i = tid; i < ntc; i += VXB_THREADS) cellWork(s.list[i]); } // level 0: the histogram is taken in pass A
 			else
 			{
-				for (int r = tid; r < 256; r += T)
+				for (int r = tid; r < 256; r += VXB_THREADS)
 				{
 					unsigned bits = reinterpret_cast<const unsigned short*>(s.nt32)[r];
 					while (bits) { const int x = __ffs(bits) - 1; bits &= bits - 1; cellWork(r * 16 + x); }
 				}
 			}
 			__syncthreads();
-			if (!inCap && emitMine && tid < 128) { d.ntScratch[(size_t)s.emitIdx * 256 + tid] = s.nt32[tid]; d.ntScratch[(size_t)s.emitIdx * 256 + 128 + tid] = s.wpre[tid]; }
+			if (!inCap && emitMine) vxb_save_nt(d, s.emitIdx, s.nt32, s.wpre);
 		}
 
 		// every cell of every transition face votes too, trivial ones included (:1859) - observable at the next level
@@ -444,7 +570,7 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 					__syncthreads();
 					if (tid == 0) { d.cacheValid[level][coordId] = 1; s.pageReady = 1; }
 				}
-				for (int fc = tid; fc < 256; fc += T)
+				for (int fc = tid; fc < 256; fc += VXB_THREADS)
 				{
 				const int row = fc >> 4, col = fc & 15;
 				// most face cells have no child with a material: test all six faces first (independent loads, all in flight
@@ -482,103 +608,19 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 
 		if (ntc > 0 && !inCap)
 		{
-			if (tid == 0 && emitMine) d.bigList[atomicAdd(&d.counters->bigCount[0], 1u)] = s.emitIdx;
+			if (tid == 0 && emitMine) d.bigList[atomicAdd(&d.counters->bigCount, 1u)] = s.emitIdx;
 		}
 		else if (ntc > 0 && emitMine)
 		{
-			// ---- pass A: material, case code, zero mask, owned slots ----
-			for (unsigned i = tid; i < ntc; i += T)
-			{
-				const int c = s.list[i];
-				signed char v[8];
-				vxb_tile_samples<PITCH, ROWS>(tile, c, v);
-				const unsigned code = vxb_case_code(v);
-				const unsigned zm = vxb_zero_mask(v);
-				unsigned matId, matBlend;
-				if (level == 0)
-				{
-					atomicAdd(&s.hist[s.tabClass[code]], 1u); // PerCaseCellsCount (:1574)
-					const size_t gi = ((size_t)((bz * 16 + (c >> 8))) * d.n + (by * 16 + ((c >> 4) & 15))) * d.n + (bx * 16 + (c & 15));
-					matId = g.mat[gi]; matBlend = g.blend[gi];
-				}
-				else
-				{
-					const unsigned e = d.cachePages[level][(size_t)coordId * 4096 + c]; // voted above
-					matId = e & 0xFF; matBlend = e >> 8;
-				}
-				unsigned slotK = 0xFFFFu;
-				const int nv = s.tabCell[s.tabClass[code] * 16] >> 4;
-				for (int k = 0; k < nv; ++k)
-				{
-					const VxbVertexDesc vd = vxb_regular_vertex_desc_lite(s.tabVert[code * 12 + k], zm);
-					const int sl = vxb_regular_owned_slot(vd);
-					if (sl >= 0) slotK = (slotK & ~(0xFu << (4 * sl))) | ((unsigned)k << (4 * sl));
-				}
-				s.cz[i] = (unsigned short)(code | (zm << 8));
-				s.recA[i] = matId | (matBlend << 8) | (slotK << 16);
-			}
-			__syncthreads();
-
-			// ---- pass B: new-vs-reuse decisions ----
-			for (unsigned i = tid; i < ntc; i += T)
-			{
-				const int c = s.list[i];
-				const unsigned code = s.cz[i] & 0xFF, zm = s.cz[i] >> 8;
-				const unsigned geo = s.tabCell[s.tabClass[code] * 16];
-				const unsigned rowStart = vxb_rank_of(s.nt32, s.wpre, c & ~15), sliceStart = s.wpre[(c >> 8) * 8];
-				const int mask = (i > rowStart ? 1 : 0) | (rowStart > sliceStart ? 2 : 0) | (sliceStart > 0 ? 4 : 0);
-				const unsigned myMat = s.recA[i] & 0xFF;
-				unsigned newMask = 0, quirkMask = 0;
-				for (int k = 0; k < (int)(geo >> 4); ++k)
-				{
-					// new-vs-reuse decision (:1610-1644) from the owner cell's record
-					const VxbVertexDesc vd = vxb_regular_vertex_desc_lite(s.tabVert[code * 12 + k], zm);
-					bool isNew = true;
-					if (!vd.atC7 && (vd.dir & mask) == vd.dir) // dir == 8 never passes: mask < 8
-					{
-						const int oc = c - (vd.dir & 1) - ((vd.dir >> 1) & 1) * 16 - ((vd.dir >> 2) & 1) * 256;
-						int ok = VXB_NO_SLOT; unsigned oa = 0;
-						if ((s.nt32[oc >> 5] >> (oc & 31)) & 1u)
-						{
-							oa = s.recA[vxb_rank_of(s.nt32, s.wpre, oc)];
-							ok = (oa >> (16 + 4 * vd.slot)) & 0xF;
-						}
-						if (ok != VXB_NO_SLOT) { if ((oa & 0xFF) == myMat) isNew = false; } // else: material split, new at its natural place
-						else if (vd.endpoint) quirkMask |= 1u << k;                            // :1633-1640 creates the vertex at v0
-					}
-					if (isNew) newMask |= 1u << k;
-				}
-				s.recB[i] = newMask | (quirkMask << 12) | ((unsigned)mask << 24);
-				s.vbase[i] = (unsigned short)__popc(newMask);
-				s.tbase[i] = (unsigned short)(geo & 0xF);
-			}
-			__syncthreads();
-
-			// ---- exclusive scans in serial cell order (contiguous chunk per thread) ----
 			unsigned nverts, ntris;
-			{
-				const unsigned per = (ntc + T - 1) / T;
-				const unsigned i0 = min(tid * per, ntc), i1 = min(i0 + per, ntc);
-				unsigned sv = 0, st = 0;
-				for (unsigned i = i0; i < i1; ++i) { sv += s.vbase[i]; st += s.tbase[i]; }
-				unsigned total;
-				const unsigned base = vxb_block_scan(sv | (st << 16), s.warpSums, total);
-				nverts = total & 0xFFFF; ntris = total >> 16;
-				unsigned bv = base & 0xFFFF, bt = base >> 16;
-				for (unsigned i = i0; i < i1; ++i)
-				{
-					const unsigned cv = s.vbase[i], ct = s.tbase[i];
-					s.vbase[i] = (unsigned short)bv; s.tbase[i] = (unsigned short)bt;
-					bv += cv; bt += ct;
-				}
-			}
+			vxb_decide_cells<PITCH, ROWS, true>(s, tile, d, level, coordId, bx, by, bz, ntc, nverts, ntris);
 			const bool inCta = MODE == 0 && nverts <= (unsigned)VL_CAP;
 			if (MODE == 0 && !inCta)
 			{
-				// too many vertices for the in-CTA path: hand the block to vxb_decide_kernel<4096, 1> + the flat kernels
+				// too many vertices for the in-CTA path: hand the block to vxb_big_block_kernel + the flat kernels
 				__syncthreads();
-				if (tid < 128) { d.ntScratch[(size_t)s.emitIdx * 256 + tid] = s.nt32[tid]; d.ntScratch[(size_t)s.emitIdx * 256 + 128 + tid] = s.wpre[tid]; }
-				if (tid == 0) d.bigList[atomicAdd(&d.counters->bigCount[0], 1u)] = s.emitIdx;
+				vxb_save_nt(d, s.emitIdx, s.nt32, s.wpre);
+				if (tid == 0) d.bigList[atomicAdd(&d.counters->bigCount, 1u)] = s.emitIdx;
 			}
 			else
 			{
@@ -593,25 +635,13 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 					&& (unsigned long long)cellBase + ntc <= d.ccap && slot < d.rcap;
 				if (fits && MODE != 0)
 				{
-					for (unsigned i = tid; i < ntc; i += T)
-					{
-						const unsigned rb = s.recB[i];
-						VxbCellRec cr;
-						cr.a = (unsigned)s.list[i] | ((unsigned)s.cz[i] << 12) | ((rb >> 24) << 28);
-						cr.b = s.recA[i];
-						cr.c = rb & 0x00FFFFFFu;
-						cr.d = (unsigned)s.vbase[i] | ((unsigned)s.tbase[i] << 16);
-						*reinterpret_cast<uint4*>(&d.cellRecs[cellBase + i]) = *reinterpret_cast<const uint4*>(&cr);
-						d.cellBlock[cellBase + i] = slot;
-						unsigned nm = rb & 0xFFFu, j = voff + s.vbase[i];
-						while (nm) { const int k = __ffs(nm) - 1; nm &= nm - 1; d.vlist[j++] = ((cellBase + i) << 4) | (unsigned)k; }
-					}
-					if (tid < 128) { d.ntScratch[(size_t)s.emitIdx * 256 + tid] = s.nt32[tid]; d.ntScratch[(size_t)s.emitIdx * 256 + 128 + tid] = s.wpre[tid]; }
+					vxb_write_cell_records(s, d, ntc, voff, cellBase, slot);
+					vxb_save_nt(d, s.emitIdx, s.nt32, s.wpre);
 				}
 				if (fits && MODE == 0)
 				{
 					// ---- the block's new vertices, one thread each (:1576-1726), from the halo tile ----
-					for (unsigned i = tid; i < ntc; i += T)
+					for (unsigned i = tid; i < ntc; i += VXB_THREADS)
 					{
 						unsigned nm = s.recB[i] & 0xFFFu, j = s.vbase[i];
 						while (nm) { const int k = __ffs(nm) - 1; nm &= nm - 1; s.vl[j++] = (unsigned short)((i << 4) | (unsigned)k); }
@@ -620,7 +650,7 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 					VxbTileView tv;
 					tv.dist = tileRaw; tv.ox = bx * 16; tv.oy = by * 16; tv.oz = bz * 16; tv.sx = hsx; tv.sy = hsy; tv.sz = hsz;
 					tv.mat = g.mat; tv.blend = g.blend; tv.n = d.n; // the two material / blend taps of a vertex stay global loads
-					for (unsigned j = tid; j < nverts; j += T)
+					for (unsigned j = tid; j < nverts; j += VXB_THREADS)
 					{
 						const unsigned e = s.vl[j];
 						const unsigned i = e >> 4; const int k = e & 15;
@@ -653,8 +683,10 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 					__syncthreads(); // the positions are read back by the degenerate test below
 					if (NBUF == 1 && nextItem < workCount) { int l2, x2, y2, z2; decode(nextItem, l2, x2, y2, z2); issue(0, l2, x2, y2, z2); nextIssued = true; } // the tile is not read any more
 					// ---- triangles, one thread per non-trivial cell (:1714-1726 + the degenerate filter of :1300-1321) ----
+					// (the step of vxb_triangle_kernel with the owner records in shared memory; one function shared by the two
+					// gives vxb_triangle_kernel a 40th register)
 					unsigned removed = 0;
-					for (unsigned i = tid; i < ntc; i += T)
+					for (unsigned i = tid; i < ntc; i += VXB_THREADS)
 					{
 						const int c = s.list[i];
 						const unsigned code = s.cz[i] & 0xFF, zm = s.cz[i] >> 8;
@@ -709,16 +741,7 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 					if (removed) atomicAdd(&s.removed, removed);
 					__syncthreads();
 				}
-				if (fits && tid == 0)
-				{
-					VxbBlockRec br;
-					br.packed = ((unsigned)level << 28) | coordId; br.emitIdx = s.emitIdx; br.voff = voff; br.ioff = ioff; br.cellBase = cellBase;
-					br.ntc = ntc; br.nverts = nverts; br.ntris = ntris; br.removed = (MODE == 0) ? s.removed : 0u;
-					for (int f = 0; f < 6; ++f) { br.tvoff[f] = 0; br.tioff[f] = 0; br.tvcount[f] = 0; br.ticount[f] = 0; }
-					br.pad[0] = br.pad[1] = br.pad[2] = 0;
-					d.blockRecs[slot] = br;
-					if (level > 0 && level != d.lastLevel && d.transitions) d.transList[atomicAdd(&d.counters->transBlocks, 1u)] = slot;
-				}
+				if (fits && tid == 0) vxb_write_block_rec(d, slot, level, coordId, s.emitIdx, voff, ioff, cellBase, ntc, nverts, ntris, (MODE == 0) ? s.removed : 0u);
 			}
 		}
 		if (AHEAD && tid == 0) s.ahead = ahead;
@@ -736,10 +759,11 @@ __global__ void __launch_bounds__(T, VXB_OCC) vxb_block_kernel(const __grid_cons
 }
 
 // ------------------------------------------------------------------------------------------------
-// decide: everything that needs the block as a unit (ordering, reuse, scans); no vertex math
+// vxb_big_block_kernel: the blocks vxb_block_kernel hands over in bigList (more than 1024 non-trivial cells, or a level-0
+// block with more than 2048 new vertices).  Reloads the block's tile and its non-trivial bits, runs the decide passes over
+// up to 4096 cells (every possible block) and writes cell records + the vertex work list for the flat kernels.
 // ------------------------------------------------------------------------------------------------
-template <int CAP_C>
-struct __align__(128) VxbDecideSmem
+struct __align__(128) VxbBigBlockSmem
 {
 	signed char tile[VXB_TILE_BYTES + 96];
 	unsigned int nt32[128];
@@ -750,57 +774,34 @@ struct __align__(128) VxbDecideSmem
 	unsigned int warpSums[8];
 	unsigned long long mbar;
 	unsigned int item, voff, ioff, cellBase, slot;
-	unsigned int levelEnd[VXB_MAX_LEVELS + 1];
-	unsigned int recA[CAP_C];     // matId | matBlend<<8 | slotK<<16
-	unsigned int recB[CAP_C];     // newMask | quirkMask<<12 | reuse mask << 24
-	unsigned short list[CAP_C];   // compact index -> cell id
-	unsigned short cz[CAP_C];     // case code | zero mask << 8
-	unsigned short vbase[CAP_C];  // exclusive scan of new-vertex counts
-	unsigned short tbase[CAP_C];  // exclusive scan of triangle counts
+	unsigned int recA[4096];     // matId | matBlend<<8 | slotK<<16
+	unsigned int recB[4096];     // newMask | quirkMask<<12 | reuse mask << 24
+	unsigned short list[4096];   // compact index -> cell id
+	unsigned short cz[4096];     // case code | zero mask << 8
+	unsigned short vbase[4096];  // exclusive scan of new-vertex counts
+	unsigned short tbase[4096];  // exclusive scan of triangle counts
 };
 
-// TIER 0: items come from the emit list (all levels, top level first); blocks with > CAP_C cells go to bigList.
-// TIER 1: items come from bigList (CAP_C = 4096 = every possible block).
-// group 0 = level 0 only, group 1 = levels >= 1, group 2 = all levels (single-stream runs)
-template <int CAP_C, int TIER>
-__global__ void __launch_bounds__(VXB_THREADS, (CAP_C <= 1024 ? VXB_OCC : 2)) vxb_decide_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap1, const VxbDev d, const int group)
+__global__ void __launch_bounds__(VXB_THREADS, 2) vxb_big_block_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap1, const VxbDev d)
 {
-	const int levelLo = (group == 1) ? 1 : 0, levelHi = (group == 0) ? 0 : d.levels - 1, g2 = group & 1;
-	const int levelCount = levelHi - levelLo + 1;
-	typedef VxbDecideSmem<CAP_C> Smem;
 	extern __shared__ __align__(128) unsigned char smemRaw[];
-	Smem& s = *reinterpret_cast<Smem*>(smemRaw);
+	VxbBigBlockSmem& s = *reinterpret_cast<VxbBigBlockSmem*>(smemRaw);
 	const int tid = threadIdx.x;
-	const VxbGrid g = d.grid;
 	unsigned phase = 0;
 
-	if (tid == 0)
-	{
-		vxb_mbar_init(&s.mbar, 1);
-		unsigned acc = 0; // work id -> level: the top level first (its blocks are the largest)
-		for (int l = levelHi; l >= levelLo; --l) { acc += d.counters->emitCount[l]; s.levelEnd[levelHi - l] = acc; }
-	}
+	if (tid == 0) vxb_mbar_init(&s.mbar, 1);
 	for (int i = tid; i < 256; i += VXB_THREADS) { s.tabClass[i] = vxbGRegularCellClass[i]; s.tabCell[i] = vxbGRegularCellData[i]; }
 	for (int i = tid; i < 3072; i += VXB_THREADS) s.tabVert[i] = vxbGRegularVertexData[i];
 	__syncthreads();
-	const unsigned workCount = (TIER == 0) ? s.levelEnd[levelCount - 1] : d.counters->bigCount[g2];
-	unsigned int* const bigList = d.bigList + (g2 ? d.workBase[1] : 0u); // group 1's rejects live behind level 0's segment
+	const unsigned workCount = d.counters->bigCount;
 
 	for (;;)
 	{
-		if (tid == 0) s.item = atomicAdd(TIER == 0 ? &d.counters->emitCursor[g2] : &d.counters->bigCursor[g2], 1u);
+		if (tid == 0) s.item = atomicAdd(&d.counters->bigCursor, 1u);
 		__syncthreads();
 		const unsigned item = s.item;
 		if (item >= workCount) break;
-		unsigned emitIdx;
-		if (TIER == 0)
-		{
-			int q = 0;
-			while (item >= s.levelEnd[q]) ++q;
-			const int lv = levelHi - q;
-			emitIdx = d.workBase[lv] + (item - (q ? s.levelEnd[q - 1] : 0u));
-		}
-		else emitIdx = bigList[item];
+		const unsigned emitIdx = d.bigList[item];
 		const unsigned packed = d.emitList[emitIdx];
 		const int level = (int)(packed >> 28);
 		const unsigned coordId = packed & 0x0FFFFFFFu;
@@ -810,107 +811,12 @@ __global__ void __launch_bounds__(VXB_THREADS, (CAP_C <= 1024 ? VXB_OCC : 2)) vx
 		if (tid < 128) { s.nt32[tid] = d.ntScratch[(size_t)emitIdx * 256 + tid]; s.wpre[tid] = d.ntScratch[(size_t)emitIdx * 256 + 128 + tid]; }
 		__syncthreads();
 		const unsigned ntc = s.wpre[127] + __popc(s.nt32[127]);
-		if (ntc > (unsigned)CAP_C)
-		{
-			if (tid == 0) bigList[atomicAdd(&d.counters->bigCount[g2], 1u)] = emitIdx; // only reachable in TIER 0
-			__syncthreads();
-			continue;
-		}
 		vxb_tile_issue(s.tile, &s.mbar, &tmap, &tmap1, d, level, bx, by, bz);
 		vxb_tile_complete(s.tile, &s.mbar, phase, d, level, bx, by, bz);
-		// ordered compact list of the non-trivial cells: thread = cell row (z, y), 16 bits each
-		{
-			unsigned bits = reinterpret_cast<const unsigned short*>(s.nt32)[tid];
-			unsigned pos = s.wpre[tid >> 1] + ((tid & 1) ? __popc(s.nt32[tid >> 1] & 0xFFFFu) : 0u);
-			while (bits) { const int x = __ffs(bits) - 1; bits &= bits - 1; s.list[pos++] = (unsigned short)(tid * 16 + x); }
-		}
+		vxb_compact_cells(s.nt32, s.wpre, s.list);
 		__syncthreads();
-
-		// ---- pass A: material, case code, zero mask, owned slots ----
-		for (unsigned i = tid; i < ntc; i += VXB_THREADS)
-		{
-			const int c = s.list[i];
-			signed char v[8];
-			vxb_tile_samples<VXB_TILE_PITCH, 17>(s.tile, c, v);
-			const unsigned code = vxb_case_code(v);
-			const unsigned zm = vxb_zero_mask(v);
-			unsigned matId, matBlend;
-			if (level == 0)
-			{
-				const size_t gi = ((size_t)((bz * 16 + (c >> 8))) * d.n + (by * 16 + ((c >> 4) & 15))) * d.n + (bx * 16 + (c & 15));
-				matId = g.mat[gi]; matBlend = g.blend[gi];
-			}
-			else
-			{
-				const unsigned e = d.cachePages[level][(size_t)coordId * 4096 + c]; // written by vxb_classify_kernel
-				matId = e & 0xFF; matBlend = e >> 8;
-			}
-			unsigned slotK = 0xFFFFu;
-			const int nv = s.tabCell[s.tabClass[code] * 16] >> 4;
-			for (int k = 0; k < nv; ++k)
-			{
-				const VxbVertexDesc vd = vxb_regular_vertex_desc_lite(s.tabVert[code * 12 + k], zm);
-				const int sl = vxb_regular_owned_slot(vd);
-				if (sl >= 0) slotK = (slotK & ~(0xFu << (4 * sl))) | ((unsigned)k << (4 * sl));
-			}
-			s.cz[i] = (unsigned short)(code | (zm << 8));
-			s.recA[i] = matId | (matBlend << 8) | (slotK << 16);
-		}
-		__syncthreads();
-
-		// ---- pass B: new-vs-reuse decisions ----
-		for (unsigned i = tid; i < ntc; i += VXB_THREADS)
-		{
-			const int c = s.list[i];
-			const unsigned code = s.cz[i] & 0xFF, zm = s.cz[i] >> 8;
-			const unsigned geo = s.tabCell[s.tabClass[code] * 16];
-			const unsigned rowStart = vxb_rank_of(s.nt32, s.wpre, c & ~15), sliceStart = s.wpre[(c >> 8) * 8];
-			const int mask = (i > rowStart ? 1 : 0) | (rowStart > sliceStart ? 2 : 0) | (sliceStart > 0 ? 4 : 0);
-			const unsigned myMat = s.recA[i] & 0xFF;
-			unsigned newMask = 0, quirkMask = 0;
-			for (int k = 0; k < (int)(geo >> 4); ++k)
-			{
-				// new-vs-reuse decision (:1610-1644) from the owner cell's record
-				const VxbVertexDesc vd = vxb_regular_vertex_desc_lite(s.tabVert[code * 12 + k], zm);
-				bool isNew = true;
-				if (!vd.atC7 && (vd.dir & mask) == vd.dir) // dir == 8 never passes: mask < 8
-				{
-					const int oc = c - (vd.dir & 1) - ((vd.dir >> 1) & 1) * 16 - ((vd.dir >> 2) & 1) * 256;
-					int ok = VXB_NO_SLOT; unsigned oa = 0;
-					if ((s.nt32[oc >> 5] >> (oc & 31)) & 1u)
-					{
-						oa = s.recA[vxb_rank_of(s.nt32, s.wpre, oc)];
-						ok = (oa >> (16 + 4 * vd.slot)) & 0xF;
-					}
-					if (ok != VXB_NO_SLOT) { if ((oa & 0xFF) == myMat) isNew = false; } // else: material split, new at its natural place
-					else if (vd.endpoint) quirkMask |= 1u << k;                            // :1633-1640 creates the vertex at v0
-				}
-				if (isNew) newMask |= 1u << k;
-			}
-			s.recB[i] = newMask | (quirkMask << 12) | ((unsigned)mask << 24);
-			s.vbase[i] = (unsigned short)__popc(newMask);
-			s.tbase[i] = (unsigned short)(geo & 0xF);
-		}
-		__syncthreads();
-
-		// ---- exclusive scans in serial cell order (contiguous chunk per thread) ----
 		unsigned nverts, ntris;
-		{
-			const unsigned per = (ntc + VXB_THREADS - 1) / VXB_THREADS;
-			const unsigned i0 = min(tid * per, ntc), i1 = min(i0 + per, ntc);
-			unsigned sv = 0, st = 0;
-			for (unsigned i = i0; i < i1; ++i) { sv += s.vbase[i]; st += s.tbase[i]; }
-			unsigned total;
-			const unsigned base = vxb_block_scan(sv | (st << 16), s.warpSums, total);
-			nverts = total & 0xFFFF; ntris = total >> 16;
-			unsigned bv = base & 0xFFFF, bt = base >> 16;
-			for (unsigned i = i0; i < i1; ++i)
-			{
-				const unsigned cv = s.vbase[i], ct = s.tbase[i];
-				s.vbase[i] = (unsigned short)bv; s.tbase[i] = (unsigned short)bt;
-				bv += cv; bt += ct;
-			}
-		}
+		vxb_decide_cells<VXB_TILE_PITCH, 17, false>(s, s.tile, d, level, coordId, bx, by, bz, ntc, nverts, ntris);
 		if (tid == 0)
 		{
 			s.voff = atomicAdd(&d.counters->vertices, nverts);
@@ -924,45 +830,24 @@ __global__ void __launch_bounds__(VXB_THREADS, (CAP_C <= 1024 ? VXB_OCC : 2)) vx
 			&& (unsigned long long)cellBase + ntc <= d.ccap && slot < d.rcap;
 		if (fits)
 		{
-			for (unsigned i = tid; i < ntc; i += VXB_THREADS)
-			{
-				const unsigned rb = s.recB[i];
-				VxbCellRec cr;
-				cr.a = (unsigned)s.list[i] | ((unsigned)s.cz[i] << 12) | ((rb >> 24) << 28);
-				cr.b = s.recA[i];
-				cr.c = rb & 0x00FFFFFFu;
-				cr.d = (unsigned)s.vbase[i] | ((unsigned)s.tbase[i] << 16);
-				*reinterpret_cast<uint4*>(&d.cellRecs[cellBase + i]) = *reinterpret_cast<const uint4*>(&cr);
-				d.cellBlock[cellBase + i] = slot;
-				unsigned nm = rb & 0xFFFu, j = voff + s.vbase[i];
-				while (nm) { const int k = __ffs(nm) - 1; nm &= nm - 1; d.vlist[j++] = ((cellBase + i) << 4) | (unsigned)k; }
-			}
-			if (tid == 0)
-			{
-				VxbBlockRec br;
-				br.packed = packed; br.emitIdx = emitIdx; br.voff = voff; br.ioff = ioff; br.cellBase = cellBase;
-				br.ntc = ntc; br.nverts = nverts; br.ntris = ntris; br.removed = 0;
-				for (int f = 0; f < 6; ++f) { br.tvoff[f] = 0; br.tioff[f] = 0; br.tvcount[f] = 0; br.ticount[f] = 0; }
-				br.pad[0] = br.pad[1] = br.pad[2] = 0;
-				d.blockRecs[slot] = br;
-				if (level > 0 && level != d.lastLevel && d.transitions) d.transList[atomicAdd(&d.counters->transBlocks, 1u)] = slot;
-			}
+			vxb_write_cell_records(s, d, ntc, voff, cellBase, slot);
+			if (tid == 0) vxb_write_block_rec(d, slot, level, coordId, emitIdx, voff, ioff, cellBase, ntc, nverts, ntris, 0u);
 		}
 		__syncthreads();
 	}
 }
 
 // ------------------------------------------------------------------------------------------------
-// flat kernels.  part 0 = [0, split) (group 0), part 1 = [split, total) (group 1), part 2 = everything
+// flat kernels over the blocks with cell records (levels >= 1 and the level-0 blocks of vxb_big_block_kernel): their
+// vertices and cells lie behind the split vxb_mark_split_kernel takes once vxb_block_kernel<0> is done
 // ------------------------------------------------------------------------------------------------
 __global__ void vxb_mark_split_kernel(const VxbDev d)
 {
 	d.counters->splitVertices = d.counters->vertices;
 	d.counters->splitCells = d.counters->cells;
-	d.counters->splitRecords = d.counters->records;
 }
 
-__global__ void __launch_bounds__(VXB_THREADS, VXB_FLAT_OCC) vxb_vertex_kernel(const VxbDev d, const int part)
+__global__ void __launch_bounds__(VXB_THREADS, VXB_FLAT_OCC) vxb_vertex_kernel(const VxbDev d)
 {
 	__shared__ unsigned sUsed[8];
 	if (threadIdx.x < 8) sUsed[threadIdx.x] = 0;
@@ -970,9 +855,8 @@ __global__ void __launch_bounds__(VXB_THREADS, VXB_FLAT_OCC) vxb_vertex_kernel(c
 	if (!vxb_overflowed(d))
 	{
 		const VxbGrid g = d.grid;
-		const unsigned begin = (part == 1) ? d.counters->splitVertices : 0u;
-		const unsigned total = (part == 0) ? d.counters->splitVertices : d.counters->vertices;
-		for (unsigned j = begin + blockIdx.x * blockDim.x + threadIdx.x; j < total; j += gridDim.x * blockDim.x)
+		const unsigned total = d.counters->vertices;
+		for (unsigned j = d.counters->splitVertices + blockIdx.x * blockDim.x + threadIdx.x; j < total; j += gridDim.x * blockDim.x)
 		{
 			const unsigned e = d.vlist[j];
 			const unsigned ci = e >> 4; const int k = e & 15;
@@ -1014,12 +898,11 @@ __global__ void __launch_bounds__(VXB_THREADS, VXB_FLAT_OCC) vxb_vertex_kernel(c
 	if (threadIdx.x < 8 && sUsed[threadIdx.x]) atomicOr(&d.counters->usedMaterials[threadIdx.x], sUsed[threadIdx.x]);
 }
 
-__global__ void __launch_bounds__(VXB_THREADS) vxb_triangle_kernel(const VxbDev d, const int part)
+__global__ void __launch_bounds__(VXB_THREADS) vxb_triangle_kernel(const VxbDev d)
 {
 	if (vxb_overflowed(d)) return;
-	const unsigned begin = (part == 1) ? d.counters->splitCells : 0u;
-	const unsigned total = (part == 0) ? d.counters->splitCells : d.counters->cells;
-	for (unsigned ci = begin + blockIdx.x * blockDim.x + threadIdx.x; ci < total; ci += gridDim.x * blockDim.x)
+	const unsigned total = d.counters->cells;
+	for (unsigned ci = d.counters->splitCells + blockIdx.x * blockDim.x + threadIdx.x; ci < total; ci += gridDim.x * blockDim.x)
 	{
 		const uint4 crv = *reinterpret_cast<const uint4*>(&d.cellRecs[ci]);
 		const unsigned slot = d.cellBlock[ci];
@@ -1029,11 +912,10 @@ __global__ void __launch_bounds__(VXB_THREADS) vxb_triangle_kernel(const VxbDev 
 		const unsigned int* wpre = nt32 + 128;
 		const int c = crv.x & 0xFFF;
 		const unsigned code = (crv.x >> 12) & 0xFF, zm = (crv.x >> 20) & 0xFF;
-		const int mask = (int)(crv.x >> 28);
 		const unsigned cls = vxbGRegularCellClass[code];
 		const unsigned char* cd = &vxbGRegularCellData[cls * 16];
 		const unsigned geo = cd[0];
-		const unsigned myMat = crv.y & 0xFF, newMask = crv.z & 0xFFF;
+		const unsigned newMask = crv.z & 0xFFF;
 		// block-local vertex ids (< 49152) as 16-bit halves of six registers: a table-indexed array would live in local memory
 		unsigned w[6] = { 0u, 0u, 0u, 0u, 0u, 0u };
 		unsigned nextNew = crv.w & 0xFFFF;
@@ -1062,7 +944,6 @@ __global__ void __launch_bounds__(VXB_THREADS) vxb_triangle_kernel(const VxbDev 
 			const unsigned pair = i == 0 ? w[0] : i == 1 ? w[1] : i == 2 ? w[2] : i == 3 ? w[3] : i == 4 ? w[4] : w[5];
 			return (k & 1u) ? (pair >> 16) : (pair & 0xFFFFu);
 		};
-		(void)mask; (void)myMat;
 		unsigned* out = d.idx + ioff + (crv.w >> 16) * 3;
 		unsigned removed = 0;
 		// A level-0 cell without a zero sample has every table vertex strictly inside a distinct cell edge (t in 1..255):

@@ -6,13 +6,10 @@
 //                            (VoxelGrid::CompressBlock's BF_Empty rule, VoxelGrid.cpp:610-672).
 //   vxb_block_info_kernel    turns the raw flags into BF_Empty / sign-mix bits (exact slow path when
 //                            the run-count bound is inconclusive).
-//   per LOD level:
-//     vxb_select_kernel      block walk (GenerateBlockListForLevel :385-466 + AreBlockAndNeighborsEmpty
+//   vxb_select_kernel        per LOD level, the block walk (GenerateBlockListForLevel :385-466 + AreBlockAndNeighborsEmpty
 //                            :1511-1527): appends the blocks that can produce output or side effects.
-//     vxb_classify_kernel    (vxb_emit.cuh) tiles, case codes, material votes - the only cross-level dependency.
-//   then, once for all levels (vxb_emit.cuh): vxb_decide_kernel, vxb_vertex_kernel, vxb_triangle_kernel,
-//   vxb_transition_kernel, vxb_finish_kernel (PolygonizeBlock :1529-1750, GenerateTransitionCells :1754-2131,
-//   PushBlocksToResult :1266-1428).
+//   then the per-block and flat kernels of vxb_emit.cuh (PolygonizeBlock :1529-1750, GenerateTransitionCells :1754-2131,
+//   PushBlocksToResult :1266-1428).  Launch order and costs: DESIGN.md §4.
 #pragma once
 
 #define VXB_MAX_LEVELS 12
@@ -38,17 +35,16 @@ struct VxbCounters
 	unsigned int usedMaterials[8];
 	unsigned int workCount[VXB_MAX_LEVELS];
 	unsigned int workCursor[VXB_MAX_LEVELS];
-	unsigned int emitCount[VXB_MAX_LEVELS]; // blocks with non-trivial cells, per level (vxb_classify_kernel)
-	unsigned int emitCursor[2];             // per group: 0 = level 0, 1 = levels >= 1 (the groups run on two streams)
-	unsigned int bigCount[2], bigCursor[2]; // blocks with > 1024 non-trivial cells (second tier of vxb_decide_kernel)
+	unsigned int emitCount[VXB_MAX_LEVELS]; // emitted blocks (blocks with non-trivial cells), per level (vxb_block_kernel)
+	unsigned int bigCount, bigCursor;       // bigList: blocks for vxb_big_block_kernel
 	unsigned int cells;                     // cursor of the cell-record arena
-	unsigned int splitVertices, splitCells, splitRecords; // cursors after group 0 (level 0): later kernels split their ranges there
+	unsigned int splitVertices, splitCells; // cursors after level 0: the flat kernels work behind them
 	unsigned int transBlocks, transCursor;  // emitted mid-level blocks (vxb_transition_kernel work list)
 	unsigned int finishCursor;
 	unsigned int coarseCursor;              // item cursor of the single launch that handles the coarse levels
 };
 
-// One non-trivial cell of an emitted block (written by vxb_decide_kernel, read by the flat kernels)
+// One non-trivial cell of an emitted block (written by vxb_block_kernel<1|2> and vxb_big_block_kernel, read by the flat kernels)
 struct VxbCellRec
 {
 	unsigned int a; // cell id (0..4095) | case code << 12 | zero mask << 20 | reuse mask << 28
@@ -996,8 +992,6 @@ __device__ __forceinline__ int vxb_vote_cell(const VxbVoteSource d, const int bx
 	if (!bestCount) return -1;
 	return (int)(bestId | (((bestBlend / (unsigned)bestCount) & 0xFFu) << 8));
 }
-
-struct VxbDecision { bool isNew, quirkV0; unsigned ownerIdx; int ok; };
 
 // Block id as the reference assigns it: full run = running counter over levels in z,y,x order (:395-401);
 // incremental run = continuation of that counter over the level's dirty box (:456-464)
