@@ -313,6 +313,13 @@ void vxb_host_free(void* p);
  * automatically on overflow; this only avoids the retry. */
 int vxb_set_capacity(vxb_context* ctx, uint64_t vertices, uint64_t indices, uint64_t trans_vertices, uint64_t trans_indices);
 
+/* Test hook: caps the grid of the persistent kernels (vxb_block_kernel<0|1|2>, vxb_big_block_kernel,
+ * vxb_transition_kernel and the flat vertex / triangle kernels) at `ctas` CTAs; 0 = the occupancy-sized grid (the
+ * default).  The cap only ever lowers a grid, so every CTA of a launch stays resident, as the coarse levels' waits
+ * for their children need.  With a few CTAs each one walks many work items, so small grids exercise the code that
+ * runs only from a CTA's second item on.  The output does not depend on it. */
+int vxb_set_launch_limit(vxb_context* ctx, uint32_t ctas);
+
 /* Per-kernel device time of the last vxb_polygonize run with VXB_FLAG_KERNEL_TIMES, for bench.py's roofline line:
  * which = 0: vxb_scan_kernel (streams the level-0 distance volume once), 1: block info, sign-mix pyramid + selection kernels,
  * 2: vxb_block_kernel<1>/<2> (levels >= 1: classification, votes, decisions) + vxb_big_block_kernel, 3: vxb_block_kernel<0>

@@ -31,11 +31,13 @@ SMALL = {
     "noise32": lambda: gridgen.noise_full(32),
     "noise16": lambda: gridgen.noise_full(16, seed=2),
     "positive_noise32": lambda: gridgen.noise_full(32, seed=4, lo=1, hi=4),
+    "patchwork64": lambda: gridgen.patchwork(64),
 }
 MEDIUM = {
     "hostile128": lambda: gridgen.hostile(128, seed=11),
     "sphere128": lambda: sphere(128),
     "noise64": lambda: gridgen.noise_full(64, seed=9, lo=-3, hi=2),
+    "patchwork128": lambda: gridgen.patchwork(128),
 }
 
 
@@ -47,4 +49,18 @@ def _terrain(n):
 # the benchmark's terrain at a size the golden digests can cover (generated on the host: the same bytes everywhere)
 LARGE = {
     "terrain256": lambda: _terrain(256),
+    "patchwork256": lambda: gridgen.patchwork(256),
 }
+
+# only against the live reference (tests/test_gpu_paths.py): too large for the CPU tests
+HUGE = {
+    "patchwork512": lambda: gridgen.patchwork(512),
+    "patchwork1024": lambda: gridgen.patchwork(1024),
+}
+
+
+def by_name(name):
+    for table in (SMALL, MEDIUM, LARGE, HUGE):
+        if name in table:
+            return table[name]()
+    raise KeyError(name)

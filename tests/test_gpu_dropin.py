@@ -82,23 +82,32 @@ def _edit_sequence(n, count, seed=42):
     return edits
 
 
-@pytest.mark.parametrize("name,n,count", [("hostile", 64, 12), ("terrain", 128, 20)])
+def _edge_edit_sequence(n, count):
+    """Sphere edits whose boxes touch the grid's faces, edges and corners (tests/gridgen.edge_edit_sequence)."""
+    import gridgen
+    return [(pos, r, ext, harness.IT_ADD if add else harness.IT_SUBTRACT) for pos, r, ext, add in gridgen.edge_edit_sequence(n, count)]
+
+
+@pytest.mark.parametrize("name,n,count", [("hostile", 64, 12), ("terrain", 128, 20), ("patchwork", 128, 18)])
 def test_incremental_edits_match_reference(reference, dropin, name, n, count):
     """Execute(grid, materials, modification) after Grid::InjectSurface: the drop-in must follow the reference's
     INCREMENTAL behaviour (stale consistency bits, vote-only cache overwrites, id continuation, erase + append order),
-    which is not the same as a fresh polygonization (SURVEY.md 8 a9)."""
+    which is not the same as a fresh polygonization (SURVEY.md 8 a9).  The patchwork case edits at the grid's edges."""
+    import gridgen
     if name == "hostile":
-        import gridgen
         dist, mat, blend = gridgen.hostile(n, seed=3)
+    elif name == "patchwork":
+        dist, mat, blend = gridgen.patchwork(n)
     else:
         from voxels_b200 import synth
         dist, mat, blend = (t.numpy() for t in synth.terrain(n))
+    edits = _edge_edit_sequence(n, count) if name == "patchwork" else _edit_sequence(n, count)
     state = []
     for lib in (reference, dropin):
         g = lib.grid_from_dense(dist, mat, blend)
         s, _ = lib.polygonize(g)
         state.append([lib, g, s, lib.modification_create()])
-    for step, (pos, radius, extent, kind) in enumerate(_edit_sequence(n, count)):
+    for step, (pos, radius, extent, kind) in enumerate(edits):
         dumps = []
         for st in state:
             lib, g, s, mod = st

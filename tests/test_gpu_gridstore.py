@@ -128,24 +128,57 @@ def test_pack_equals_reference_pack_for_save(reference, gpu_context, name):
 def test_device_edits_then_incremental_polygonize_match_reference(reference, gpu_context):
     """BASELINE configs[4] without the host round trip: edits on the device grid + vxb_polygonize_region, compared with the
     reference's InjectSurface + incremental Execute after every edit (blocks re-created per dirty box, ids, geometry)."""
+    _device_edits_case(reference, gpu_context, "terrain", 0)
+
+
+def test_device_edge_edits_few_ctas_match_reference(reference, gpu_context):
+    """The same on patchwork128, with edits at the grid's faces, edges and corners (the clipped dirty ranges and the
+    ranged decode of the coarse levels at the edge) and the persistent kernels capped at 2 CTAs."""
+    _device_edits_case(reference, gpu_context, "patchwork", 2)
+
+
+def _device_edits_case(reference, gpu_context, name, limit):
+    import gridgen
     n = 128
-    s = capi.Surface.terrain(n)
-    g = reference.grid_create_builtin(n, s)
-    surf, _ = reference.polygonize(g)
-    mod = reference.modification_create()
     ctx = gpu_context
     ctx.set_materials(None, None)
-    ctx.fill(n, s)
+    if name == "terrain":
+        s = capi.Surface.terrain(n)
+        g = reference.grid_create_builtin(n, s)
+        ctx.fill(n, s)
+    else:
+        dist, mat, blend = gridgen.patchwork(n)
+        g = reference.grid_from_dense(dist, mat, blend)
+        ctx.upload_dense(dist, mat, blend)
+    surf, _ = reference.polygonize(g)
+    mod = reference.modification_create()
+    ctx.set_launch_limit(limit)
+    try:
+        _edit_run(reference, ctx, g, surf, mod, name, n)
+    finally:
+        ctx.set_launch_limit(0)
+
+
+def _edit_run(reference, ctx, g, surf, mod, name, n):
+    import gridgen
     ctx.polygonize()
-    dist0 = reference.grid_to_dense(g)[0]
-    rng = np.random.RandomState(3)
     edits = []
-    while len(edits) < 25:
-        x, y, z = (int(v) for v in rng.randint(16, n - 16, size=3))
-        if abs(int(dist0[z, y, x])) >= 4:
-            continue
-        r = float(rng.choice([4, 6, 8]))
-        edits.append((np.array([x, y, z], np.float32), np.full(3, 2 * r + 4, np.float32), capi.Surface.sphere((0, 0, 0), r), 0 if len(edits) % 2 == 0 else 2))
+    if name == "terrain":
+        dist0 = reference.grid_to_dense(g)[0]
+        rng = np.random.RandomState(3)
+        while len(edits) < 25:
+            x, y, z = (int(v) for v in rng.randint(16, n - 16, size=3))
+            if abs(int(dist0[z, y, x])) >= 4:
+                continue
+            r = float(rng.choice([4, 6, 8]))
+            edits.append((np.array([x, y, z], np.float32), np.full(3, 2 * r + 4, np.float32), capi.Surface.sphere((0, 0, 0), r), 0 if len(edits) % 2 == 0 else 2))
+    else:
+        for pos, r, ext, add in gridgen.edge_edit_sequence(n, 18):
+            edits.append((np.array(pos, np.float32), np.full(3, ext, np.float32), capi.Surface.sphere((0, 0, 0), r), 0 if add else 2))
+    _device_edits(reference, ctx, g, surf, mod, edits)
+
+
+def _device_edits(reference, ctx, g, surf, mod, edits):
     for i, (pos, ext, sph, kind) in enumerate(edits):
         box = reference.grid_inject_builtin(g, pos, ext, sph, kind)
         s2, _ = reference.polygonize(g, modification=mod, surface=surf, box=box)

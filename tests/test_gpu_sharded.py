@@ -70,10 +70,11 @@ def assert_same(a, b, levels):
 
 
 @pytest.mark.parametrize("name,world,group", [("hostile128", 2, 0), ("hostile128", 4, 32), ("hostile128", 2, 32), ("sphere128", 2, 0),
-                                              ("noise64", 2, 0), ("hostile64", 2, 0), ("hostile128", 1, 0), ("sphere128", 4, 0)])
+                                              ("noise64", 2, 0), ("hostile64", 2, 0), ("hostile128", 1, 0), ("sphere128", 4, 0),
+                                              ("patchwork256", 4, 32), ("patchwork256", 8, 0)])
 def test_virtual_ranks_equal_single_run(gpu_context, name, world, group):
     import voxels_b200
-    dist, mat, blend = (grids.MEDIUM.get(name) or grids.SMALL[name])()
+    dist, mat, blend = grids.by_name(name)
     n = dist.shape[0]
     gpu_context.set_materials(None, None)
     gpu_context.upload_dense(dist, mat, blend)

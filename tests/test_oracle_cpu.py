@@ -87,3 +87,21 @@ def test_terrain_generator_is_deterministic_and_parity_on_it(reference, restatem
     for l in range(reference.surface_levels(s)):
         assert not compare.level_diff(reference.surface_level(s, l), restatement.level(h, l), "L%d" % l)
     reference.surface_destroy(s); reference.grid_destroy(g); restatement.destroy(h)
+
+
+def test_skip_quirk_level0_and_statistics(reference, restatement):
+    """Level-0 blocks skipped with their BF_Empty neighbourhood although the surface runs along their faces (:520).  The
+    coarse cells over them read an uninitialised Cell::Material in the reference (:1052-1086; the texture bytes of their
+    vertices change with the thread count), which this project defines as {EMPTY, 0}; level 0 and the statistics are
+    defined and must match."""
+    import gridgen
+    dist, mat, blend = gridgen.skip_quirk()
+    g = reference.grid_from_dense(dist, mat, blend)
+    s, _ = reference.polygonize(g, threads=4)
+    h = restatement.run(dist, mat, blend)
+    assert np.array_equal(reference.grid_empty_flags(g), restatement.empty_flags(h, dist.shape[0]))
+    assert np.array_equal(reference.surface_stats(s), restatement.stats(h))
+    assert reference.surface_levels(s) == restatement.levels(h)
+    assert not compare.level_diff(reference.surface_level(s, 0), restatement.level(h, 0), "L0")
+    assert len(reference.surface_level(s, 1).rows) > 0      # the coarse levels do have a surface over the skipped blocks
+    reference.surface_destroy(s); reference.grid_destroy(g); restatement.destroy(h)

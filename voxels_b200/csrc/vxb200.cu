@@ -115,6 +115,8 @@ struct vxb_context
 	uint8_t* latticePtr = nullptr;  // lattice1.p, or the cube's fourth channel
 	bool haveLattice1 = false, latticeOff = false;
 	int gridBlock[3] = { 0, 0, 0 }, gridBigBlock = 0, gridTransition = 0;
+	uint32_t launchLimit = 0;      // vxb_set_launch_limit: cap on the persistent kernels' grids (0 = none)
+	unsigned persistentGrid(int grid) const { return launchLimit ? std::min<unsigned>((unsigned)grid, launchLimit) : (unsigned)grid; }
 	DevBuf<unsigned char> mixInfo, coarseDone;
 	DevBuf<unsigned short> mixCount;
 	// lattices of the coarse levels (VxbDev::coarseLattice): own buffer, or - sharded runs - an area of the buffer the peers map
@@ -1157,6 +1159,13 @@ int vxb_set_capacity(vxb_context* ctx, uint64_t v, uint64_t i, uint64_t tv, uint
 	return VXB_OK;
 }
 
+int vxb_set_launch_limit(vxb_context* ctx, uint32_t ctas)
+{
+	if (!ctx) return VXB_ERR_ARGUMENT;
+	ctx->launchLimit = ctas; // part of the graph key: the next run re-captures
+	return VXB_OK;
+}
+
 // shardPhase: -1 = not a sharded run; 0 = scan + block info (no sync); 1 = plan + the levels below the coarse ones + page
 // publication (no sync); 2 = coarse levels, emission, directory (syncs, result); 3 = everything, the two exchanges by
 // ncclAllGather on the context's stream (needs vxb_shard_nccl_init)
@@ -1306,7 +1315,7 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 		KernelTimer timer{ ctx, kernelTimes };
 		uint32_t launches = 0;
 		for (int k = 0; k < 10; ++k) ctx->kindLaunches[k] = 0;
-		const unsigned flatGrid = (unsigned)ctx->smCount * 8;
+		const unsigned flatGrid = ctx->persistentGrid(ctx->smCount * 8);
 		cudaStream_t st = ctx->stream;
 
 		bool latticeForked = false;
@@ -1383,7 +1392,7 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 			if (selectLevel(0))
 			{
 				timer.begin(3);
-				vxb_block_kernel<0><<<ctx->gridBlock[0], VXB_THREADS, sizeof(VxbBlockSmem<0>), st>>>(ctx->tmapDist19, ctx->tmapDist19, dev, 0);
+				vxb_block_kernel<0><<<ctx->persistentGrid(ctx->gridBlock[0]),VXB_THREADS, sizeof(VxbBlockSmem<0>), st>>>(ctx->tmapDist19, ctx->tmapDist19, dev, 0);
 				timer.end(); ++launches; ++ctx->kindLaunches[3];
 			}
 			vxb_mark_split_kernel<<<1, 1, 0, st>>>(dev); ++launches; // level 0 is complete: the flat kernels work behind the split
@@ -1392,7 +1401,7 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 				if (!selectLevel(l)) continue;
 				if (l >= VXB_LATTICE_LO) joinLattice();
 				timer.begin(2);
-				vxb_block_kernel<1><<<ctx->gridBlock[1], VXB_THREADS, sizeof(VxbBlockSmem<1>), st>>>(ctx->tmap, ctx->tmap1, dev, l);
+				vxb_block_kernel<1><<<ctx->persistentGrid(ctx->gridBlock[1]),VXB_THREADS, sizeof(VxbBlockSmem<1>), st>>>(ctx->tmap, ctx->tmap1, dev, l);
 				timer.end(); ++launches; ++ctx->kindLaunches[2];
 			}
 			if (sharded && peers.count) { timer.begin(9); vxb_publish_kernel<<<(unsigned)ctx->smCount * 4, VXB_THREADS, 0, st>>>(dev, peers); timer.end(); ++launches; ++ctx->kindLaunches[9]; }
@@ -1405,12 +1414,12 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 			{
 				joinLattice(); // the lattices are complete
 				timer.begin(2);
-				vxb_block_kernel<2><<<ctx->gridBlock[2], VXB_THREADS, sizeof(VxbBlockSmem<2>), st>>>(ctx->tmap, ctx->tmap1, dev, coarseLo);
+				vxb_block_kernel<2><<<ctx->persistentGrid(ctx->gridBlock[2]),VXB_THREADS, sizeof(VxbBlockSmem<2>), st>>>(ctx->tmap, ctx->tmap1, dev, coarseLo);
 				timer.end(); ++launches; ++ctx->kindLaunches[2];
 			}
 			// blocks too large for the shared-memory path of vxb_block_kernel (> 1024 non-trivial cells / > 2048 level-0 vertices)
 			timer.begin(2);
-			vxb_big_block_kernel<<<ctx->gridBigBlock, VXB_THREADS, sizeof(VxbBigBlockSmem), st>>>(ctx->tmap, ctx->tmap1, dev);
+			vxb_big_block_kernel<<<ctx->persistentGrid(ctx->gridBigBlock),VXB_THREADS, sizeof(VxbBigBlockSmem), st>>>(ctx->tmap, ctx->tmap1, dev);
 			timer.end(); ++launches; ++ctx->kindLaunches[2];
 			// vertices + triangles of everything but the level-0 blocks done inside vxb_block_kernel<0>, next to the transition
 			// cells (which need the block records and the material pages only)
@@ -1430,7 +1439,7 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 			{
 				cudaStream_t ts = fork ? ctx->stream2 : st;
 				timer.begin(6);
-				vxb_transition_kernel<<<ctx->gridTransition, VXB_TR_THREADS, 0, ts>>>(dev);
+				vxb_transition_kernel<<<ctx->persistentGrid(ctx->gridTransition),VXB_TR_THREADS, 0, ts>>>(dev);
 				vxb_transition_vertex_kernel<<<flatGrid, VXB_THREADS, 0, ts>>>(dev);
 				timer.end(); launches += 2; ctx->kindLaunches[6] += 2;
 				if (fork)
@@ -1509,7 +1518,7 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 			for (const CUtensorMap* mp : maps) { memcpy(k, mp, sizeof(CUtensorMap)); k += sizeof(CUtensorMap); }
 			const void* ptrs[4] = { ctx->dDist, ctx->scanFlags.p, ctx->blockInfo.p, ctx->haveLattice1 ? ctx->latticePtr : nullptr };
 			memcpy(k, ptrs, sizeof(ptrs)); k += sizeof(ptrs);
-			const int scalars[6] = { computed, (int)validBytes, (int)nb0, (int)n, shardPhase, (int)flags };
+			const int scalars[7] = { computed, (int)validBytes, (int)nb0, (int)n, shardPhase, (int)flags, (int)ctx->launchLimit };
 			memcpy(k, scalars, sizeof(scalars));
 			if (!ctx->graphExec || key != ctx->graphKey)
 			{
