@@ -43,6 +43,32 @@ def _hostile_band(x, y, z, d, seed, vmax, materials):
     return np.ascontiguousarray(q), np.ascontiguousarray(mat), np.ascontiguousarray(blend)
 
 
+def hostile_full_range(n, seed=13, materials=5):
+    """hostile()'s wavy surface with distances over the whole int8 range: the field saturates at -128 / 127 a few voxels
+    off the surface, the band adds noise of +-100 and forced zeros, and (-128, 127) / (127, -128) pairs sit on cell edges
+    along x, y and z.  The values are clipped to [-128, 127] before the cast (no wrap of 128 to -128)."""
+    z, y, x = np.meshgrid(np.arange(n), np.arange(n), np.arange(n), indexing="ij")
+    d = z - (n / 2.0 + 6 * np.sin(0.21 * x) * np.cos(0.17 * y) + 3 * np.sin(0.05 * (x + y)))
+    h = _hash3(x, y, z, seed)
+    q = (np.sign(d) * np.ceil(np.abs(24 * d))).astype(np.int64)
+    near = np.abs(d) < 6
+    q = np.where(near, q + (h % np.uint64(201)).astype(np.int64) - 100, q)
+    q = np.where(near & ((h >> np.uint64(8)) % np.uint64(4) == 0), 0, q)
+    q = np.clip(q, -128, 127)
+    for axis, bit in ((0, 12), (1, 16), (2, 20)):   # z, y, x pairs: voxel v and its +1 neighbour along the axis
+        pick = near & ((h >> np.uint64(bit)) % np.uint64(8) == 0)
+        pick &= (np.stack([z, y, x])[axis] % 2 == 0) & (np.stack([z, y, x])[axis] < n - 1)
+        lo = np.where((h >> np.uint64(bit + 3)) & np.uint64(1), -128, 127)
+        src = np.argwhere(pick)
+        dst = src.copy(); dst[:, axis] += 1
+        q[tuple(src.T)] = lo[pick]
+        q[tuple(dst.T)] = np.where(lo[pick] == -128, 127, -128)
+    hm = _hash3(x // 5, y // 5, z // 3, seed + 1)
+    mat = (hm % np.uint64(materials)).astype(np.uint8)
+    blend = ((h >> np.uint64(24)) & np.uint64(0xFF)).astype(np.uint8)
+    return np.ascontiguousarray(q.astype(np.int8)), np.ascontiguousarray(mat), np.ascontiguousarray(blend)
+
+
 def noise_full(n, seed=3, lo=-5, hi=5):
     """Every voxel random in [lo, hi]: (almost) every cell non-trivial, worst case for counts."""
     z, y, x = np.meshgrid(np.arange(n), np.arange(n), np.arange(n), indexing="ij")
@@ -241,3 +267,166 @@ def skip_quirk(n=64):
     for a, part in zip((dist, mat, blend), _patch_content(BAND, bx, by, bz, 1)):
         a[0:16, 48:64, 0:16] = part[0]
     return dist, mat, blend
+
+
+# ---- rle_edges: the run-length thresholds of the grid store -------------------------------------------------------------
+# CompressBlock (VoxelGrid.cpp:610-672) ends a run at a value change or after 255 bytes and stores a channel raw once 2048
+# run ends were seen, i.e. at 2049 runs or more; BF_Empty = run-length coded and every voxel of one strict sign.  The
+# kernels decide BF_Empty from the scan's count of value changes inside the 16-byte rows (x): with 2048 or more the block
+# is raw, below 1777 it cannot reach 2049 runs (at most 255 row seams + 16 splits + 1 more), and in between
+# vxb_block_info_kernel walks the block (vxb_kernels.cuh).  Block contents below are [z, y, x] = 4096 bytes in
+# CompressBlock's order (x fastest).
+
+def runs_of(flat):
+    """CompressBlock's run count of 4096 bytes: maximal runs of one value, each cut every 255 bytes."""
+    flat = np.asarray(flat)
+    ends = np.flatnonzero(flat[1:] != flat[:-1]) + 1
+    lengths = np.diff(np.concatenate([[0], ends, [flat.size]]))
+    return int(((lengths + 254) // 255).sum())
+
+
+def inrow_changes(flat):
+    """The scan's count: adjacent bytes that differ inside the 16-byte rows (row seams not counted)."""
+    rows = np.asarray(flat).reshape(-1, 16)
+    return int((rows[:, 1:] != rows[:, :-1]).sum())
+
+
+def _from_runs(values, lengths):
+    out = np.repeat(np.asarray(values, np.int64), np.asarray(lengths, np.int64))
+    assert out.size == 4096, out.size
+    return out
+
+
+def _pairs(a, b):
+    """a a b b a a b b ...: 2048 runs of 2, 1792 in-row changes (7 per row) + 255 changes at the row seams."""
+    return np.where((np.arange(4096) // 2) % 2 == 0, a, b).astype(np.int64)
+
+
+def _with_split_runs(a, b, runs):
+    """510 bytes of a (two runs: one 255-byte cut), then `runs` - 2 runs alternating b, a, ...: first runs of 1 byte,
+    then of 2, as many of each as fill the other 3586 bytes."""
+    k = runs - 2
+    ones = 2 * k - 3586
+    return _from_runs([a] + [b, a] * (k // 2) + [b] * (k % 2), [510] + [1] * ones + [2] * (k - ones))
+
+
+def _threshold_block(kind, s):
+    """One threshold block's distance bytes (int8), of sign s: values s, 2s and 3s, or a zero."""
+    a, b, c = s, 2 * s, 3 * s
+    v = _pairs(a, b)
+    if kind == "runs2047":
+        v[4092:] = a                                       # the last pair joins the one before: 2047 runs
+    elif kind == "runs2048":
+        pass
+    elif kind == "runs2049":
+        v[1] = c                                           # a c b b ...: one more run end
+    elif kind in ("inrow1776", "inrow1777"):
+        rows = v.reshape(256, 16)
+        rows[:1792 - int(kind[5:]), 14:] = rows[:1792 - int(kind[5:]), 13:14]   # the row's last change goes
+    elif kind in ("inrow2047", "inrow2048"):
+        rows = v.reshape(256, 16)
+        full = 32 if kind == "inrow2048" else 31
+        rows[:full] = np.where(np.arange(16) % 2 == 0, a, b)   # 15 in-row changes instead of 7
+        if kind == "inrow2047":
+            rows[31] = np.where(np.arange(16) % 2 == 0, a, b); rows[31, 15] = rows[31, 14]   # 14
+    elif kind in ("split2048", "split2049"):
+        v = _with_split_runs(a, b, int(kind[5:]))
+    elif kind == "zero_first":
+        v[0] = 0
+    elif kind == "zero_last":
+        v[4095] = 0
+    elif kind == "uniform":
+        v[:] = -128 if s < 0 else 127
+    else:
+        raise ValueError(kind)
+    return v.astype(np.int8)
+
+
+# not BF_Empty (nothing of rle_edges_kept is skipped) / BF_Empty (rle_edges_skipped), each as a -1/-2 block among +4 ones
+# and a +1/+2 block on the low x side of a uniform -4 block
+KEPT_VARIANTS = ("runs2049", "inrow2047", "inrow2048", "split2049", "zero_first", "zero_last")
+SKIPPED_VARIANTS = ("runs2047", "runs2048", "inrow1776", "inrow1777", "split2048")
+_SKIPPED_EXTRA = [("uniform", -1), ("uniform", 1)]
+
+
+def _channel_variant(kind, lo, hi):
+    """A material / blend channel at a run-length threshold, values lo / hi (uint8)."""
+    if kind in ("runs2047", "runs2048", "runs2049"):
+        v = _threshold_block(kind, 1)
+        return np.select([v == 1, v == 2], [lo, hi], lo ^ hi)
+    if kind == "seams":   # runs of exactly 255, 256, 510 and 511 bytes, starting off the row seams (+ 1- and 3-byte fillers)
+        lengths, values, total, i = [], [], 0, 0
+        cycle = (7, 255, 256, 1, 510, 3, 511)
+        while total < 4096:
+            L = min(cycle[i % len(cycle)], 4096 - total)
+            lengths.append(L); values.append((lo, hi, (lo + 1) & 0xFF)[i % 3]); total += L; i += 1
+        return _from_runs(values, lengths)
+    return np.full(4096, {"uniform0": 0, "uniform80": 0x80, "uniformFF": 0xFF}[kind])
+
+
+CHANNEL_VARIANTS = ("runs2047", "runs2048", "runs2049", "seams", "uniform0", "uniform80", "uniformFF")
+
+
+def _thresholds(variants, extra):
+    slots = [(x, y, z) for z in (0, 3, 6) for y in (0, 3, 6) for x in (0, 3)]
+    placed = [(kind, s) for kind in variants for s in (-1, 1)] + list(extra)
+    assert len(placed) <= len(slots)
+    return [(kind, s, slot) for (kind, s), slot in zip(placed, slots)]
+
+
+def rle_edges_thresholds(name):
+    """(variant, sign, (bx, by, bz)) of every threshold block of rle_edges_kept / rle_edges_skipped."""
+    if name == "rle_edges_kept":
+        return _thresholds(KEPT_VARIANTS, [])
+    assert name == "rle_edges_skipped", name
+    return _thresholds(SKIPPED_VARIANTS, _SKIPPED_EXTRA)
+
+
+def _rle_edges(n, variants, extra):
+    """Threshold blocks T on the slots x in {0, 3}, y and z in {0, 3, 6}: three blocks apart, so that the level-0 skip of T
+    and its 26 neighbours depends on T's flag alone (a block with non-trivial cells is within one block of its T).  The
+    material / blend threshold channels fill the blocks with x >= 6, more than a block away from every surface, so that no
+    cell ever reads them (their materials include 255, EMPTY_MATERIAL) and they only meet the codec."""
+    assert n == 128
+    nb = n // 16
+    dist = np.full((n, n, n), 4, np.int8)
+    mat = np.zeros((n, n, n), np.uint8)
+    blend = np.zeros((n, n, n), np.uint8)
+
+    def put(a, bx, by, bz, flat):
+        a[bz * 16:bz * 16 + 16, by * 16:by * 16 + 16, bx * 16:bx * 16 + 16] = np.asarray(flat).reshape(16, 16, 16)
+
+    l = np.arange(16)
+    lz, ly, lx = np.meshgrid(l, l, l, indexing="ij")
+    for k, (kind, s, (bx, by, bz)) in enumerate(_thresholds(variants, extra)):
+        put(dist, bx, by, bz, _threshold_block(kind, s))
+        h = _hash3(lx + 16 * bx, ly + 16 * by, lz + 16 * bz, 29 + k)
+        put(mat, bx, by, bz, (1 + (_hash3(lx // 4, ly // 4, lz // 4, k) % np.uint64(3))).astype(np.uint8))
+        put(blend, bx, by, bz, (h & np.uint64(0xFF)).astype(np.uint8))
+        if s > 0:   # the surface along T's high x face: a uniform -4 block there
+            put(dist, bx + 1, by, bz, np.full(4096, -4))
+            put(mat, bx + 1, by, bz, np.full(4096, 2))
+    k = 0
+    for bz in range(nb):
+        for by in range(nb):
+            for bx in (6, 7):
+                if k < len(CHANNEL_VARIANTS) ** 2:
+                    mv, bv = CHANNEL_VARIANTS[k % len(CHANNEL_VARIANTS)], CHANNEL_VARIANTS[k // len(CHANNEL_VARIANTS)]
+                    put(mat, bx, by, bz, _channel_variant(mv, 1, 2))
+                    put(blend, bx, by, bz, _channel_variant(bv, 0x7F, 0x80))
+                k += 1
+    return dist, mat, blend
+
+
+def rle_edges_kept(n=128):
+    """Threshold blocks that are not BF_Empty: 2049 runs found by the walk, 2047 in-row changes (walked) and 2048 (raw
+    without a walk), 2049 runs with 255-byte cuts, a single 0 as the first / last byte.  Nothing is skipped at level 0,
+    so every level is defined in the reference."""
+    return _rle_edges(n, KEPT_VARIANTS, [])
+
+
+def rle_edges_skipped(n=128):
+    """Threshold blocks that are BF_Empty: 2047 / 2048 runs found by the walk, 1776 (not walked) / 1777 (walked) in-row
+    changes, 2048 runs with 255-byte cuts, uniform -128 and uniform 127.  The reference skips them with their neighbours
+    although the surface runs along their faces; like skip_quirk, its coarse levels are then undefined."""
+    return _rle_edges(n, SKIPPED_VARIANTS, _SKIPPED_EXTRA)

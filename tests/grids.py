@@ -32,6 +32,7 @@ SMALL = {
     "noise16": lambda: gridgen.noise_full(16, seed=2),
     "positive_noise32": lambda: gridgen.noise_full(32, seed=4, lo=1, hi=4),
     "patchwork64": lambda: gridgen.patchwork(64),
+    "hostile64_full_range": lambda: gridgen.hostile_full_range(64),
 }
 MEDIUM = {
     "hostile128": lambda: gridgen.hostile(128, seed=11),
@@ -59,8 +60,16 @@ HUGE = {
 }
 
 
+# the grid store's thresholds (tests/test_gpu_gridstore_edges.py): not in the tables above, whose every level is compared
+# with the reference, because the reference's coarse levels of rle_edges_skipped are undefined (see gridgen.skip_quirk)
+RLE_EDGES = {
+    "rle_edges_kept": gridgen.rle_edges_kept,
+    "rle_edges_skipped": gridgen.rle_edges_skipped,
+}
+
+
 def by_name(name):
-    for table in (SMALL, MEDIUM, LARGE, HUGE):
+    for table in (SMALL, MEDIUM, LARGE, HUGE, RLE_EDGES):
         if name in table:
             return table[name]()
     raise KeyError(name)

@@ -156,6 +156,12 @@ class VoxelsLib:
         self.L.vxh_pack_destroy(pack)
         return np.frombuffer(data, np.uint8).copy()
 
+    def grid_load(self, blob):
+        """Grid::Load of a PackForSave-format blob (numpy uint8); None when the reference refuses it."""
+        blob = np.ascontiguousarray(blob, np.uint8)
+        g = self.L.vxh_grid_load(self._ptr(blob), blob.size)
+        return g or None
+
     def grid_destroy(self, grid):
         self.L.vxh_grid_destroy(grid)
 

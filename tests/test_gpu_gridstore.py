@@ -98,20 +98,25 @@ def test_inject_material_equals_reference(reference, gpu_context):
     reference.grid_destroy(g)
 
 
-@pytest.mark.parametrize("name", ["terrain128", "hostile64", "noise32", "positive_noise32", "zeros32"])
+@pytest.mark.parametrize("name", ["terrain128", "hostile64", "noise32", "positive_noise32", "zeros32", "hostile64_full_range",
+                                  "rle_edges_kept", "rle_edges_skipped", "patchwork128"])
 def test_pack_equals_reference_pack_for_save(reference, gpu_context, name):
-    """GPU run-length coding incl. 255-byte run splits, RLE-ineffective (raw) blocks and the BF_Empty flag."""
+    """GPU run-length coding incl. 255-byte run splits, RLE-ineffective (raw) blocks and the BF_Empty flag; the rle_edges
+    grids put channels of 2047, 2048 (4096 bytes, run-length coded) and 2049 runs (raw) side by side.  The host packer
+    must give the same bytes, and the GPU decoder must read a 4096-byte channel as raw only when its flag says so."""
     import grids
+    import voxels_b200
     if name == "terrain128":
         dist, mat, blend = reference.builtin_dense(128, capi.Surface.terrain(128))
     elif name == "zeros32":
         dist = np.zeros((32, 32, 32), np.int8); mat = np.zeros((32, 32, 32), np.uint8); blend = np.full((32, 32, 32), 255, np.uint8)
         dist[:, :, 16:] = 3; dist[5, 5, 5] = -1
     else:
-        dist, mat, blend = grids.SMALL[name]()
+        dist, mat, blend = grids.by_name(name)
     g = reference.grid_from_dense(dist, mat, blend)
     want = reference.grid_pack(g)
     reference.grid_destroy(g)
+    assert np.array_equal(voxels_b200.pack_dense(dist, mat, blend), want), "host pack_dense differs from Grid::PackForSave"
     gpu_context.upload_dense(dist, mat, blend)
     got = gpu_context.pack()
     assert len(got) == len(want), "blob size %d vs %d" % (len(got), len(want))
@@ -119,7 +124,7 @@ def test_pack_equals_reference_pack_for_save(reference, gpu_context, name):
         bad = np.nonzero(got != want)[0]
         raise AssertionError("blob differs at %d bytes, first offset %d" % (len(bad), bad[0]))
     # and back: the packed form decodes (on the GPU) to the same voxels
-    gpu_context.upload_packed(got)
+    gpu_context.upload_packed(want)
     back = gpu_context.download_dense()
     for a, b in zip((dist, mat, blend), back):
         assert np.array_equal(a, b)

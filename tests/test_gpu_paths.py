@@ -6,13 +6,11 @@ flip, the double-buffer swap of the levels >= 1, the per-CTA accumulators, the i
 transition kernels) never sees hostile content.  vxb_set_launch_limit caps those grids at a few CTAs, so each one
 walks many items of mixed kinds.  patchwork512 / patchwork1024 reach the coarse lattice of mode 1 (level 2 of a
 1024^3 grid) with big blocks on it."""
-import numpy as np
 import pytest
 
-import compare
 import gridgen
 import grids
-from parity import run_both
+from parity import run_both, run_skipping_grid
 
 pytestmark = pytest.mark.gpu
 
@@ -90,18 +88,7 @@ def test_skip_quirk_against_reference_and_restatement(reference, restatement, li
     dist, mat, blend = gridgen.skip_quirk()
     ctx = _context(limit)
     try:
-        problems, res = run_both(reference, ctx, dist, mat, blend, max_levels=1)
-        assert not problems, "\n".join(problems[:10])
-        ctx.polygonize()
-        res = ctx.download()
-        h = restatement.run(dist, mat, blend)
-        try:
-            for l in range(restatement.levels(h)):
-                problems += compare.level_diff(restatement.level(h, l), res.level(l), "L%d" % l)
-            if not np.array_equal(restatement.stats(h), res.stats):
-                problems.append("stats differ")
-        finally:
-            restatement.destroy(h)
+        problems = run_skipping_grid(reference, restatement, ctx, dist, mat, blend)
         assert not problems, "\n".join(problems[:10])
     finally:
         ctx.close()

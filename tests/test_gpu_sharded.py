@@ -71,7 +71,10 @@ def assert_same(a, b, levels):
 
 @pytest.mark.parametrize("name,world,group", [("hostile128", 2, 0), ("hostile128", 4, 32), ("hostile128", 2, 32), ("sphere128", 2, 0),
                                               ("noise64", 2, 0), ("hostile64", 2, 0), ("hostile128", 1, 0), ("sphere128", 4, 0),
-                                              ("patchwork256", 4, 32), ("patchwork256", 8, 0)])
+                                              ("patchwork256", 4, 32), ("patchwork256", 8, 0),
+                                              # every rank walks the threshold blocks of its own layers (vxb_block_info_kernel)
+                                              ("rle_edges_kept", 2, 0), ("rle_edges_kept", 4, 0), ("rle_edges_skipped", 2, 0),
+                                              ("rle_edges_skipped", 4, 0)])
 def test_virtual_ranks_equal_single_run(gpu_context, name, world, group):
     import voxels_b200
     dist, mat, blend = grids.by_name(name)

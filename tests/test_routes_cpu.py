@@ -9,7 +9,11 @@ Routes (DESIGN.md section 2):
   - emitted blocks on every face, edge and corner of the grid, at level 0 and at the coarsest level of 2^3 blocks or more
 and, in the grid built for it (gridgen.skip_quirk), the level-0 skip of a block whose 27-neighbourhood is BF_Empty although
 the surface runs along its faces (TransVoxelImpl.cpp:520).  The patchwork grids must never reach that skip: the
-reference's coarse cells over a skipped block read an uninitialised material, so their output is not defined."""
+reference's coarse cells over a skipped block read an uninitialised material, so their output is not defined.
+
+The grid store's thresholds are pinned the same way: the rle_edges grids reach BF_Empty through the walk of
+vxb_block_info_kernel with both outcomes, the 2048 / 2049-run codec boundary in all three channels, and (only
+rle_edges_skipped) the skip; hostile64_full_range spans the whole int8 range."""
 import itertools
 
 import numpy as np
@@ -105,3 +109,125 @@ def test_patchwork_is_deterministic_and_bounded():
     assert 1000 < int((kinds != gridgen.UNI_POS).sum()) < 20000   # a bounded amount of work at 1024^3
     for k in range(len(gridgen.KIND_NAMES)):
         assert (gridgen.patchwork_kinds(128) == k).any(), "patchwork128 has no %s block" % gridgen.KIND_NAMES[k]
+
+
+# ---- the grid store's thresholds (gridgen.rle_edges_*, hostile64_full_range; tests/test_gpu_gridstore_edges.py) ------
+
+RLE_EDGES = ("rle_edges_kept", "rle_edges_skipped")
+BF_EMPTY = 1
+
+
+def _blocks(a):
+    """Every 16^3 block of a as a row of 4096 bytes in CompressBlock's order, block order z, y, x."""
+    nb = a.shape[0] // 16
+    return a.reshape(nb, 16, nb, 16, nb, 16).transpose(0, 2, 4, 1, 3, 5).reshape(-1, 4096)
+
+
+def _pack_table(blob, nb):
+    """(sizes [blocks, 3], flags [blocks]) of a PackForSave blob."""
+    sizes = blob[16:16 + nb ** 3 * 12].view(np.uint32).reshape(-1, 3).astype(np.int64)
+    offsets = 16 + nb ** 3 * 12 + np.concatenate([[0], np.cumsum(4 + sizes.sum(axis=1))[:-1]])
+    flags = np.array([int(blob[o:o + 4].view(np.uint32)[0]) for o in offsets])
+    return sizes, flags
+
+
+def _reference_state(reference, dist, mat, blend):
+    g = reference.grid_from_dense(dist, mat, blend)
+    try:
+        return reference.grid_empty_flags(g), reference.grid_pack(g)
+    finally:
+        reference.grid_destroy(g)
+
+
+@pytest.mark.parametrize("name", RLE_EDGES)
+def test_rle_edges_empty_flags(reference, restatement, name):
+    """Every threshold block has the BF_Empty flag it was built for in the reference, and the restatement agrees."""
+    dist, mat, blend = grids.by_name(name)
+    nb = dist.shape[0] // 16
+    empty, _ = _reference_state(reference, dist, mat, blend)
+    want = name == "rle_edges_skipped"
+    for kind, s, (bx, by, bz) in gridgen.rle_edges_thresholds(name):
+        assert bool(empty[(bz * nb + by) * nb + bx]) == want, "%s %+d at block %s" % (kind, s, (bx, by, bz))
+    h = restatement.run(dist, mat, blend)
+    try:
+        assert np.array_equal(restatement.empty_flags(h, dist.shape[0]), empty)
+    finally:
+        restatement.destroy(h)
+
+
+def test_rle_edges_reach_the_walk_both_ways(reference):
+    """A numpy model of the scan's in-row count: one-signed blocks with a count in [1777, 2047] are walked, with both
+    outcomes; one-signed blocks with 2048 are decided non-empty without a walk; 1776 is not walked.  The model's run count
+    (runs of one value cut every 255 bytes) decides BF_Empty exactly as the reference does."""
+    seen = set()
+    for name in RLE_EDGES:
+        dist, mat, blend = grids.by_name(name)
+        empty, _ = _reference_state(reference, dist, mat, blend)
+        for b, flat in enumerate(_blocks(dist)):
+            one_signed = (flat > 0).all() or (flat < 0).all()
+            changes, runs = gridgen.inrow_changes(flat), gridgen.runs_of(flat)
+            assert bool(empty[b]) == (one_signed and runs <= 2048), "%s block %d: %d runs" % (name, b, runs)
+            if not one_signed:
+                continue
+            if 1777 <= changes < 2048:
+                seen.add(("walked", bool(empty[b]), runs))
+            elif changes >= 2048:
+                seen.add(("non-empty without a walk", bool(empty[b]), None))
+            seen.add(("in-row", changes))
+    for want in [("walked", True, 2047), ("walked", True, 2048), ("walked", False, 2049),
+                 ("non-empty without a walk", False, None), ("in-row", 1776), ("in-row", 1777), ("in-row", 2047), ("in-row", 2048)]:
+        assert want in seen, want
+
+
+def test_rle_edges_pack_table(reference):
+    """PackForSave's size table holds channels of exactly 4096 run-length coded bytes (raw flag clear, 2048 runs) next to
+    raw ones, in all three channels; the model's run count gives every size."""
+    coded4096, raw = set(), set()
+    for name in RLE_EDGES:
+        arrays = grids.by_name(name)
+        nb = arrays[0].shape[0] // 16
+        _, blob = _reference_state(reference, *arrays)
+        sizes, flags = _pack_table(blob, nb)
+        for ch, a in enumerate(arrays):
+            runs = np.array([gridgen.runs_of(flat) for flat in _blocks(a)])
+            is_raw = (flags >> (1 + ch)) & 1 == 1
+            assert np.array_equal(is_raw, runs > 2048), (name, ch)
+            assert np.array_equal(sizes[:, ch], np.where(is_raw, 4096, 2 * runs)), (name, ch)
+            if ((sizes[:, ch] == 4096) & ~is_raw).any():
+                coded4096.add(ch)
+            if is_raw.any():
+                raw.add(ch)
+    assert coded4096 == raw == {0, 1, 2}, (coded4096, raw)
+
+
+@pytest.mark.parametrize("name", RLE_EDGES + ("hostile64_full_range",))
+def test_rle_edges_skip_and_full_range(reference, name):
+    """rle_edges_skipped skips level-0 blocks with non-trivial cells; rle_edges_kept and hostile64_full_range skip none
+    (their coarse levels are defined in the reference: it gives the same output at 1 and 4 threads)."""
+    import golden_hash
+    dist, mat, blend = grids.by_name(name)
+    nb = dist.shape[0] // 16
+    empty, _ = _reference_state(reference, dist, mat, blend)
+    skipped = skipped_blocks(empty.reshape(nb, nb, nb).astype(bool)) & (gridgen.nontrivial_cells_per_block(dist, 0) > 0)
+    if name == "rle_edges_skipped":
+        assert skipped.sum() >= 8, skipped.sum()
+        return
+    assert not skipped.any(), skipped.sum()
+    g = reference.grid_from_dense(dist, mat, blend)
+    digests = []
+    for threads in (1, 4):
+        s, _ = reference.polygonize(g, threads=threads)
+        digests.append([golden_hash.level_digests(reference.surface_level(s, l)) for l in range(reference.surface_levels(s))])
+        reference.surface_destroy(s)
+    reference.grid_destroy(g)
+    assert digests[0] == digests[1]
+
+
+def test_full_range_grid_spans_int8():
+    dist, _, _ = grids.by_name("hostile64_full_range")
+    d = dist.astype(np.int64)
+    assert d.min() == -128 and d.max() == 127 and (d == 0).any()
+    assert len(np.unique(d)) == 256
+    for axis in range(3):   # (-128, 127) and (127, -128) on cell edges along every axis
+        a, b = np.moveaxis(d, axis, 0)[:-1], np.moveaxis(d, axis, 0)[1:]
+        assert ((a == -128) & (b == 127)).any() and ((a == 127) & (b == -128)).any(), axis
