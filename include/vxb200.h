@@ -162,6 +162,67 @@ int vxb_grid_pack(vxb_context* ctx, void* out, size_t capacity, size_t* written)
 /* The dense volumes back to HOST memory (n^3 bytes each; any pointer may be NULL). */
 int vxb_grid_download_dense(vxb_context* ctx, int8_t* dist, uint8_t* mat, uint8_t* blend);
 
+/* ---- client-composed surfaces: SDF programs ---------------------------------------------------------------------------
+ * A client's own VoxelSurface as data: a stack program of SDF primitives and CSG operators, evaluated on the device by the
+ * fill and edit kernels and on the host by voxels_b200/csrc/vxb_program.h (the same source, bit-identical floats).  Ops run
+ * in order on a value stack; every value carries the material / blend of the primitive it came from.
+ *
+ * Primitives (push one value).  The sample point p (grid, Z-up coordinates) is first mapped to local coordinates
+ * q = M p + t, xform = rows {m0, m1, m2, t}, each component ((m_i.x * p.x + m_i.y * p.y) + m_i.z * p.z) + t_i:
+ *   SPHERE    p[0] = r:               |q| - r = sqrt((qx*qx + qy*qy) + qz*qz) - r
+ *   BOX       p[0..2] = half extents: e = |q| - h per axis; sqrt((mx*mx + my*my) + mz*mz) + min(max(ex, max(ey, ez)), 0)
+ *                                     with m = max(e, 0) (the exact box distance)
+ *   CYLINDER  p[0] = r, p[1] = half height, axis = local z: a = sqrt(qx*qx + qy*qy) - r, b = |qz| - h;
+ *                                     min(max(a, b), 0) + sqrt(max(a, 0)^2 + max(b, 0)^2)
+ *   CAPSULE   p[0] = r, p[1] = half length of the segment along local z: c = qz - clamp(qz, -h, h);
+ *                                     sqrt((qx*qx + qy*qy) + c*c) - r
+ *   TORUS     p[0] = R (ring), p[1] = r (tube), ring in the local xy plane: a = sqrt(qx*qx + qy*qy) - R; sqrt(a*a + qz*qz) - r
+ *   PLANE     p[0..2] = n, p[3] = d0:  ((nx*qx + ny*qy) + nz*qz) - d0
+ *   TERRAIN   p[0] = N, p[1..2] = (ox, oy), seed: VXB_SURFACE_TERRAIN evaluated at q (its own material and blend)
+ * SPHERE, PLANE and TERRAIN are vxb_surface's formulas: a one-op program with M = identity and t = -centre (t = 0 for PLANE
+ * and TERRAIN) gives the bytes vxb_grid_fill gives.  Every primitive value is clamped to +-100, as the final value is.
+ * Operators (a = the value below the top, b = the top):
+ *   UNION         min(a, b)                              material of the smaller value
+ *   INTERSECT     max(a, b)                              material of the larger value
+ *   SUBTRACT      max(a, -b)                             material of the side that won
+ *   SMOOTH_UNION  p[0] = k > 0: h = max(k - |a - b|, 0) / k; min(a, b) - ((h*h) * k) * 0.25   material of the smaller value
+ *   OFFSET        p[0] = r: d - r                        material kept
+ *   SHELL         p[0] = thickness: |d| - thickness      material kept
+ * Ties go to the left operand (a).  Floats: +, -, *, /, sqrt, floor and compare-selects only, in the order written.
+ * Limits: at most VXB_PROGRAM_MAX_OPS ops, a stack depth of VXB_PROGRAM_MAX_DEPTH, at most VXB_PROGRAM_MAX_TERRAIN TERRAIN
+ * ops.  A malformed program (NULL / empty, unknown code, stack underflow or overflow, not exactly one value at the end, a
+ * non-finite float in any op, k <= 0, a negative radius / extent / thickness, N <= 0, material or blend > 255, too many
+ * ops or TERRAIN ops) returns VXB_ERR_ARGUMENT naming the op index in vxb_last_error and leaves the grid untouched. */
+enum
+{
+	VXB_OP_SPHERE = 0, VXB_OP_BOX, VXB_OP_CYLINDER, VXB_OP_CAPSULE, VXB_OP_TORUS, VXB_OP_PLANE, VXB_OP_TERRAIN,  /* push one value */
+	VXB_OP_UNION = 16, VXB_OP_INTERSECT, VXB_OP_SUBTRACT, VXB_OP_SMOOTH_UNION,                               /* pop two, push one */
+	VXB_OP_OFFSET = 32, VXB_OP_SHELL                                                                        /* pop one, push one */
+};
+enum { VXB_PROGRAM_MAX_OPS = 64, VXB_PROGRAM_MAX_DEPTH = 8, VXB_PROGRAM_MAX_TERRAIN = 2 };
+typedef struct vxb_op
+{
+	uint32_t code, material, blend, seed;  /* material / blend: primitives; seed: TERRAIN */
+	float xform[12];                       /* primitives: local = M p + t, rows {m0, m1, m2, t} */
+	float p[8];                            /* shape parameters; SMOOTH_UNION p[0] = k; OFFSET p[0] = r; SHELL p[0] = thickness */
+} vxb_op;                                  /* 96 bytes */
+/* vxb_grid_fill with a program: the same sample coordinates, quantisation (round away from zero, clamp +-4), cube pieces
+ * and bookkeeping.  Two passes: a per-block interval pass writes the 16^3 blocks it proves constant (every sample +4 or
+ * every sample -4, one primitive selected throughout, not TERRAIN) and lists the others; the listed blocks are then
+ * evaluated per voxel. */
+int vxb_grid_fill_program(vxb_context* ctx, uint32_t n, const vxb_op* ops, uint32_t count, const float start[3], float step);
+/* vxb_grid_inject_surface with a program: the same sample coordinates, combine rules for `type` and returned box. */
+int vxb_grid_inject_program(vxb_context* ctx, const float position[3], const float extents[3], const vxb_op* ops, uint32_t count,
+	int type, float out_min[3], float out_max[3]);
+/* What the last vxb_grid_fill_program of this context did (this rank's pieces with a cube): blocks it covered, blocks the
+ * interval pass wrote, and the device time of the two passes (CUDA events). */
+typedef struct vxb_program_stats
+{
+	uint64_t blocks, culled;
+	float pass_a_ms, pass_b_ms;
+} vxb_program_stats;
+int vxb_grid_program_stats(vxb_context* ctx, vxb_program_stats* out);
+
 /* MaterialMap::GetMaterial pre-tabulated (include/MaterialMap.h:19-30): table = 256 x
  * {DiffuseIds0[3], DiffuseIds1[3]}, valid = 256 bytes (0 = GetMaterial returned nullptr).
  * NULL table = identity map, NULL valid = all valid. */

@@ -2,7 +2,8 @@
 
   oracle/_ref/...                 everything compiled from the reference checkout (oracle/Makefile): the Transvoxel
                                   tables re-packed for the device (_ref/gen), the reference itself (test oracle) and
-                                  the drop-in's objects that need the reference's headers (_ref/dropin)
+                                  the drop-in's objects that need the reference's headers (_ref/dropin), and the
+                                  SDF-program harness over the reference (oracle/programs.mk)
   voxels_b200/lib/libvxb200.so    CUDA kernels + C ABI (include/vxb200.h), sm_90a (H100) only
   voxels_b200/lib/libvoxels_b200.so, build/libvxh_b200.so   C++ drop-in Polygonizer + test harness over it
   build/oracle/libvxr_restate.so  CPU restatement (test infrastructure)
@@ -56,6 +57,9 @@ def build_oracle():
                                % (os.path.relpath(TABLES, REPO), REF))
         targets = ["restate"]
     _run(["make", "-C", ORACLE] + targets + ["REF=" + REF], stdout=subprocess.DEVNULL)
+    if have_reference():
+        # the SDF-program harness over the reference (tests/program_harness.py)
+        _run(["make", "-C", ORACLE, "-f", "programs.mk", "programs", "REF=" + REF], stdout=subprocess.DEVNULL)
 
 
 def build_cuda(force=False, verbose=False):

@@ -63,6 +63,98 @@ class Surface(C.Structure):
         return s
 
 
+OP_SPHERE, OP_BOX, OP_CYLINDER, OP_CAPSULE, OP_TORUS, OP_PLANE, OP_TERRAIN = range(7)
+OP_UNION, OP_INTERSECT, OP_SUBTRACT, OP_SMOOTH_UNION = range(16, 20)
+OP_OFFSET, OP_SHELL = 32, 33
+PROGRAM_MAX_OPS, PROGRAM_MAX_DEPTH, PROGRAM_MAX_TERRAIN = 64, 8, 2
+
+
+class Op(C.Structure):
+    """vxb_op (include/vxb200.h): one instruction of an SDF program.  Primitives take their placement as `at` (the local
+    origin in grid coordinates) and `rotation` (3x3, local -> grid axes; any invertible matrix, so scales and shears too):
+    the stored transform is local = inverse(rotation) (p - at).  `xform` (12 floats, rows {m0, m1, m2, t}) overrides both."""
+    _fields_ = [("code", C.c_uint32), ("material", C.c_uint32), ("blend", C.c_uint32), ("seed", C.c_uint32),
+                ("xform", C.c_float * 12), ("p", C.c_float * 8)]
+
+    @staticmethod
+    def _make(code, params=(), at=None, rotation=None, xform=None, material=0, blend=0, seed=0):
+        o = Op()
+        o.code, o.material, o.blend, o.seed = code, material, blend, seed
+        for k, v in enumerate(params):
+            o.p[k] = v
+        if code < 16:
+            if xform is None:
+                m = np.eye(3) if rotation is None else np.linalg.inv(np.asarray(rotation, np.float64))
+                c = np.zeros(3) if at is None else np.asarray(at, np.float64)
+                xform = np.concatenate([m.ravel(), -(m @ c)])
+            for k, v in enumerate(np.asarray(xform, np.float32).ravel()):
+                o.xform[k] = float(v)
+        return o
+
+    @staticmethod
+    def sphere(radius, at=None, rotation=None, material=0, blend=0, xform=None):
+        return Op._make(OP_SPHERE, (radius,), at, rotation, xform, material, blend)
+
+    @staticmethod
+    def box(half, at=None, rotation=None, material=0, blend=0, xform=None):
+        return Op._make(OP_BOX, tuple(half), at, rotation, xform, material, blend)
+
+    @staticmethod
+    def cylinder(radius, half_height, at=None, rotation=None, material=0, blend=0, xform=None):
+        return Op._make(OP_CYLINDER, (radius, half_height), at, rotation, xform, material, blend)
+
+    @staticmethod
+    def capsule(radius, half_length, at=None, rotation=None, material=0, blend=0, xform=None):
+        return Op._make(OP_CAPSULE, (radius, half_length), at, rotation, xform, material, blend)
+
+    @staticmethod
+    def torus(ring, tube, at=None, rotation=None, material=0, blend=0, xform=None):
+        return Op._make(OP_TORUS, (ring, tube), at, rotation, xform, material, blend)
+
+    @staticmethod
+    def plane(normal, d0, at=None, rotation=None, material=0, blend=0, xform=None):
+        return Op._make(OP_PLANE, (normal[0], normal[1], normal[2], d0), at, rotation, xform, material, blend)
+
+    @staticmethod
+    def terrain(period, origin=(0.0, 0.0), seed=1234, at=None, rotation=None, xform=None):
+        return Op._make(OP_TERRAIN, (float(period), float(origin[0]), float(origin[1])), at, rotation, xform, seed=seed)
+
+    @staticmethod
+    def union():
+        return Op._make(OP_UNION)
+
+    @staticmethod
+    def intersect():
+        return Op._make(OP_INTERSECT)
+
+    @staticmethod
+    def subtract():
+        return Op._make(OP_SUBTRACT)
+
+    @staticmethod
+    def smooth_union(k):
+        return Op._make(OP_SMOOTH_UNION, (k,))
+
+    @staticmethod
+    def offset(r):
+        return Op._make(OP_OFFSET, (r,))
+
+    @staticmethod
+    def shell(thickness):
+        return Op._make(OP_SHELL, (thickness,))
+
+
+def program_array(ops):
+    """A list of Op as the contiguous vxb_op array the C ABI takes (also accepts such an array)."""
+    if isinstance(ops, C.Array):
+        return ops
+    return (Op * len(ops))(*ops)
+
+
+class ProgramStats(C.Structure):
+    _fields_ = [("blocks", C.c_uint64), ("culled", C.c_uint64), ("pass_a_ms", C.c_float), ("pass_b_ms", C.c_float)]
+
+
 class DrawLists(C.Structure):
     _fields_ = [("regular_count", C.c_uint32), ("transition_count", C.c_uint32), ("counts", C.c_void_p), ("regular", C.c_void_p),
                 ("regular_info", C.c_void_p), ("transition", C.c_void_p), ("transition_info", C.c_void_p)]
@@ -135,6 +227,9 @@ def load_library():
         "vxb_grid_inject_material": (C.c_int, [vp, vp, vp, u32, C.c_int, vp, vp]),
         "vxb_grid_pack": (C.c_int, [vp, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
         "vxb_grid_download_dense": (C.c_int, [vp, vp, vp, vp]),
+        "vxb_grid_fill_program": (C.c_int, [vp, u32, vp, u32, vp, C.c_float]),
+        "vxb_grid_inject_program": (C.c_int, [vp, vp, vp, vp, u32, C.c_int, vp, vp]),
+        "vxb_grid_program_stats": (C.c_int, [vp, C.POINTER(ProgramStats)]),
         "vxb_result_device_arenas": (C.c_int, [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
         "vxb_result_select_lod": (C.c_int, [vp, vp, C.c_float, C.POINTER(DrawLists)]),
         "vxb_result_download_draws": (C.c_int, [vp, vp, vp, vp, vp]),
@@ -178,7 +273,8 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_shard_buffers_get", "vxb_shard_set_peer", "vxb_shard_export", "vxb_shard_import", "vxb_shard_nccl_unique_id",
                     "vxb_shard_nccl_init", "vxb_grid_fill", "vxb_grid_inject_surface", "vxb_grid_inject_material", "vxb_grid_pack",
                     "vxb_grid_download_dense", "vxb_result_device_arenas", "vxb_result_select_lod", "vxb_result_download_draws", "vxb_cube_create", "vxb_cube_info", "vxb_cube_export", "vxb_cube_import", "vxb_cube_piece",
-                    "vxb_grid_upload_packed_streamed", "vxb_result_download_begin", "vxb_result_download_end"]
+                    "vxb_grid_upload_packed_streamed", "vxb_result_download_begin", "vxb_result_download_end",
+                    "vxb_grid_fill_program", "vxb_grid_inject_program", "vxb_grid_program_stats"]
 
 
 def nccl_unique_id():
@@ -352,6 +448,28 @@ class Context:
         lo = np.zeros(3, np.float32); hi = np.zeros(3, np.float32)
         self._check(self.L.vxb_grid_inject_material(self.h, _ptr(p), _ptr(e), material, 1 if add_subtract_blend else 0, _ptr(lo), _ptr(hi)), "vxb_grid_inject_material")
         return np.concatenate([lo, hi])
+
+    def fill_program(self, n, ops, start=(0.0, 0.0, 0.0), step=1.0):
+        """Grid::Create(n, n, n, start, step, &surface) with an SDF program (a list of Op); with a cube: this rank's pieces."""
+        arr = program_array(ops)
+        st = np.ascontiguousarray(start, np.float32)
+        self._check(self.L.vxb_grid_fill_program(self.h, n, C.cast(arr, C.c_void_p), len(arr), _ptr(st), step), "vxb_grid_fill_program")
+        self.n = n
+
+    def inject_program(self, position, extents, ops, inject_type):
+        """VoxelGrid::InjectSurface with an SDF program sampled relative to `position`; returns the modified box (Y-up)."""
+        arr = program_array(ops)
+        p = np.ascontiguousarray(position, np.float32); e = np.ascontiguousarray(extents, np.float32)
+        lo = np.zeros(3, np.float32); hi = np.zeros(3, np.float32)
+        self._check(self.L.vxb_grid_inject_program(self.h, _ptr(p), _ptr(e), C.cast(arr, C.c_void_p), len(arr), inject_type, _ptr(lo), _ptr(hi)),
+                    "vxb_grid_inject_program")
+        return np.concatenate([lo, hi])
+
+    def program_stats(self):
+        """The last fill_program: blocks covered, blocks written by the cull pass, pass A / pass B device milliseconds."""
+        s = ProgramStats()
+        self._check(self.L.vxb_grid_program_stats(self.h, C.byref(s)), "vxb_grid_program_stats")
+        return s
 
     def pack(self):
         """Grid::PackForSave of the device grid (GPU run-length coding): numpy uint8 blob."""

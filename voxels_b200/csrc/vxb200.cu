@@ -10,6 +10,7 @@
 #include <chrono>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -76,6 +77,9 @@ struct vxb_context
 	DevBuf<uint8_t> volDist, volMat, volBlend, staging;
 	DevBuf<unsigned long long> packOffsets;
 	DevBuf<float> fillColumns;
+	DevBuf<unsigned int> progList, progCount;       // vxb_grid_fill_program: blocks left to the per-voxel pass + their count
+	cudaEvent_t progEv[3] = { nullptr, nullptr, nullptr };
+	vxb_program_stats progStats = { 0, 0, 0.f, 0.f };
 	DevBuf<vxb_draw_command> drawCmd, drawTCmd;
 	DevBuf<vxb_draw_info> drawInfo, drawTInfo;
 	DevBuf<unsigned int> drawCounts;
@@ -687,6 +691,8 @@ void vxb_destroy(vxb_context* ctx)
 	if (ctx->shard.comm && ncclApi().ok) { ncclApi().commDestroy(ctx->shard.comm); ctx->shard.comm = nullptr; }
 	releaseCube(ctx);
 	ctx->fillColumns.release(); ctx->packSizes.release(); ctx->packFlags.release(); ctx->packError.release();
+	ctx->progList.release(); ctx->progCount.release();
+	for (cudaEvent_t e : ctx->progEv) if (e) cudaEventDestroy(e);
 	ctx->drawCmd.release(); ctx->drawTCmd.release(); ctx->drawInfo.release(); ctx->drawTInfo.release(); ctx->drawCounts.release();
 	ctx->mixInfo.release(); ctx->coarseDone.release(); ctx->mixCount.release(); ctx->coarseLatticeBuf.release(); ctx->coarseMaps.release();
 	ctx->volDist.release(); ctx->volMat.release(); ctx->volBlend.release(); ctx->staging.release(); ctx->packOffsets.release(); ctx->updCoords.release(); ctx->lattice1.release();
@@ -1061,6 +1067,110 @@ int vxb_grid_inject_material(vxb_context* ctx, const float position[3], const fl
 	vxb_inject_material_kernel<<<(unsigned)(a.bn[0] * a.bn[1] * a.bn[2]), 256, 0, ctx->stream>>>(a, ctx->volMat.p, ctx->volBlend.p);
 	VXB_CUDA(ctx, cudaGetLastError());
 	ctx->haveResult = false;
+	return VXB_OK;
+}
+
+namespace
+{
+// validates the program (vxp_validate) and copies it into its kernel-parameter form, with the permutation tables of its
+// TERRAIN ops; nothing on the device is touched before this has passed
+int loadProgram(vxb_context* ctx, const char* who, const vxb_op* ops, uint32_t count, VxbProgram& p)
+{
+	const char* why = "";
+	const int bad = vxp_validate(ops, count, &why);
+	if (bad >= 0)
+	{
+		char buf[256];
+		snprintf(buf, sizeof(buf), "%s: op %d: %s", who, bad, why);
+		return fail(ctx, VXB_ERR_ARGUMENT, buf);
+	}
+	memset(&p, 0, sizeof(p));
+	memcpy(p.ops, ops, count * sizeof(vxb_op));
+	p.count = (int)count;
+	int t = 0;
+	for (uint32_t i = 0; i < count; ++i)
+		if (ops[i].code == VXB_OP_TERRAIN) vxs_permutation(ops[i].seed, p.perm[t++]);
+	return VXB_OK;
+}
+}
+
+int vxb_grid_fill_program(vxb_context* ctx, uint32_t n, const vxb_op* ops, uint32_t count, const float start[3], float step)
+{
+	if (!ctx) return VXB_ERR_ARGUMENT;
+	if (!validSize(n)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_grid_fill_program: bad size");
+	std::unique_ptr<VxbProgramFillArgs> args(new VxbProgramFillArgs);
+	int r = loadProgram(ctx, "vxb_grid_fill_program", ops, count, args->prog);
+	if (r != VXB_OK) return r;
+	cudaSetDevice(ctx->device);
+	const bool pieces = ctx->cube.active;
+	if (pieces && ctx->cube.n != n) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_grid_fill_program: n differs from the cube's");
+	r = pieces ? VXB_OK : ensureGridStorage(ctx, n);
+	if (r != VXB_OK) return r;
+	const size_t nb = n / 16;
+	VXB_CUDA(ctx, ctx->progList.ensure(nb * nb * nb));
+	VXB_CUDA(ctx, ctx->progCount.ensure(1));
+	for (cudaEvent_t& e : ctx->progEv) if (!e) VXB_CUDA(ctx, cudaEventCreate(&e));
+	for (int k = 0; k < 3; ++k) args->start[k] = start ? start[k] : 0.f;
+	args->step = step;
+	args->n = (int)n;
+	signed char* dDist = const_cast<signed char*>(reinterpret_cast<const signed char*>(pieces ? ctx->dDist : reinterpret_cast<const int8_t*>(ctx->volDist.p)));
+	unsigned char* dMat = pieces ? const_cast<unsigned char*>(ctx->dMat) : ctx->volMat.p;
+	unsigned char* dBlend = pieces ? const_cast<unsigned char*>(ctx->dBlend) : ctx->volBlend.p;
+	// block ranges: the whole grid, or the z-pieces this rank backs (multiples of 32 planes, so whole block layers)
+	std::vector<std::pair<unsigned, unsigned> > ranges;
+	if (pieces) for (uint32_t p = ctx->cube.rank; p < ctx->cube.pieces; p += ctx->cube.world)
+		ranges.push_back(std::make_pair((unsigned)(p * ctx->cube.groupPlanes / 16 * nb * nb), (unsigned)((p + 1) * ctx->cube.groupPlanes / 16 * nb * nb)));
+	else ranges.push_back(std::make_pair(0u, (unsigned)(nb * nb * nb)));
+	uint64_t blocks = 0;
+	VXB_CUDA(ctx, cudaMemsetAsync(ctx->progCount.p, 0, sizeof(unsigned), ctx->stream));
+	cudaEventRecord(ctx->progEv[0], ctx->stream);
+	for (const auto& rg : ranges)
+	{
+		args->b0 = rg.first; args->b1 = rg.second;
+		blocks += rg.second - rg.first;
+		vxb_program_cull_kernel<<<(rg.second - rg.first + 255) / 256, 256, 0, ctx->stream>>>(*args, dDist, dMat, dBlend, ctx->progList.p, ctx->progCount.p);
+	}
+	cudaEventRecord(ctx->progEv[1], ctx->stream);
+	vxb_program_fill_kernel<<<(unsigned)ctx->smCount * 8, 256, 0, ctx->stream>>>(*args, ctx->progList.p, ctx->progCount.p, dDist, dMat, dBlend);
+	cudaEventRecord(ctx->progEv[2], ctx->stream);
+	const cudaError_t e = cudaGetLastError();
+	const cudaError_t e2 = cudaStreamSynchronize(ctx->stream);
+	if (e != cudaSuccess || e2 != cudaSuccess) return fail(ctx, VXB_ERR_CUDA, "vxb_grid_fill_program", e != cudaSuccess ? e : e2);
+	unsigned listed = 0;
+	VXB_CUDA(ctx, cudaMemcpy(&listed, ctx->progCount.p, sizeof(unsigned), cudaMemcpyDeviceToHost));
+	ctx->progStats.blocks = blocks;
+	ctx->progStats.culled = blocks - listed;
+	cudaEventElapsedTime(&ctx->progStats.pass_a_ms, ctx->progEv[0], ctx->progEv[1]);
+	cudaEventElapsedTime(&ctx->progStats.pass_b_ms, ctx->progEv[1], ctx->progEv[2]);
+	if (pieces) { ctx->haveResult = false; ctx->haveFullRun = false; return VXB_OK; }
+	return finishUpload(ctx);
+}
+
+int vxb_grid_inject_program(vxb_context* ctx, const float position[3], const float extents[3], const vxb_op* ops, uint32_t count,
+	int type, float outMin[3], float outMax[3])
+{
+	if (!ctx || !position || !extents) return VXB_ERR_ARGUMENT;
+	if (type < 0 || type > 2) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_grid_inject_program: bad injection type");
+	std::unique_ptr<VxbProgramEditArgs> a(new VxbProgramEditArgs);
+	const int lr = loadProgram(ctx, "vxb_grid_inject_program", ops, count, a->prog);
+	if (lr != VXB_OK) return lr;
+	cudaSetDevice(ctx->device);
+	VxbEditArgs e;
+	const int r = prepareEdit(ctx, "vxb_grid_inject_program: needs a context-owned grid (upload or fill)", position, extents, e, outMin, outMax);
+	if (r < 0) return r;
+	if (r == 1) return VXB_OK;
+	for (int k = 0; k < 3; ++k) { a->position[k] = e.position[k]; a->extents[k] = e.extents[k]; a->b0[k] = e.b0[k]; a->bn[k] = e.bn[k]; }
+	a->type = type; a->n = e.n;
+	vxb_inject_program_kernel<<<(unsigned)(e.bn[0] * e.bn[1] * e.bn[2]), 256, 0, ctx->stream>>>(*a, reinterpret_cast<signed char*>(ctx->volDist.p));
+	VXB_CUDA(ctx, cudaGetLastError());
+	ctx->haveResult = false;
+	return VXB_OK;
+}
+
+int vxb_grid_program_stats(vxb_context* ctx, vxb_program_stats* out)
+{
+	if (!ctx || !out) return VXB_ERR_ARGUMENT;
+	*out = ctx->progStats;
 	return VXB_OK;
 }
 

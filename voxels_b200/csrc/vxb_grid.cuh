@@ -5,8 +5,11 @@
 //   vxb_pack_sizes_kernel / vxb_pack_write_kernel VoxelGrid::CompressBlock + PackForSave                :610-672, :269-315
 // The surfaces are the built-in ones of vxb_surfaces.h (a client callback cannot run on the device); their floats are
 // bit-identical to the CPU adapter's, so the bytes equal what the reference grid store produces for the same surface.
+//   vxb_program_cull_kernel + vxb_program_fill_kernel   Grid::Create with an SDF program (vxb_program.h): block cull, per voxel
+//   vxb_inject_program_kernel                     VoxelGrid::InjectSurface with an SDF program
 #pragma once
 #include "vxb_surfaces.h"
+#include "vxb_program.h"
 
 struct VxbFillArgs
 {
@@ -161,6 +164,146 @@ __global__ void __launch_bounds__(256) vxb_inject_material_kernel(const __grid_c
 			blend[o] = (unsigned char)(v < 0 ? 0 : (v > 255 ? 255 : v));
 		}
 		else { mat[o] = (unsigned char)a.material; blend[o] = (unsigned char)outputBlend; }
+	}
+}
+
+// ---- SDF programs (vxb_program.h): Grid::Create / InjectSurface with a client-composed surface ----------------------
+// The program travels by value as a __grid_constant__ kernel parameter (64 ops = 6 KB): no device buffer and no
+// __constant__ symbol shared between the contexts of one process.
+struct VxbProgram
+{
+	vxb_op ops[VXB_PROGRAM_MAX_OPS];
+	unsigned char perm[VXB_PROGRAM_MAX_TERRAIN][512]; // one table per TERRAIN op, in program order
+	int count;
+};
+
+struct VxbProgramFillArgs
+{
+	VxbProgram prog;
+	float start[3], step;
+	int n;
+	unsigned b0, b1;         // pass A: block ids [b0, b1) (VoxelGrid order, id = x + y nb + z nb^2)
+};
+
+__device__ __forceinline__ void vxb_program_perm_to_smem(const VxbProgram& p, unsigned char* sPerm)
+{
+	for (int i = threadIdx.x; i < VXB_PROGRAM_MAX_TERRAIN * 512; i += blockDim.x) sPerm[i] = p.perm[i >> 9][i & 511];
+	__syncthreads();
+}
+
+// Pass A: one thread per 16^3 block decides (vxp_block_cull, double interval arithmetic) whether every sample quantises to
+// the same +-4 with one primitive's material; the CTA then writes its constant blocks row by row (thread i: row i / cnt of
+// block i % cnt, so that neighbouring threads store neighbouring 16-byte segments of a grid row) and appends the others
+// to `list` for pass B.
+__global__ void __launch_bounds__(256) vxb_program_cull_kernel(const __grid_constant__ VxbProgramFillArgs a, signed char* __restrict__ dist,
+	unsigned char* __restrict__ mat, unsigned char* __restrict__ blend, unsigned* __restrict__ list, unsigned* __restrict__ listCount)
+{
+	__shared__ unsigned sConst[256]; // bit 31: constant block; bits 0-7 distance byte, 8-15 material, 16-23 blend
+	const unsigned nb = (unsigned)a.n >> 4;
+	const unsigned first = a.b0 + blockIdx.x * 256u;
+	const unsigned cnt = min(256u, a.b1 - first);
+	const unsigned t = threadIdx.x;
+	unsigned word = 0;
+	bool listed = false;
+	if (t < cnt)
+	{
+		const unsigned b = first + t;
+		int d;
+		unsigned m, bl;
+		if (vxp_block_cull(a.prog.ops, a.prog.count, a.start, a.step, (int)(b % nb), (int)((b / nb) % nb), (int)(b / (nb * nb)), d, m, bl))
+			word = 0x80000000u | ((unsigned)d & 0xFFu) | (m << 8) | (bl << 16);
+		else listed = true;
+	}
+	sConst[t] = word;
+	const unsigned lane = t & 31u, mask = __ballot_sync(0xFFFFFFFFu, listed);
+	unsigned base = 0;
+	if (lane == 0 && mask) base = atomicAdd(listCount, (unsigned)__popc(mask));
+	base = __shfl_sync(0xFFFFFFFFu, base, 0);
+	if (listed) list[base + __popc(mask & ((1u << lane) - 1u))] = first + t;
+	__syncthreads();
+	const size_t n = (size_t)a.n;
+	for (unsigned i = t; i < 256u * cnt; i += 256u)
+	{
+		const unsigned j = i % cnt, r = i / cnt;
+		const unsigned wv = sConst[j];
+		if (!(wv >> 31)) continue;
+		const unsigned b = first + j;
+		const size_t bx = b % nb, by = (b / nb) % nb, bz = b / (nb * nb);
+		const size_t o = ((bz * 16 + (r >> 4)) * n + by * 16 + (r & 15)) * n + bx * 16;
+		const unsigned dd = (wv & 0xFFu) * 0x01010101u, mm = ((wv >> 8) & 0xFFu) * 0x01010101u, bb = ((wv >> 16) & 0xFFu) * 0x01010101u;
+		*reinterpret_cast<uint4*>(dist + o) = make_uint4(dd, dd, dd, dd);
+		*reinterpret_cast<uint4*>(mat + o) = make_uint4(mm, mm, mm, mm);
+		*reinterpret_cast<uint4*>(blend + o) = make_uint4(bb, bb, bb, bb);
+	}
+}
+
+// Pass B: one CTA per listed block (grid-stride over the list), thread = one 16-voxel row: every thread runs the same op
+// sequence (uniform branches); the row's bytes are collected in 16-byte shift registers and stored once per channel.
+__global__ void __launch_bounds__(256) vxb_program_fill_kernel(const __grid_constant__ VxbProgramFillArgs a, const unsigned* __restrict__ list,
+	const unsigned* __restrict__ listCount, signed char* __restrict__ dist, unsigned char* __restrict__ mat, unsigned char* __restrict__ blend)
+{
+	__shared__ unsigned char sPerm[VXB_PROGRAM_MAX_TERRAIN * 512];
+	vxb_program_perm_to_smem(a.prog, sPerm);
+	const unsigned total = *listCount;
+	const unsigned nb = (unsigned)a.n >> 4;
+	const int y = (int)(threadIdx.x & 15), z = (int)(threadIdx.x >> 4);
+	for (unsigned it = blockIdx.x; it < total; it += gridDim.x)
+	{
+		const unsigned b = list[it];
+		const int bx = (int)(b % nb), by = (int)((b / nb) % nb), bz = (int)(b / (nb * nb));
+		const float fy = vxb_fill_coord(a.start[1], a.step, by * 16 + y), fz = vxb_fill_coord(a.start[2], a.step, bz * 16 + z);
+		uint4 rd = make_uint4(0, 0, 0, 0), rm = rd, rb = rd;
+		for (int k = 0; k < 16; ++k)
+		{
+			const float fx = vxb_fill_coord(a.start[0], a.step, bx * 16 + k);
+			unsigned m, bl;
+			const float d = vxp_eval(a.prog.ops, a.prog.count, sPerm, fx, fy, fz, m, bl);
+			int v = vxs_round_away(d);
+			v = v > 4 ? 4 : (v < -4 ? -4 : v); // toGridDistValue
+			// 16-byte shift registers: after 16 steps byte k holds voxel k
+			rd = make_uint4((rd.x >> 8) | (rd.y << 24), (rd.y >> 8) | (rd.z << 24), (rd.z >> 8) | (rd.w << 24), (rd.w >> 8) | (((unsigned)v & 0xFFu) << 24));
+			rm = make_uint4((rm.x >> 8) | (rm.y << 24), (rm.y >> 8) | (rm.z << 24), (rm.z >> 8) | (rm.w << 24), (rm.w >> 8) | ((m & 0xFFu) << 24));
+			rb = make_uint4((rb.x >> 8) | (rb.y << 24), (rb.y >> 8) | (rb.z << 24), (rb.z >> 8) | (rb.w << 24), (rb.w >> 8) | ((bl & 0xFFu) << 24));
+		}
+		const size_t o = (((size_t)bz * 16 + z) * a.n + (size_t)by * 16 + y) * a.n + (size_t)bx * 16;
+		*reinterpret_cast<uint4*>(dist + o) = rd;
+		*reinterpret_cast<uint4*>(mat + o) = rm;
+		*reinterpret_cast<uint4*>(blend + o) = rb;
+	}
+}
+
+struct VxbProgramEditArgs
+{
+	VxbProgram prog;
+	float position[3], extents[3];
+	int type, n;
+	int b0[3], bn[3];        // first touched block and number of touched blocks per axis (prepareEdit)
+};
+
+// vxb_inject_surface_kernel with a program: one CTA per touched block, no cull pass (edit boxes are small)
+__global__ void __launch_bounds__(256) vxb_inject_program_kernel(const __grid_constant__ VxbProgramEditArgs a, signed char* __restrict__ dist)
+{
+	__shared__ unsigned char sPerm[VXB_PROGRAM_MAX_TERRAIN * 512];
+	vxb_program_perm_to_smem(a.prog, sPerm);
+	const int bx = a.b0[0] + (int)(blockIdx.x % a.bn[0]), by = a.b0[1] + (int)((blockIdx.x / a.bn[0]) % a.bn[1]), bz = a.b0[2] + (int)(blockIdx.x / (a.bn[0] * a.bn[1]));
+	const float base[3] = { (float)(bx * 16), (float)(by * 16), (float)(bz * 16) };
+	float start[3]; int cnt[3];
+	for (int k = 0; k < 3; ++k) vxb_edit_section(a.position[k], a.extents[k], base[k], start[k], cnt[k]);
+	const int total = cnt[0] * cnt[1] * cnt[2];
+	const float s0[3] = { base[0] + start[0] - a.position[0], base[1] + start[1] - a.position[1], base[2] + start[2] - a.position[2] };
+	for (int i = threadIdx.x; i < total; i += blockDim.x)
+	{
+		const int kx = i % cnt[0], ky = (i / cnt[0]) % cnt[1], kz = i / (cnt[0] * cnt[1]);
+		const unsigned vx = (unsigned)(start[0] + (float)kx), vy = (unsigned)(start[1] + (float)ky), vz = (unsigned)(start[2] + (float)kz);
+		unsigned m, bl;
+		const float sv = vxp_eval(a.prog.ops, a.prog.count, sPerm, s0[0] + (float)kx, s0[1] + (float)ky, s0[2] + (float)kz, m, bl);
+		const size_t o = ((size_t)(bz * 16 + vz) * a.n + (by * 16 + vy)) * a.n + (bx * 16 + vx);
+		const float value = (float)dist[o];
+		float f;
+		if (a.type == 0) f = fminf(value, sv);            // IT_Add            :443
+		else if (a.type == 1) f = fmaxf(value, sv);       // IT_SubtractAddInner :446
+		else f = fmaxf(-sv, value);                       // IT_Subtract       :449
+		dist[o] = (signed char)vxs_round_away(f);         // no +-4 clamp here (:441-452)
 	}
 }
 

@@ -245,6 +245,10 @@ class ShardedGrid:
         """Grid::Create(..., &surface) on the device: the whole grid (replicated) or this rank's pieces (cube)."""
         self.ctx.fill(self.n, surface, start, step)
 
+    def fill_program(self, ops, start=(0.0, 0.0, 0.0), step=1.0):
+        """fill() with an SDF program (a list of capi.Op): the whole grid (replicated) or this rank's pieces (cube)."""
+        self.ctx.fill_program(self.n, ops, start, step)
+
     def upload_packed(self, blob_ptr, nbytes):
         """The grid's PackForSave bytes from (pinned) host memory: decoded on the GPU, whole (replicated) or this rank's pieces."""
         self.ctx.upload_packed(blob_ptr, nbytes)
