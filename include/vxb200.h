@@ -257,7 +257,7 @@ typedef struct vxb_region_info
  * MaxCornerModified, OUTPUT coordinates: the box Grid::InjectSurface returns).  Needs a preceding full vxb_polygonize of
  * the same context: its consistency / material caches are updated in place exactly like the reference's PolygonMap
  * caches (bits are only ever set, votes only overwrite), block ids continue the context's running counter.  The
- * result (vxb_result_info / vxb_result_download) holds ONLY the re-created blocks. */
+ * result (vxb_result_info / vxb_result_download) holds ONLY the re-created blocks; a vxb_mesh keeps the whole surface. */
 int vxb_polygonize_region(vxb_context* ctx, const float min_corner[3], const float max_corner[3], uint32_t flags);
 int vxb_region_info_get(vxb_context* ctx, vxb_region_info* out);
 
@@ -359,6 +359,60 @@ int vxb_result_device_arenas(vxb_context* ctx, const void** vertices, const uint
 int vxb_result_select_lod(vxb_context* ctx, const float camera[3], float base_distance, vxb_draw_lists* out);
 /* the two lists copied to HOST memory (tests, debugging); capacities in entries, any pointer may be NULL */
 int vxb_result_download_draws(vxb_context* ctx, vxb_draw_command* regular, vxb_draw_info* regular_info, vxb_draw_command* transition, vxb_draw_info* transition_info);
+
+/* ---- the mesh: the polygonized surface kept resident in HBM across edits -------------------------------------------------
+ * The context's result holds what the LAST run made: after vxb_polygonize_region only the re-created blocks.  A mesh keeps
+ * the whole surface: vxb_mesh_apply takes the context's last run into it on the GPU, in the reference's block order
+ * (PolygonMap::Levels[l].Blocks after Execute, TransVoxelImpl.cpp:395-401, :443-450, :1293):
+ *   after vxb_polygonize          the content is replaced by the run's blocks, per level in coord_id order
+ *   after vxb_polygonize_region   per level, the blocks whose block coordinates lie in the run's dirty range (the box of
+ *                                 vxb_region_info.min_dirty / max_dirty) are erased, the survivors keep their order and
+ *                                 the re-created blocks follow them in coord_id order
+ * The mesh copies (it never aliases the context's arenas; vxb_result_* behave as without it).  Vertices are the bytes of
+ * vxb_result_download: unmapped materials have all-zero textures.  Block ids are the context's.  An apply is refused with
+ * VXB_ERR_STATE, leaving the mesh untouched, when the context has no result, when the result is a sharded run's, when that
+ * run was already applied, and for a region run when the mesh missed one of the context's runs since its last full run.
+ * Every block's index ranges start at a multiple of 4 indices (16-byte aligned); the arenas also hold the ranges of erased
+ * blocks until the next compaction (when the tail would overflow, or when the garbage exceeds the live data, the live
+ * blocks are copied into a second arena set, grown to 1.5 x the live data when needed).  Pointers from
+ * vxb_mesh_device_arenas and vxb_mesh_select_lod stay valid until an apply changes `generation`.  vxb_destroy releases the
+ * context's meshes. */
+typedef struct vxb_mesh vxb_mesh;
+/* capacity: initial arena capacities in elements {vertices, indices, trans vertices, trans indices}; NULL = sized by the
+ * first apply */
+int vxb_mesh_create(vxb_context* ctx, const uint64_t capacity[4], vxb_mesh** out);
+void vxb_mesh_destroy(vxb_mesh* mesh);
+int vxb_mesh_apply(vxb_mesh* mesh);
+typedef struct vxb_mesh_info
+{
+	uint32_t levels;              /* LOD levels of the grid the mesh was built from */
+	uint32_t block_count;
+	uint32_t level_blocks[12];    /* blocks per level */
+	uint64_t vertex_span;         /* download sizes: the used prefix of each arena (elements) */
+	uint64_t index_span;
+	uint64_t trans_vertex_span;
+	uint64_t trans_index_span;
+	uint64_t vertex_total;        /* live elements over all blocks */
+	uint64_t index_total;
+	uint64_t trans_vertex_total;
+	uint64_t trans_index_total;
+	uint64_t capacity[4];         /* arena capacities in elements */
+	uint32_t stats[20];           /* vxb_result_info.stats of the last applied run (PolygonMap::Stats after it) */
+	uint32_t compactions;         /* applies that copied the live blocks into the second arena set */
+	uint32_t growths;             /* applies that enlarged the arenas */
+	uint64_t generation;          /* changes whenever the directory or an arena moves (growth, compaction) */
+	uint64_t bytes_copied;        /* device bytes the last apply wrote into the mesh (arenas and directory) */
+	float apply_ms;               /* device time of the last apply (CUDA events) */
+	uint32_t pad;
+} vxb_mesh_info;
+int vxb_mesh_info_get(vxb_mesh* mesh, vxb_mesh_info* out);
+/* The directory in mesh order (level ascending, then surface order) and the used prefix of each arena (spans of
+ * vxb_mesh_info) to HOST memory; any pointer may be NULL. */
+int vxb_mesh_download(vxb_mesh* mesh, vxb_block_record* records, void* vertices, uint32_t* indices, void* trans_vertices, uint32_t* trans_indices);
+int vxb_mesh_device_arenas(vxb_mesh* mesh, const vxb_block_record** records, const void** vertices, const uint32_t** indices,
+	const void** trans_vertices, const uint32_t** trans_indices);
+/* vxb_result_select_lod over the mesh's blocks; the lists are the mesh's own (the context's stay as they are) */
+int vxb_mesh_select_lod(vxb_mesh* mesh, const float camera[3], float base_distance, vxb_draw_lists* out);
 
 /* GetMaterial(id) == nullptr handling (TransVoxelImpl.cpp:1364-1368: textures stay zero, one LS_Error log per
  * vertex): after vxb_result_download the material ids of those vertices, in the reference's logging order

@@ -164,10 +164,21 @@ DRAW_COMMAND_DTYPE = np.dtype([("index_count", "<u4"), ("instance_count", "<u4")
 DRAW_INFO_DTYPE = np.dtype([("block_id", "<u4"), ("level", "<u4"), ("block_adj", "<u4"), ("face", "<u4")])
 
 
+class MeshInfo(C.Structure):
+    """vxb_mesh_info (include/vxb200.h)."""
+    _fields_ = [("levels", C.c_uint32), ("block_count", C.c_uint32), ("level_blocks", C.c_uint32 * 12), ("vertex_span", C.c_uint64),
+                ("index_span", C.c_uint64), ("trans_vertex_span", C.c_uint64), ("trans_index_span", C.c_uint64),
+                ("vertex_total", C.c_uint64), ("index_total", C.c_uint64), ("trans_vertex_total", C.c_uint64),
+                ("trans_index_total", C.c_uint64), ("capacity", C.c_uint64 * 4), ("stats", C.c_uint32 * 20),
+                ("compactions", C.c_uint32), ("growths", C.c_uint32), ("generation", C.c_uint64), ("bytes_copied", C.c_uint64),
+                ("apply_ms", C.c_float), ("pad", C.c_uint32)]
+
+
 class NcclId(C.Structure):
     _fields_ = [("internal", C.c_char * 128)]
 
 
+ERR_STATE = -3
 ERR_CAPACITY = -4
 
 # vxb_pack_producer (include/vxb200.h): void (*)(void* user, uint32_t layer0, uint32_t layer1)
@@ -256,6 +267,13 @@ def load_library():
         "vxb_set_launch_limit": (C.c_int, [vp, u32]),
         "vxb_kernel_ms": (C.c_int, [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(u32)]),
         "vxb_result_unmapped_materials": (u64, [vp, vp, u64]),
+        "vxb_mesh_create": (C.c_int, [vp, vp, C.POINTER(vp)]),
+        "vxb_mesh_destroy": (None, [vp]),
+        "vxb_mesh_apply": (C.c_int, [vp]),
+        "vxb_mesh_info_get": (C.c_int, [vp, C.POINTER(MeshInfo)]),
+        "vxb_mesh_download": (C.c_int, [vp, vp, vp, vp, vp, vp]),
+        "vxb_mesh_device_arenas": (C.c_int, [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
+        "vxb_mesh_select_lod": (C.c_int, [vp, vp, C.c_float, C.POINTER(DrawLists)]),
         "vxb_host_alloc": (vp, [C.c_size_t]),
         "vxb_host_free": (None, [vp]),
     }
@@ -274,7 +292,9 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_shard_nccl_init", "vxb_grid_fill", "vxb_grid_inject_surface", "vxb_grid_inject_material", "vxb_grid_pack",
                     "vxb_grid_download_dense", "vxb_result_device_arenas", "vxb_result_select_lod", "vxb_result_download_draws", "vxb_cube_create", "vxb_cube_info", "vxb_cube_export", "vxb_cube_import", "vxb_cube_piece",
                     "vxb_grid_upload_packed_streamed", "vxb_result_download_begin", "vxb_result_download_end",
-                    "vxb_grid_fill_program", "vxb_grid_inject_program", "vxb_grid_program_stats"]
+                    "vxb_grid_fill_program", "vxb_grid_inject_program", "vxb_grid_program_stats",
+                    "vxb_mesh_create", "vxb_mesh_destroy", "vxb_mesh_apply", "vxb_mesh_info_get", "vxb_mesh_download",
+                    "vxb_mesh_device_arenas", "vxb_mesh_select_lod"]
 
 
 def nccl_unique_id():
@@ -366,6 +386,74 @@ def merge_results(results):
     return merged
 
 
+def _device_to_numpy(ptr, count, dtype):
+    """`count` elements of `dtype` at a device address, copied to a numpy array (through torch)."""
+    import torch
+    out = np.zeros(count, dtype)
+    if count:
+        t = torch.as_tensor(DevicePointer(ptr, count * dtype.itemsize), device=torch.device("cuda", torch.cuda.current_device()))
+        out.view(np.uint8)[:] = t.cpu().numpy()
+    return out
+
+
+class Mesh:
+    """vxb_mesh: the polygonized surface kept in HBM across edits (include/vxb200.h "mesh").  apply() after every run of the
+    context (full or region) splices the run into the mesh on the GPU in the reference's block order."""
+
+    def __init__(self, ctx, capacity=None):
+        self.ctx, self.L = ctx, ctx.L
+        h = C.c_void_p()
+        cap = None if capacity is None else (C.c_uint64 * 4)(*capacity)
+        ctx._check(self.L.vxb_mesh_create(ctx.h, cap, C.byref(h)), "vxb_mesh_create")
+        self.h = h
+        ctx._meshes.append(self)
+
+    def close(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            self.L.vxb_mesh_destroy(self.h)
+            self.ctx._meshes.remove(self)
+        self.h = None
+
+    def apply_rc(self):
+        """vxb_mesh_apply's return code (0, or ERR_STATE when the apply is refused)."""
+        return self.L.vxb_mesh_apply(self.h)
+
+    def apply(self):
+        self.ctx._check(self.apply_rc(), "vxb_mesh_apply")
+        return self.info()
+
+    def info(self):
+        i = MeshInfo()
+        self.ctx._check(self.L.vxb_mesh_info_get(self.h, C.byref(i)), "vxb_mesh_info_get")
+        return i
+
+    def download(self):
+        """The directory in mesh order and the used prefix of each arena, as a Result (Result.level(l) = surface order)."""
+        info = self.info()
+        records = np.zeros(info.block_count, RECORD_DTYPE)
+        verts = np.zeros(info.vertex_span, VERTEX_DTYPE); idx = np.zeros(info.index_span, np.uint32)
+        tverts = np.zeros(info.trans_vertex_span, VERTEX_DTYPE); tidx = np.zeros(info.trans_index_span, np.uint32)
+        self.ctx._check(self.L.vxb_mesh_download(self.h, _ptr(records), _ptr(verts), _ptr(idx), _ptr(tverts), _ptr(tidx)), "vxb_mesh_download")
+        return Result(self.ctx.n, info, records, verts, idx, tverts, tidx)
+
+    def device_arenas(self):
+        """(records, vertices, indices, trans vertices, trans indices) device addresses."""
+        p = [C.c_void_p() for _ in range(5)]
+        self.ctx._check(self.L.vxb_mesh_device_arenas(self.h, *[C.byref(x) for x in p]), "vxb_mesh_device_arenas")
+        return tuple(x.value for x in p)
+
+    def select_lod(self, camera, base_distance, lists_out=None):
+        """(regular commands, regular infos, transition commands, transition infos) copied to numpy; the device-resident
+        vxb_draw_lists go to `lists_out` (a DrawLists) when given."""
+        cam = np.ascontiguousarray(camera, np.float32)
+        lists = DrawLists() if lists_out is None else lists_out
+        self.ctx._check(self.L.vxb_mesh_select_lod(self.h, _ptr(cam), base_distance, C.byref(lists)), "vxb_mesh_select_lod")
+        return (_device_to_numpy(lists.regular, lists.regular_count, DRAW_COMMAND_DTYPE),
+                _device_to_numpy(lists.regular_info, lists.regular_count, DRAW_INFO_DTYPE),
+                _device_to_numpy(lists.transition, lists.transition_count, DRAW_COMMAND_DTYPE),
+                _device_to_numpy(lists.transition_info, lists.transition_count, DRAW_INFO_DTYPE))
+
+
 class Context:
     """vxb_context wrapper.  Raises VxbError on any failure (no CUDA device included)."""
 
@@ -378,11 +466,19 @@ class Context:
         self.h = h
         self.n = 0
         self._keep = None
+        self._meshes = []
 
     def close(self):
         if getattr(self, "h", None):
+            for m in self._meshes:   # vxb_destroy releases them
+                m.h = None
+            self._meshes = []
             self.L.vxb_destroy(self.h)
             self.h = None
+
+    def mesh(self, capacity=None):
+        """A device-resident mesh of this context (capacity: {vertices, indices, trans vertices, trans indices} or None)."""
+        return Mesh(self, capacity)
 
     def __del__(self):
         try:

@@ -30,6 +30,7 @@
 #include "vxb_emit.cuh"
 #include "vxb_grid.cuh"
 #include "vxb_draw.cuh"
+#include "vxb_mesh.cuh"
 
 static_assert(sizeof(VxbVertex) == 48, "PolygonVertex layout");
 static_assert(sizeof(vxb_block_record) == 128, "record layout");
@@ -183,6 +184,9 @@ struct vxb_context
 	size_t validBytes = 0;
 
 	bool haveResult = false;
+	uint64_t runSerial = 0;                 // counts the runs (vxb_polygonize*), so that a mesh can tell whether it missed one
+	bool resultSharded = false, resultRegion = false;
+	std::vector<vxb_mesh*> meshes;          // released by vxb_destroy
 	vxb_result_info info;
 	std::vector<vxb_block_record> sortedRecords;
 	uint8_t lutValid[256];
@@ -683,6 +687,7 @@ void vxb_destroy(vxb_context* ctx)
 {
 	if (!ctx) return;
 	cudaSetDevice(ctx->device);
+	for (vxb_mesh* m : std::vector<vxb_mesh*>(ctx->meshes)) vxb_mesh_destroy(m);
 	if (ctx->stream) cudaStreamSynchronize(ctx->stream);
 	if (ctx->stream2) cudaStreamSynchronize(ctx->stream2);
 	if (ctx->graphExec) cudaGraphExecDestroy(ctx->graphExec);
@@ -1287,6 +1292,7 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 	if (ctx->downloadOpen) return fail(ctx, VXB_ERR_STATE, "vxb_polygonize: a result download is open (vxb_result_download_end first)");
 	cudaSetDevice(ctx->device);
 	ctx->haveResult = false;
+	++ctx->runSerial;
 	const uint32_t n = ctx->n;
 	const int levels = ctx->levels;
 	const int computed = (maxLevels == 0 || (int)maxLevels > levels) ? levels : (int)maxLevels;
@@ -1714,6 +1720,7 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 	for (int i = 0; i < 16; ++i) info.stats[4 + i] = hc.perCase[i];
 	for (int i = 0; i < 8; ++i) info.used_materials[i] = hc.usedMaterials[i];
 	ctx->haveResult = true;
+	ctx->resultSharded = sharded; ctx->resultRegion = region != nullptr;
 	if (!region && !sharded) { ctx->haveFullRun = (computed == levels); ctx->nextId = (uint32_t)totalBlocks; }
 	else if (sharded) ctx->haveFullRun = false;
 	return VXB_OK;
@@ -2049,33 +2056,50 @@ int vxb_result_device_arenas(vxb_context* ctx, const void** vertices, const uint
 	return VXB_OK;
 }
 
+} // extern "C"
+
+namespace
+{
+// vxb_lod_select_kernel over `blocks` records of d.records into the given lists (sized to `cap` blocks)
+int selectLod(vxb_context* ctx, const VxbDev& d, uint32_t blocks, size_t cap, const float camera[3], float baseDistance,
+	DevBuf<vxb_draw_command>& cmd, DevBuf<vxb_draw_info>& info, DevBuf<vxb_draw_command>& tcmd, DevBuf<vxb_draw_info>& tinfo,
+	DevBuf<unsigned int>& counts, vxb_draw_lists& l)
+{
+	VXB_CUDA(ctx, cmd.ensure(cap)); VXB_CUDA(ctx, info.ensure(cap));
+	VXB_CUDA(ctx, tcmd.ensure(cap * 6)); VXB_CUDA(ctx, tinfo.ensure(cap * 6));
+	VXB_CUDA(ctx, counts.ensure(2));
+	VXB_CUDA(ctx, cudaMemsetAsync(counts.p, 0, 8, ctx->stream));
+	VxbLodArgs a;
+	for (int k = 0; k < 3; ++k) a.camera[k] = camera[k];
+	a.baseDistance = baseDistance;
+	a.counts = counts.p;
+	a.regular = cmd.p; a.regularInfo = info.p; a.transition = tcmd.p; a.transitionInfo = tinfo.p;
+	a.capacity = (unsigned)(cap * 6);
+	if (blocks) vxb_lod_select_kernel<<<(blocks + 255) / 256, 256, 0, ctx->stream>>>(d, a, blocks);
+	unsigned n[2] = { 0, 0 };
+	VXB_CUDA(ctx, cudaMemcpyAsync(n, counts.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+	VXB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	VXB_CUDA(ctx, cudaGetLastError());
+	l.regular_count = n[0]; l.transition_count = n[1];
+	l.counts = counts.p;
+	l.regular = cmd.p; l.regular_info = info.p; l.transition = tcmd.p; l.transition_info = tinfo.p;
+	return VXB_OK;
+}
+}
+
+extern "C"
+{
+
 int vxb_result_select_lod(vxb_context* ctx, const float camera[3], float baseDistance, vxb_draw_lists* out)
 {
 	if (!ctx || !camera) return VXB_ERR_ARGUMENT;
 	if (!ctx->haveResult) return fail(ctx, VXB_ERR_STATE, "no result: call vxb_polygonize first");
 	cudaSetDevice(ctx->device);
 	const uint32_t blocks = ctx->info.block_count;
-	const size_t cap = blocks ? blocks : 1;
-	VXB_CUDA(ctx, ctx->drawCmd.ensure(cap)); VXB_CUDA(ctx, ctx->drawInfo.ensure(cap));
-	VXB_CUDA(ctx, ctx->drawTCmd.ensure(cap * 6)); VXB_CUDA(ctx, ctx->drawTInfo.ensure(cap * 6));
-	VXB_CUDA(ctx, ctx->drawCounts.ensure(2));
-	VXB_CUDA(ctx, cudaMemsetAsync(ctx->drawCounts.p, 0, 8, ctx->stream));
-	VxbLodArgs a;
-	for (int k = 0; k < 3; ++k) a.camera[k] = camera[k];
-	a.baseDistance = baseDistance;
-	a.counts = ctx->drawCounts.p;
-	a.regular = ctx->drawCmd.p; a.regularInfo = ctx->drawInfo.p; a.transition = ctx->drawTCmd.p; a.transitionInfo = ctx->drawTInfo.p;
-	a.capacity = (unsigned)(cap * 6);
-	if (blocks) vxb_lod_select_kernel<<<(blocks + 255) / 256, 256, 0, ctx->stream>>>(ctx->lastDev, a, blocks);
-	unsigned counts[2] = { 0, 0 };
-	VXB_CUDA(ctx, cudaMemcpyAsync(counts, ctx->drawCounts.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
-	VXB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	VXB_CUDA(ctx, cudaGetLastError());
-	vxb_draw_lists& l = ctx->drawLists;
-	l.regular_count = counts[0]; l.transition_count = counts[1];
-	l.counts = ctx->drawCounts.p;
-	l.regular = ctx->drawCmd.p; l.regular_info = ctx->drawInfo.p; l.transition = ctx->drawTCmd.p; l.transition_info = ctx->drawTInfo.p;
-	if (out) *out = l;
+	const int r = selectLod(ctx, ctx->lastDev, blocks, blocks ? blocks : 1, camera, baseDistance, ctx->drawCmd, ctx->drawInfo, ctx->drawTCmd,
+		ctx->drawTInfo, ctx->drawCounts, ctx->drawLists);
+	if (r != VXB_OK) return r;
+	if (out) *out = ctx->drawLists;
 	return VXB_OK;
 }
 
@@ -2113,6 +2137,308 @@ int vxb_kernel_ms(vxb_context* ctx, int which, float* ms, uint32_t* launches)
 	if (!ctx || which < 0 || which > 9) return VXB_ERR_ARGUMENT;
 	if (ms) *ms = ctx->kindMs[which];
 	if (launches) *launches = ctx->kindLaunches[which];
+	return VXB_OK;
+}
+
+} // extern "C"
+
+// ---- the mesh (include/vxb200.h "mesh"; kernels: vxb_mesh.cuh) ----
+struct vxb_mesh
+{
+	vxb_context* ctx = nullptr;
+	struct Arenas
+	{
+		DevBuf<VxbVertex> v, tv;
+		DevBuf<unsigned int> i, ti;
+		VxbMeshArenas view() const { VxbMeshArenas a; a.v = v.p; a.i = i.p; a.tv = tv.p; a.ti = ti.p; return a; }
+		cudaError_t ensure(const uint64_t cap[4])
+		{
+			cudaError_t e = v.ensure(cap[0]);
+			if (e == cudaSuccess) e = i.ensure(cap[1]);
+			if (e == cudaSuccess) e = tv.ensure(cap[2]);
+			if (e == cudaSuccess) e = ti.ensure(cap[3]);
+			return e;
+		}
+		void release() { v.release(); i.release(); tv.release(); ti.release(); }
+	} set[2];                                   // set[active] holds the mesh; the other one is the target of a compaction
+	int active = 0;
+	uint64_t cap[4] = { 0, 0, 0, 0 }, span[4] = { 0, 0, 0, 0 }, total[4] = { 0, 0, 0, 0 };
+	DevBuf<vxb_block_record> dir, scratch;      // the directory, and the merged one an apply writes before it replaces it
+	size_t dirCap = 0;                          // every (level, coord) slot of the grid: a mesh holds each block at most once
+	DevBuf<unsigned int> keys, vals, keysOut, valsOut, jobSrc, jobDst;
+	DevBuf<VxbMeshScan> items, prefix;
+	DevBuf<unsigned char> cubTemp;
+	DevBuf<VxbMeshCounts> counts;
+	DevBuf<vxb_draw_command> drawCmd, drawTCmd;
+	DevBuf<vxb_draw_info> drawInfo, drawTInfo;
+	DevBuf<unsigned int> drawCounts;
+	vxb_draw_lists drawLists;
+	cudaEvent_t ev[2] = { nullptr, nullptr };
+	bool content = false;                       // a run has been applied
+	uint64_t serial = 0;                        // vxb_context::runSerial of that run
+	uint32_t n = 0;
+	vxb_mesh_info info;
+};
+
+namespace
+{
+void releaseMesh(vxb_mesh* m)
+{
+	for (vxb_mesh::Arenas& a : m->set) a.release();
+	m->dir.release(); m->scratch.release();
+	m->keys.release(); m->vals.release(); m->keysOut.release(); m->valsOut.release(); m->jobSrc.release(); m->jobDst.release();
+	m->items.release(); m->prefix.release(); m->cubTemp.release(); m->counts.release();
+	m->drawCmd.release(); m->drawTCmd.release(); m->drawInfo.release(); m->drawTInfo.release(); m->drawCounts.release();
+	for (cudaEvent_t e : m->ev) if (e) cudaEventDestroy(e);
+}
+
+uint64_t grownCapacity(uint64_t live) { return (std::max<uint64_t>(live + live / 2, 1024) + 3) & ~(uint64_t)3; }
+}
+
+extern "C"
+{
+
+int vxb_mesh_create(vxb_context* ctx, const uint64_t capacity[4], vxb_mesh** out)
+{
+	if (!ctx || !out) return VXB_ERR_ARGUMENT;
+	*out = nullptr;
+	cudaSetDevice(ctx->device);
+	vxb_mesh* m = new vxb_mesh;
+	m->ctx = ctx;
+	memset(&m->info, 0, sizeof(m->info));
+	memset(&m->drawLists, 0, sizeof(m->drawLists));
+	cudaError_t e = cudaEventCreate(&m->ev[0]);
+	if (e == cudaSuccess) e = cudaEventCreate(&m->ev[1]);
+	if (e == cudaSuccess && capacity)
+	{
+		for (int a = 0; a < 4; ++a) m->cap[a] = (capacity[a] + 3) & ~(uint64_t)3;
+		e = m->set[0].ensure(m->cap);
+	}
+	if (e != cudaSuccess) { releaseMesh(m); delete m; return fail(ctx, VXB_ERR_CUDA, "vxb_mesh_create", e); }
+	ctx->meshes.push_back(m);
+	*out = m;
+	return VXB_OK;
+}
+
+void vxb_mesh_destroy(vxb_mesh* m)
+{
+	if (!m) return;
+	vxb_context* ctx = m->ctx;
+	cudaSetDevice(ctx->device);
+	cudaStreamSynchronize(ctx->stream);
+	ctx->meshes.erase(std::remove(ctx->meshes.begin(), ctx->meshes.end(), m), ctx->meshes.end());
+	releaseMesh(m);
+	delete m;
+}
+
+int vxb_mesh_apply(vxb_mesh* m)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!ctx->haveResult) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_apply: no result: call vxb_polygonize first");
+	if (ctx->resultSharded) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_apply: the result is a sharded run's (a mesh takes single-context runs)");
+	if (m->content && m->serial == ctx->runSerial) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_apply: this run was already applied");
+	const bool region = ctx->resultRegion;
+	if (region && !(m->content && m->serial + 1 == ctx->runSerial))
+		return fail(ctx, VXB_ERR_STATE, "vxb_mesh_apply: the mesh missed a run of the context since its last full run (apply every run, or start again from a full run)");
+	cudaSetDevice(ctx->device);
+	cudaStream_t st = ctx->stream;
+	const uint32_t n = ctx->n;
+	const int levels = ctx->levels;
+
+	// ---- buffers: every (level, coord) slot of the grid; a new grid size moves the directory ----
+	VxbMeshRange g;
+	memset(&g, 0, sizeof(g));
+	g.erase = region ? 1 : 0;
+	size_t slots = 0;
+	for (int l = 0; l < levels; ++l)
+	{
+		g.levelBase[l] = (unsigned)slots; slots += blocksAtLevel(n, l);
+		g.nb[l] = (int)((n >> 4) >> l);
+		if (region)
+		{
+			// the dirty box in OUTPUT axes (x, z, y) and block units; its corners are multiples of the block size
+			const float m3 = (float)((1 << l) * 16);
+			const float* lo = ctx->region.min_dirty[l]; const float* hi = ctx->region.max_dirty[l];
+			g.lo[l][0] = (int)(lo[0] / m3); g.lo[l][1] = (int)(lo[2] / m3); g.lo[l][2] = (int)(lo[1] / m3);
+			g.hi[l][0] = (int)(hi[0] / m3); g.hi[l][1] = (int)(hi[2] / m3); g.hi[l][2] = (int)(hi[1] / m3);
+		}
+	}
+	if (slots > m->dirCap)
+	{
+		VXB_CUDA(ctx, m->dir.ensure(slots)); VXB_CUDA(ctx, m->scratch.ensure(slots));
+		VXB_CUDA(ctx, m->drawCmd.ensure(slots)); VXB_CUDA(ctx, m->drawInfo.ensure(slots));
+		VXB_CUDA(ctx, m->drawTCmd.ensure(slots * 6)); VXB_CUDA(ctx, m->drawTInfo.ensure(slots * 6));
+		VXB_CUDA(ctx, m->drawCounts.ensure(2));
+		m->dirCap = slots;
+		++m->info.generation;
+	}
+	VXB_CUDA(ctx, m->keys.ensure(slots)); VXB_CUDA(ctx, m->vals.ensure(slots));
+	VXB_CUDA(ctx, m->keysOut.ensure(slots)); VXB_CUDA(ctx, m->valsOut.ensure(slots));
+	VXB_CUDA(ctx, m->jobSrc.ensure(slots * 2)); VXB_CUDA(ctx, m->jobDst.ensure(slots * 2));
+	VXB_CUDA(ctx, m->items.ensure(slots * 2)); VXB_CUDA(ctx, m->prefix.ensure(slots * 2));
+	VXB_CUDA(ctx, m->counts.ensure(1));
+
+	const unsigned meshCount = region ? m->info.block_count : 0, runCount = ctx->info.block_count, all = meshCount + runCount;
+	int sortBits = 1;
+	while (sortBits < 32 && ((size_t)1 << sortBits) < slots) ++sortBits;
+	size_t sortBytes = 0, scanBytes = 0;
+	VXB_CUDA(ctx, cub::DeviceRadixSort::SortPairs(nullptr, sortBytes, m->keys.p, m->keysOut.p, m->vals.p, m->valsOut.p, (int)runCount, 0, sortBits, st));
+	VXB_CUDA(ctx, cub::DeviceScan::ExclusiveScan(nullptr, scanBytes, m->items.p, m->prefix.p, VxbMeshScanSum(), VxbMeshScan{ 0, 0, 0, 0, 0 }, (int)all, st));
+	size_t tempBytes = std::max<size_t>(std::max(sortBytes, scanBytes), 1);
+	VXB_CUDA(ctx, m->cubTemp.ensure(tempBytes));
+	tempBytes = m->cubTemp.count;
+
+	// ---- count, sort the run's records by (level, coord_id), read the totals ----
+	VXB_CUDA(ctx, cudaEventRecord(m->ev[0], st));
+	VXB_CUDA(ctx, cudaMemsetAsync(m->counts.p, 0, sizeof(VxbMeshCounts), st));
+	if (all)
+		vxb_mesh_count_kernel<<<(all + 255) / 256, 256, 0, st>>>(m->dir.p, meshCount, ctx->records.p, runCount, g, m->items.p, m->keys.p, m->vals.p, m->counts.p);
+	if (runCount)
+	{
+		VXB_CUDA(ctx, cub::DeviceRadixSort::SortPairs(m->cubTemp.p, tempBytes, m->keys.p, m->keysOut.p, m->vals.p, m->valsOut.p, (int)runCount, 0, sortBits, st));
+		vxb_mesh_gather_kernel<<<(runCount + 255) / 256, 256, 0, st>>>(ctx->records.p, m->valsOut.p, runCount, m->items.p + meshCount);
+	}
+	VXB_CUDA(ctx, cudaGetLastError());
+	VxbMeshCounts c;
+	VXB_CUDA(ctx, cudaMemcpyAsync(&c, m->counts.p, sizeof(c), cudaMemcpyDeviceToHost, st));
+	VXB_CUDA(ctx, cudaStreamSynchronize(st));
+
+	// ---- where the blocks go: the tail of the active set, or a compaction into the other one ----
+	uint64_t live[4], newCap[4], tail[4];
+	bool compact = false, grow = false;
+	for (int a = 0; a < 4; ++a)
+	{
+		live[a] = c.survivorElems[a] + c.freshElems[a];
+		tail[a] = region ? m->span[a] : 0;
+		newCap[a] = live[a] > m->cap[a] ? grownCapacity(live[a]) : m->cap[a];
+		grow = grow || newCap[a] != m->cap[a];
+		if (region && (tail[a] + c.freshElems[a] > m->cap[a] || tail[a] - c.survivorElems[a] > live[a])) compact = true;
+	}
+	if (tail[0] > 0xFFFFFFFFull || tail[1] > 0xFFFFFFFFull || tail[2] > 0xFFFFFFFFull || tail[3] > 0xFFFFFFFFull ||
+		newCap[0] > 0xFFFFFFFFull || newCap[1] > 0xFFFFFFFFull || newCap[2] > 0xFFFFFFFFull || newCap[3] > 0xFFFFFFFFull)
+		return fail(ctx, VXB_ERR_CAPACITY, "vxb_mesh_apply: the mesh outgrows 32-bit arena offsets");
+	const bool hadArenas = m->cap[0] || m->cap[1] || m->cap[2] || m->cap[3];
+	int target = m->active;
+	if (compact)
+	{
+		target = 1 - m->active;
+		VXB_CUDA(ctx, m->set[target].ensure(newCap));
+	}
+	else if (grow)
+	{
+		// a full apply replaces the content: the active set is simply reallocated
+		m->set[m->active].release();
+		VXB_CUDA(ctx, m->set[m->active].ensure(newCap));
+	}
+	for (int a = 0; a < 4; ++a) { if (compact || !region) tail[a] = 0; }
+
+	bool anyUnmapped = false;
+	for (unsigned i = 0; i < 256; ++i) if (!ctx->lutValid[i] && ((ctx->info.used_materials[i >> 5] >> (i & 31)) & 1u)) anyUnmapped = true;
+
+	if (all)
+	{
+		VXB_CUDA(ctx, cub::DeviceScan::ExclusiveScan(m->cubTemp.p, tempBytes, m->items.p, m->prefix.p, VxbMeshScanSum(), VxbMeshScan{ 0, 0, 0, 0, 0 }, (int)all, st));
+		const uint4 t4 = make_uint4((unsigned)tail[0], (unsigned)tail[1], (unsigned)tail[2], (unsigned)tail[3]);
+		vxb_mesh_place_kernel<<<(all + 255) / 256, 256, 0, st>>>(m->dir.p, meshCount, ctx->records.p, m->valsOut.p, runCount, g, m->prefix.p,
+			m->counts.p, t4, compact ? 1 : 0, m->scratch.p, m->jobSrc.p, m->jobDst.p);
+	}
+	unsigned survivors = 0, fresh = 0;
+	for (int l = 0; l < VXB_MAX_LEVELS; ++l) { survivors += c.survivors[l]; fresh += c.fresh[l]; }
+	const unsigned jobs = compact ? survivors + fresh : fresh;
+	VxbMeshArenas runSrc;
+	runSrc.v = ctx->verts.p; runSrc.i = ctx->idx.p; runSrc.tv = ctx->tverts.p; runSrc.ti = ctx->tidx.p;
+	if (jobs)
+		vxb_mesh_copy_kernel<<<jobs, 128, 0, st>>>(m->jobSrc.p, m->jobDst.p, m->dir.p, ctx->records.p, m->scratch.p, m->set[m->active].view(),
+			runSrc, m->set[target].view(), anyUnmapped ? 1 : 0);
+	VXB_CUDA(ctx, cudaGetLastError());
+	const unsigned merged = survivors + fresh;
+	if (merged) VXB_CUDA(ctx, cudaMemcpyAsync(m->dir.p, m->scratch.p, sizeof(vxb_block_record) * merged, cudaMemcpyDeviceToDevice, st));
+	VXB_CUDA(ctx, cudaEventRecord(m->ev[1], st));
+	VXB_CUDA(ctx, cudaStreamSynchronize(st));
+
+	// ---- the new state ----
+	if (compact && grow) m->set[m->active].release(); // too small to take the next compaction
+	if (compact || grow) ++m->info.generation;
+	if (compact) ++m->info.compactions;
+	if (grow && hadArenas) ++m->info.growths;
+	m->active = target;
+	const uint64_t elemBytes[4] = { sizeof(VxbVertex), 4, sizeof(VxbVertex), 4 };
+	uint64_t copied = (uint64_t)merged * sizeof(vxb_block_record);
+	for (int a = 0; a < 4; ++a)
+	{
+		const uint64_t moved = c.freshElems[a] + (compact ? c.survivorElems[a] : 0);
+		copied += moved * elemBytes[a];
+		m->cap[a] = newCap[a];
+		m->span[a] = (compact || !region) ? live[a] : tail[a] + c.freshElems[a];
+		m->total[a] = c.survivorRaw[a] + c.freshRaw[a];
+	}
+	vxb_mesh_info& i = m->info;
+	i.levels = (uint32_t)levels;
+	i.block_count = merged;
+	for (int l = 0; l < 12; ++l) i.level_blocks[l] = c.survivors[l] + c.fresh[l];
+	i.vertex_span = m->span[0]; i.index_span = m->span[1]; i.trans_vertex_span = m->span[2]; i.trans_index_span = m->span[3];
+	i.vertex_total = m->total[0]; i.index_total = m->total[1]; i.trans_vertex_total = m->total[2]; i.trans_index_total = m->total[3];
+	for (int a = 0; a < 4; ++a) i.capacity[a] = m->cap[a];
+	memcpy(i.stats, ctx->info.stats, sizeof(i.stats));
+	i.bytes_copied = copied;
+	VXB_CUDA(ctx, cudaEventElapsedTime(&i.apply_ms, m->ev[0], m->ev[1]));
+	m->content = true;
+	m->serial = ctx->runSerial;
+	m->n = n;
+	return VXB_OK;
+}
+
+int vxb_mesh_info_get(vxb_mesh* m, vxb_mesh_info* out)
+{
+	if (!m || !out) return VXB_ERR_ARGUMENT;
+	*out = m->info;
+	return VXB_OK;
+}
+
+int vxb_mesh_download(vxb_mesh* m, vxb_block_record* records, void* vertices, uint32_t* indices, void* transVertices, uint32_t* transIndices)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	cudaSetDevice(ctx->device);
+	const vxb_mesh::Arenas& a = m->set[m->active];
+	cudaStream_t st = ctx->stream;
+	if (records && m->info.block_count) VXB_CUDA(ctx, cudaMemcpyAsync(records, m->dir.p, sizeof(vxb_block_record) * m->info.block_count, cudaMemcpyDeviceToHost, st));
+	if (vertices && m->span[0]) VXB_CUDA(ctx, cudaMemcpyAsync(vertices, a.v.p, m->span[0] * sizeof(VxbVertex), cudaMemcpyDeviceToHost, st));
+	if (indices && m->span[1]) VXB_CUDA(ctx, cudaMemcpyAsync(indices, a.i.p, m->span[1] * 4, cudaMemcpyDeviceToHost, st));
+	if (transVertices && m->span[2]) VXB_CUDA(ctx, cudaMemcpyAsync(transVertices, a.tv.p, m->span[2] * sizeof(VxbVertex), cudaMemcpyDeviceToHost, st));
+	if (transIndices && m->span[3]) VXB_CUDA(ctx, cudaMemcpyAsync(transIndices, a.ti.p, m->span[3] * 4, cudaMemcpyDeviceToHost, st));
+	VXB_CUDA(ctx, cudaStreamSynchronize(st));
+	return VXB_OK;
+}
+
+int vxb_mesh_device_arenas(vxb_mesh* m, const vxb_block_record** records, const void** vertices, const uint32_t** indices,
+	const void** transVertices, const uint32_t** transIndices)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	const vxb_mesh::Arenas& a = m->set[m->active];
+	if (records) *records = m->dir.p;
+	if (vertices) *vertices = a.v.p;
+	if (indices) *indices = a.i.p;
+	if (transVertices) *transVertices = a.tv.p;
+	if (transIndices) *transIndices = a.ti.p;
+	return VXB_OK;
+}
+
+int vxb_mesh_select_lod(vxb_mesh* m, const float camera[3], float baseDistance, vxb_draw_lists* out)
+{
+	if (!m || !camera) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_select_lod: nothing applied yet");
+	cudaSetDevice(ctx->device);
+	VxbDev d;
+	memset(&d, 0, sizeof(d));
+	d.n = (int)m->n; d.levels = (int)m->info.levels; d.lastLevel = d.levels - 1;
+	d.records = m->dir.p;
+	const int r = selectLod(ctx, d, m->info.block_count, m->dirCap, camera, baseDistance, m->drawCmd, m->drawInfo, m->drawTCmd, m->drawTInfo,
+		m->drawCounts, m->drawLists);
+	if (r != VXB_OK) return r;
+	if (out) *out = m->drawLists;
 	return VXB_OK;
 }
 
