@@ -42,11 +42,15 @@ std::string g_createError;
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
 	const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
+// device buffers free themselves; release() is for code that frees one early on purpose.  Not copyable (the move
+// assignment deletes the copies); movable, so that a struct of buffers can be reset to a fresh one (releaseShard).
 template <typename T>
 struct DevBuf
 {
 	T* p = nullptr;
 	size_t count = 0;
+	DevBuf& operator=(DevBuf&& o) noexcept { release(); std::swap(p, o.p); std::swap(count, o.count); return *this; }
+	~DevBuf() { release(); }
 	cudaError_t ensure(size_t want)
 	{
 		if (want <= count) return cudaSuccess;
@@ -65,7 +69,9 @@ struct vxb_context
 	int device = 0;
 	int smCount = 0;
 	cudaStream_t stream = nullptr, stream2 = nullptr;
-	cudaEvent_t evBegin = nullptr, evEnd = nullptr, evFork = nullptr, evDecide0 = nullptr, evJoin = nullptr, evDir = nullptr, evVerts = nullptr;
+	cudaEvent_t evBegin = nullptr, evEnd = nullptr, evDir = nullptr;
+	cudaEvent_t evFork = nullptr, evJoin = nullptr;               // the transition cells on stream2
+	cudaEvent_t evLatticeFork = nullptr, evLatticeJoin = nullptr; // the coarse levels' lattices on stream2
 	std::vector<cudaEvent_t> evChunks; // packed upload: one per z-chunk
 	std::vector<cudaEvent_t> kevents; // per-kernel timing (pairs)
 	std::string error;
@@ -87,9 +93,11 @@ struct vxb_context
 	vxb_draw_lists drawLists;
 	VxbDev lastDev; // kernel-side view of the last run (records, arenas), for the consumer-side kernels
 	DevBuf<unsigned int> packSizes, packFlags, packError;
-	struct PinnedBuf // page-locked host scratch (grows, never shrinks)
+	struct PinnedBuf // page-locked host scratch (grows, never shrinks, frees itself)
 	{
 		void* p = nullptr; size_t bytes = 0;
+		PinnedBuf& operator=(PinnedBuf&&) = delete; // and with it the copies
+		~PinnedBuf() { if (p) cudaFreeHost(p); }
 		bool ensure(size_t want)
 		{
 			if (want <= bytes) return true;
@@ -98,7 +106,6 @@ struct vxb_context
 			if (cudaHostAlloc(&p, want, cudaHostAllocDefault) != cudaSuccess) { p = nullptr; return false; }
 			bytes = want; return true;
 		}
-		void release() { if (p) cudaFreeHost(p); p = nullptr; bytes = 0; }
 	} hostOffsets, hostRecords;
 	DevBuf<unsigned int> scanFlags;
 	DevBuf<unsigned char> blockInfo;
@@ -139,7 +146,6 @@ struct vxb_context
 	bool downloadOpen = false;            // between vxb_result_download_begin and _end
 	void* downloadVerts = nullptr;
 	void* downloadTransVerts = nullptr;
-	uint32_t shardLaunches = 0;
 	// sharded runs (vxb_shard_*)
 	struct Shard
 	{
@@ -149,8 +155,18 @@ struct vxb_context
 		DevBuf<unsigned char> sbMine;
 		DevBuf<unsigned int> sbWeight;
 		// level-sbLevel pages + valid flags in ONE buffer the peers can map: VMM allocation (real ranks) or cudaMalloc (virtual ranks)
-		unsigned char* pagesBuf = nullptr; size_t pagesBytes = 0, validBytes = 0, latticeBytes = 0, bufBytes = 0; // pages | valid | coarse lattices
-		unsigned char* peerLattice[8] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };
+		unsigned char* pagesBuf = nullptr; size_t pagesBytes = 0, validBytes = 0, latticeBytes = 0, bufBytes = 0;
+		// the layout of that buffer, this rank's (base = pagesBuf) or a peer's (base = its pages):
+		// pages | valid flags | coarse lattices | barrier area (8 peer slots, the epoch at +64, the CTA arrival counter at +128)
+		static const size_t barrierBytes = 256;
+		size_t barrierOffset() const { return pagesBytes + validBytes + latticeBytes; }
+		unsigned short* pages(void* base) const { return static_cast<unsigned short*>(base); }
+		unsigned char* valid(void* base) const { return static_cast<unsigned char*>(base) + pagesBytes; }
+		unsigned char* lattices(void* base) const { return valid(base) + validBytes; }
+		unsigned char* barrier(void* base) const { return static_cast<unsigned char*>(base) + barrierOffset(); }
+		unsigned long long* slots(void* base) const { return reinterpret_cast<unsigned long long*>(barrier(base)); }
+		unsigned long long* epoch() const { return reinterpret_cast<unsigned long long*>(barrier(pagesBuf) + 64); }
+		unsigned int* arrived() const { return reinterpret_cast<unsigned int*>(barrier(pagesBuf) + 128); }
 		bool pagesVmm = false;
 		CUdeviceptr pagesVa = 0; CUmemGenericAllocationHandle pagesHandle = 0;
 		unsigned short* peerPages[8] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };
@@ -159,13 +175,12 @@ struct vxb_context
 		std::vector<std::pair<CUdeviceptr, size_t> > peerMapped;
 		std::vector<CUmemGenericAllocationHandle> peerHandles;
 		void* comm = nullptr;                          // ncclComm_t
-		DevBuf<unsigned long long> barrierBuf;         // the tiny all-gather that orders the page exchange
 		uint32_t phaseLaunches = 0;
 	} shard;
 	// the launch sequence of a full run as a CUDA graph, re-instantiated when any kernel argument changes
 	cudaGraphExec_t graphExec = nullptr;
 	std::vector<unsigned char> graphKey;
-	uint32_t graphLaunches = 0;
+	uint32_t graphLaunches = 0, graphKindLaunches[10] = { 0, 0, 0, 0, 0, 0, 0, 0, 0, 0 }; // what a replay reports
 	bool graphDisabled = false;
 	// the cube of a sharded run (vxb_cube_*): one virtual range per volume, this rank's slab local, peers' slabs imported
 	struct Cube
@@ -180,8 +195,6 @@ struct vxb_context
 		std::vector<std::pair<CUdeviceptr, size_t> > mapped; // every mapped piece
 		size_t pieceBytes(int channel) const { return channel < 3 ? (size_t)groupPlanes * n * n : (size_t)(groupPlanes / 2) * (n / 2) * (n / 2); }
 	} cube;
-	VxbCounters lastCounters;
-	size_t validBytes = 0;
 
 	bool haveResult = false;
 	uint64_t runSerial = 0;                 // counts the runs (vxb_polygonize*), so that a mesh can tell whether it missed one
@@ -254,6 +267,33 @@ int coarseLoFor(uint32_t n, int levels)
 	return lo;
 }
 
+// level l owns entries [blockBase[l], +blocks[l]) of every per-block array of a run (VxbDev::workBase = idBase, written
+// into `dev`) and of a mesh (VxbMeshRange::levelBase); its valid flags, material pages and sign-mix bytes (levels >= 1)
+// start at validOff / pageOff / mixOff; the coarse levels' blocks (>= coarseLo) are numbered from coarseBase[l]
+struct LevelLayout
+{
+	size_t blocks[VXB_MAX_LEVELS], blockBase[VXB_MAX_LEVELS], validOff[VXB_MAX_LEVELS], pageOff[VXB_MAX_LEVELS];
+	size_t mixOff[VXB_MAX_LEVELS], coarseBase[VXB_MAX_LEVELS];
+	size_t totalBlocks = 0, validBytes = 0, pageEntries = 0, mixBytes = 0, coarseBlocks = 0;
+};
+
+LevelLayout levelLayout(uint32_t n, int levels, int coarseLo, VxbDev* dev = nullptr)
+{
+	LevelLayout L;
+	for (int l = 0; l < levels; ++l)
+	{
+		const size_t b = blocksAtLevel(n, l);
+		L.blocks[l] = b;
+		L.blockBase[l] = L.totalBlocks; L.totalBlocks += b;
+		L.validOff[l] = L.validBytes; L.validBytes += (b + 15) & ~(size_t)15;
+		L.pageOff[l] = L.pageEntries; if (l >= 1) L.pageEntries += b * 4096;
+		L.mixOff[l] = L.mixBytes; if (l >= 1) L.mixBytes += (b + 15) & ~(size_t)15;
+		L.coarseBase[l] = L.coarseBlocks; if (l >= coarseLo) L.coarseBlocks += b;
+		if (dev) { dev->workBase[l] = dev->idBase[l] = (unsigned)L.blockBase[l]; dev->coarseBase[l] = (unsigned)L.coarseBase[l]; }
+	}
+	return L;
+}
+
 #define VXB_LATTICE_LO 2 // levels >= 2 have their own sample lattice (VxbDev::coarseLattice)
 
 // byte layout of the coarse levels' lattices in one buffer: level l at offsets[l], (h + 1)^2 rows of h + 16 bytes
@@ -323,7 +363,7 @@ int buildTensorMap(vxb_context* ctx)
 		r = encodeTileMap(ctx, &ctx->tmap1, ctx->latticePtr, (uint32_t)h);
 	}
 	else ctx->tmap1 = ctx->tmap;
-	if (r == VXB_OK) r = buildCoarseLattices(ctx, ctx->shard.on ? ctx->shard.pagesBuf + ctx->shard.pagesBytes + ctx->shard.validBytes : nullptr);
+	if (r == VXB_OK) r = buildCoarseLattices(ctx, ctx->shard.on ? ctx->shard.lattices(ctx->shard.pagesBuf) : nullptr);
 	return r;
 }
 
@@ -343,25 +383,46 @@ struct Region
 	size_t count[VXB_MAX_LEVELS];
 };
 
-struct KernelTimer
+// Launches the kernels of one run and counts them: each launch toward the run's total and toward its kind (vxb_kernel_ms:
+// 0 scan, 1 block walk, 2 levels >= 1 and big blocks, 3 level 0, 4 vertices, 5 triangles, 6 transition cells, 7 finish,
+// 8 and 9 the two exchanges of a sharded run).  With VXB_FLAG_KERNEL_TIMES, when every launch is on the context's stream,
+// each launch of a kind sits between a pair of events.
+struct Launcher
 {
-	vxb_context* ctx; bool on; size_t used = 0;
-	std::vector<int> kinds;
-	void begin(int kind)
+	static const int kNoKind = -1; // vxb_mark_split_kernel: counted in the total only, and not timed
+
+	vxb_context* ctx;
+	bool timed;
+	uint32_t total = 0;            // the per-kind counts are ctx->kindLaunches
+	std::vector<int> bracketKinds; // kind of each event pair in ctx->kevents
+
+	Launcher(vxb_context* c, bool t) : ctx(c), timed(t) { reset(); }
+	void reset() { total = 0; memset(ctx->kindLaunches, 0, sizeof(ctx->kindLaunches)); }
+	template <typename... P, typename... A>
+	void operator()(int kind, cudaStream_t s, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, const A&... args)
 	{
-		if (!on) return;
-		while (ctx->kevents.size() < used + 2) { cudaEvent_t e; cudaEventCreate(&e); ctx->kevents.push_back(e); }
-		cudaEventRecord(ctx->kevents[used], ctx->stream); kinds.push_back(kind);
+		++total;
+		bracket(kind, [&] { kernel<<<grid, block, smem, s>>>(args...); });
 	}
-	void end() { if (!on) return; cudaEventRecord(ctx->kevents[used + 1], ctx->stream); used += 2; }
-	void collect()
+	// a launch of `kind` outside the total: the all-gather of exchange 0, which is not a kernel, is timed and counted as kind 8
+	template <typename F> void bracket(int kind, F launch)
+	{
+		if (kind != kNoKind) ++ctx->kindLaunches[kind];
+		if (!timed || kind == kNoKind) { launch(); return; }
+		const size_t used = 2 * bracketKinds.size();
+		while (ctx->kevents.size() < used + 2) { cudaEvent_t e; cudaEventCreate(&e); ctx->kevents.push_back(e); }
+		cudaEventRecord(ctx->kevents[used], ctx->stream);
+		launch();
+		cudaEventRecord(ctx->kevents[used + 1], ctx->stream);
+		bracketKinds.push_back(kind);
+	}
+	void collectTimes() const
 	{
 		for (int k = 0; k < 10; ++k) ctx->kindMs[k] = 0.f;
-		if (!on) return;
-		for (size_t i = 0; i < kinds.size(); ++i)
+		for (size_t i = 0; i < bracketKinds.size(); ++i)
 		{
 			float ms = 0.f; cudaEventElapsedTime(&ms, ctx->kevents[2 * i], ctx->kevents[2 * i + 1]);
-			ctx->kindMs[kinds[i]] += ms;
+			ctx->kindMs[bracketKinds[i]] += ms;
 		}
 	}
 };
@@ -443,7 +504,7 @@ void releaseShard(vxb_context* ctx)
 		if (sh.pagesHandle) api.release(sh.pagesHandle);
 	}
 	else if (sh.pagesBuf) cudaFree(sh.pagesBuf);
-	sh.sbMine.release(); sh.sbWeight.release(); sh.barrierBuf.release();
+	sh.sbMine.release(); sh.sbWeight.release();
 	void* comm = sh.comm;
 	sh = vxb_context::Shard();
 	sh.comm = comm; // the communicator outlives a re-configuration (vxb_destroy ends it)
@@ -616,11 +677,6 @@ int vxb_cube_piece(vxb_context* ctx, uint32_t piece, int8_t** dist, uint8_t** ma
 	return VXB_OK;
 }
 
-} // extern "C"
-
-extern "C"
-{
-
 int vxb_create(int device, vxb_context** out)
 {
 	if (!out) return fail(nullptr, VXB_ERR_ARGUMENT, "vxb_create: out is null");
@@ -643,14 +699,10 @@ int vxb_create(int device, vxb_context** out)
 	memset(&ctx->lastDev, 0, sizeof(ctx->lastDev));
 	if ((e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking)) != cudaSuccess ||
 		(e = cudaStreamCreateWithFlags(&ctx->stream2, cudaStreamNonBlocking)) != cudaSuccess ||
-		(e = cudaEventCreate(&ctx->evBegin)) != cudaSuccess || (e = cudaEventCreate(&ctx->evEnd)) != cudaSuccess ||
-		(e = cudaEventCreateWithFlags(&ctx->evFork, cudaEventDisableTiming)) != cudaSuccess ||
-		(e = cudaEventCreateWithFlags(&ctx->evDecide0, cudaEventDisableTiming)) != cudaSuccess ||
-		(e = cudaEventCreateWithFlags(&ctx->evJoin, cudaEventDisableTiming)) != cudaSuccess ||
-		(e = cudaEventCreateWithFlags(&ctx->evDir, cudaEventDisableTiming)) != cudaSuccess ||
-		(e = cudaEventCreateWithFlags(&ctx->evVerts, cudaEventDisableTiming)) != cudaSuccess ||
-		false)
+		(e = cudaEventCreate(&ctx->evBegin)) != cudaSuccess || (e = cudaEventCreate(&ctx->evEnd)) != cudaSuccess)
 	{ fail(nullptr, VXB_ERR_CUDA, "stream/event creation", e); vxb_destroy(ctx); return VXB_ERR_CUDA; }
+	for (cudaEvent_t* ev : { &ctx->evDir, &ctx->evFork, &ctx->evJoin, &ctx->evLatticeFork, &ctx->evLatticeJoin })
+		if ((e = cudaEventCreateWithFlags(ev, cudaEventDisableTiming)) != cudaSuccess) { fail(nullptr, VXB_ERR_CUDA, "stream/event creation", e); vxb_destroy(ctx); return VXB_ERR_CUDA; }
 
 	void* fn = nullptr;
 	cudaDriverEntryPointQueryResult qres;
@@ -691,31 +743,17 @@ void vxb_destroy(vxb_context* ctx)
 	if (ctx->stream) cudaStreamSynchronize(ctx->stream);
 	if (ctx->stream2) cudaStreamSynchronize(ctx->stream2);
 	if (ctx->graphExec) cudaGraphExecDestroy(ctx->graphExec);
-	ctx->hostOffsets.release(); ctx->hostRecords.release();
 	releaseShard(ctx);
 	if (ctx->shard.comm && ncclApi().ok) { ncclApi().commDestroy(ctx->shard.comm); ctx->shard.comm = nullptr; }
 	releaseCube(ctx);
-	ctx->fillColumns.release(); ctx->packSizes.release(); ctx->packFlags.release(); ctx->packError.release();
-	ctx->progList.release(); ctx->progCount.release();
 	for (cudaEvent_t e : ctx->progEv) if (e) cudaEventDestroy(e);
-	ctx->drawCmd.release(); ctx->drawTCmd.release(); ctx->drawInfo.release(); ctx->drawTInfo.release(); ctx->drawCounts.release();
-	ctx->mixInfo.release(); ctx->coarseDone.release(); ctx->mixCount.release(); ctx->coarseLatticeBuf.release(); ctx->coarseMaps.release();
-	ctx->volDist.release(); ctx->volMat.release(); ctx->volBlend.release(); ctx->staging.release(); ctx->packOffsets.release(); ctx->updCoords.release(); ctx->lattice1.release();
-	ctx->scanFlags.release(); ctx->blockInfo.release(); ctx->consPages.release(); ctx->validFlags.release();
-	ctx->cachePages.release(); ctx->worklist.release(); ctx->emitList.release(); ctx->bigList.release(); ctx->transList.release(); ctx->ntScratch.release(); ctx->cellBlock.release(); ctx->vlist.release(); ctx->cellRecs.release(); ctx->blockRecs.release(); ctx->tvlist.release(); ctx->verts.release(); ctx->tverts.release();
-	ctx->idx.release(); ctx->tidx.release(); ctx->records.release(); ctx->counters.release(); ctx->lut.release();
 	for (cudaEvent_t e : ctx->kevents) cudaEventDestroy(e);
-	if (ctx->evBegin) cudaEventDestroy(ctx->evBegin);
-	if (ctx->evEnd) cudaEventDestroy(ctx->evEnd);
-	if (ctx->evFork) cudaEventDestroy(ctx->evFork);
-	if (ctx->evDecide0) cudaEventDestroy(ctx->evDecide0);
-	if (ctx->evJoin) cudaEventDestroy(ctx->evJoin);
-	if (ctx->evDir) cudaEventDestroy(ctx->evDir);
-	if (ctx->evVerts) cudaEventDestroy(ctx->evVerts);
+	for (cudaEvent_t e : { ctx->evBegin, ctx->evEnd, ctx->evDir, ctx->evFork, ctx->evJoin, ctx->evLatticeFork, ctx->evLatticeJoin })
+		if (e) cudaEventDestroy(e);
 	for (cudaEvent_t e : ctx->evChunks) if (e) cudaEventDestroy(e);
 	if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
 	if (ctx->stream) cudaStreamDestroy(ctx->stream);
-	delete ctx;
+	delete ctx; // the buffers free themselves
 }
 
 const char* vxb_last_error(const vxb_context* ctx) { return ctx ? ctx->error.c_str() : g_createError.c_str(); }
@@ -1281,134 +1319,355 @@ int vxb_set_launch_limit(vxb_context* ctx, uint32_t ctas)
 	return VXB_OK;
 }
 
-// shardPhase: -1 = not a sharded run; 0 = scan + block info (no sync); 1 = plan + the levels below the coarse ones + page
-// publication (no sync); 2 = coarse levels, emission, directory (syncs, result); 3 = everything, the two exchanges by
-// ncclAllGather on the context's stream (needs vxb_shard_nccl_init)
-static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, const Region* region, int shardPhase = -1)
+} // extern "C"
+
+namespace
 {
-	const bool incremental = region != nullptr;
-	if (!ctx) return VXB_ERR_ARGUMENT;
-	if (!ctx->haveGrid) return fail(ctx, VXB_ERR_STATE, "vxb_polygonize: no grid uploaded");
-	if (ctx->downloadOpen) return fail(ctx, VXB_ERR_STATE, "vxb_polygonize: a result download is open (vxb_result_download_end first)");
-	cudaSetDevice(ctx->device);
-	ctx->haveResult = false;
-	++ctx->runSerial;
-	const uint32_t n = ctx->n;
-	const int levels = ctx->levels;
-	const int computed = (maxLevels == 0 || (int)maxLevels > levels) ? levels : (int)maxLevels;
-	const size_t nb0 = n / 16, blocks0 = nb0 * nb0 * nb0;
-	const bool sharded = shardPhase >= 0;
-	vxb_context::Shard& sh = ctx->shard;
-	const bool kernelTimes = (flags & VXB_FLAG_KERNEL_TIMES) != 0 && (!sharded || shardPhase == 3);
+// what a run is: a whole run on one context, or - vxb_polygonize_sharded's phase - a piece of a sharded run around the
+// two exchanges, or a whole sharded step with the exchanges inside
+enum RunPhase
+{
+	kRunSingle = -1,
+	kShardScan = 0,   // scan + block info (no sync)
+	kShardLevels = 1, // plan + the levels below the coarse ones + page publication (no sync)
+	kShardTail = 2,   // coarse levels, emission, directory (syncs, result)
+	kShardWhole = 3,  // everything, the two exchanges by ncclAllGather on the context's stream (needs vxb_shard_nccl_init)
+};
 
-	// ---- device state ----
-	VXB_CUDA(ctx, ctx->scanFlags.ensure(blocks0));
-	VXB_CUDA(ctx, ctx->blockInfo.ensure(blocks0));
-	VXB_CUDA(ctx, ctx->consPages.ensure(blocks0 * 128));
-	size_t totalBlocks = 0, validBytes = 0, cacheEntries = 0, mixBytes = 0;
-	size_t validOff[VXB_MAX_LEVELS], cacheOff[VXB_MAX_LEVELS], mixOff[VXB_MAX_LEVELS];
+// one run of a context and its parts; a full run is all of them in order, a whole sharded step has an exchange after the
+// scan and after the levels
+struct Run
+{
+	vxb_context* ctx;
+	vxb_context::Shard& sh;
+	cudaStream_t st;
+	const Region* region; // an incremental run's dirty box per level; null for a full run
+	RunPhase phase;
+	uint32_t flags;
+	bool sharded;
+	bool kernelTimes = false, latticeForked = false; // latticeForked: the coarse lattices are being built on stream2
+	int computed = 0;
+	LevelLayout L;
 	VxbDev dev;
-	memset(&dev, 0, sizeof(dev));
-	const int coarseLo = ctx->coarseLo;
-	size_t coarseBlocks = 0;
-	for (int l = 0; l < levels; ++l)
-	{
-		const size_t b = blocksAtLevel(n, l);
-		dev.workBase[l] = (unsigned)totalBlocks;
-		dev.idBase[l] = (unsigned)totalBlocks;
-		totalBlocks += b;
-		validOff[l] = validBytes; validBytes += (b + 15) & ~(size_t)15;
-		cacheOff[l] = cacheEntries; if (l >= 1) cacheEntries += b * 4096;
-		mixOff[l] = mixBytes; if (l >= 1) mixBytes += (b + 15) & ~(size_t)15;
-		dev.coarseBase[l] = (unsigned)coarseBlocks; if (l >= coarseLo) coarseBlocks += b;
-	}
-	VXB_CUDA(ctx, ctx->validFlags.ensure(validBytes));
-	VXB_CUDA(ctx, ctx->cachePages.ensure(cacheEntries ? cacheEntries : 1));
-	VXB_CUDA(ctx, ctx->mixInfo.ensure(mixBytes ? mixBytes : 16));
-	VXB_CUDA(ctx, ctx->mixCount.ensure(mixBytes ? mixBytes : 16));
-	VXB_CUDA(ctx, ctx->coarseDone.ensure(coarseBlocks ? coarseBlocks : 16));
-	VXB_CUDA(ctx, ctx->worklist.ensure(totalBlocks));
-	VXB_CUDA(ctx, ctx->records.ensure(totalBlocks));
-	VXB_CUDA(ctx, ctx->emitList.ensure(totalBlocks));
-	VXB_CUDA(ctx, ctx->bigList.ensure(totalBlocks));
-	VXB_CUDA(ctx, ctx->transList.ensure(totalBlocks));
-	VXB_CUDA(ctx, ctx->blockRecs.ensure(totalBlocks));
-	VXB_CUDA(ctx, ctx->ntScratch.ensure(totalBlocks * 256));
-
-	const uint64_t vol = sharded ? (uint64_t)n * n * n / sh.world * 2 : (uint64_t)n * n * n;
-	if (!ctx->capV) ctx->capV = std::max<uint64_t>(1u << 20, vol / 24);
-	if (!ctx->capI) ctx->capI = ctx->capV * 6;
-	if (!ctx->capTV) ctx->capTV = std::max<uint64_t>(1u << 18, ctx->capV / 8);
-	if (!ctx->capTI) ctx->capTI = ctx->capTV * 6;
-	if (!ctx->capC) ctx->capC = ctx->capV + ctx->capV / 4;
-
-	dev.grid.dist = ctx->dDist; dev.grid.mat = ctx->dMat; dev.grid.blend = ctx->dBlend; dev.grid.n = (int)n;
-	dev.n = (int)n; dev.levels = levels; dev.lastLevel = levels - 1; dev.computed = computed;
-	dev.scanFlags = ctx->scanFlags.p; dev.blockInfo = ctx->blockInfo.p;
-	dev.consPages = ctx->consPages.p;
-	dev.consValid = ctx->validFlags.p + validOff[0];
-	for (int l = 1; l < levels; ++l)
-	{
-		dev.cachePages[l] = ctx->cachePages.p + cacheOff[l]; dev.cacheValid[l] = ctx->validFlags.p + validOff[l];
-		dev.mixInfo[l] = ctx->mixInfo.p + mixOff[l];
-		dev.mixCount[l] = ctx->mixCount.p + mixOff[l];
-	}
-	dev.coarseLo = coarseLo; dev.coarseDone = ctx->coarseDone.p;
 	VxbCoarseLattices scanLat;
-	memset(&scanLat, 0, sizeof(scanLat));
-	scanLat.lo = VXB_LATTICE_LO; scanLat.levels = levels;
-	for (int l = VXB_LATTICE_LO; l < levels; ++l) { dev.coarseLattice[l] = ctx->coarseLatticeBase + ctx->coarseLatticeOff[l]; scanLat.p[l] = dev.coarseLattice[l]; }
-	dev.coarseMaps = ctx->coarseMaps.p;
-	dev.latticeLo = VXB_LATTICE_LO;
-	dev.worklist = ctx->worklist.p;
-	dev.records = ctx->records.p; dev.rcap = (unsigned)totalBlocks;
-	dev.counters = ctx->counters.p; dev.lut = ctx->lut.p;
-	dev.transitions = (flags & VXB_FLAG_NO_TRANSITIONS) ? 0 : 1;
-	dev.emitList = ctx->emitList.p; dev.bigList = ctx->bigList.p; dev.transList = ctx->transList.p; dev.ntScratch = ctx->ntScratch.p;
-	dev.blockRecs = ctx->blockRecs.p;
-	dev.lattice1 = ctx->haveLattice1 ? ctx->latticePtr : nullptr;
-	dev.incremental = incremental ? 1 : 0;
-	dev.ranged = region ? 1 : 0;
-	if (region)
-		for (int l = 0; l < levels; ++l)
-		{
-			for (int a = 0; a < 3; ++a) { dev.rangeMin[l][a] = region->rangeMin[l][a]; dev.rangeMax[l][a] = region->rangeMax[l][a]; }
-			dev.idStart[l] = region->idStart[l];
-		}
 	VxbPeers peers;
-	memset(&peers, 0, sizeof(peers));
 	VxbPeerLattices peerLat;
-	memset(&peerLat, 0, sizeof(peerLat));
-	if (sharded)
+	size_t blocksAt(int l) const { return region ? region->count[l] : L.blocks[l]; }
+	void joinLattice() { if (latticeForked) { cudaStreamWaitEvent(st, ctx->evLatticeJoin, 0); latticeForked = false; } }
+
+	// checks, the per-level layout, the per-run buffers, the kernels' view of the run (VxbDev) and of the peers
+	int prepare(uint32_t maxLevels)
 	{
+		if (!ctx->haveGrid) return fail(ctx, VXB_ERR_STATE, "vxb_polygonize: no grid uploaded");
+		if (ctx->downloadOpen) return fail(ctx, VXB_ERR_STATE, "vxb_polygonize: a result download is open (vxb_result_download_end first)");
+		cudaSetDevice(ctx->device);
+		ctx->haveResult = false;
+		++ctx->runSerial;
+		const uint32_t n = ctx->n;
+		const int levels = ctx->levels, coarseLo = ctx->coarseLo;
+		const size_t blocks0 = blocksAtLevel(n, 0);
+		computed = (maxLevels == 0 || (int)maxLevels > levels) ? levels : (int)maxLevels;
+		kernelTimes = (flags & VXB_FLAG_KERNEL_TIMES) != 0 && (!sharded || phase == kShardWhole);
+
+		VXB_CUDA(ctx, ctx->scanFlags.ensure(blocks0));
+		VXB_CUDA(ctx, ctx->blockInfo.ensure(blocks0));
+		VXB_CUDA(ctx, ctx->consPages.ensure(blocks0 * 128));
+		memset(&dev, 0, sizeof(dev));
+		L = levelLayout(n, levels, coarseLo, &dev);
+		VXB_CUDA(ctx, ctx->validFlags.ensure(L.validBytes));
+		VXB_CUDA(ctx, ctx->cachePages.ensure(L.pageEntries ? L.pageEntries : 1));
+		VXB_CUDA(ctx, ctx->mixInfo.ensure(L.mixBytes ? L.mixBytes : 16));
+		VXB_CUDA(ctx, ctx->mixCount.ensure(L.mixBytes ? L.mixBytes : 16));
+		VXB_CUDA(ctx, ctx->coarseDone.ensure(L.coarseBlocks ? L.coarseBlocks : 16));
+		VXB_CUDA(ctx, ctx->worklist.ensure(L.totalBlocks));
+		VXB_CUDA(ctx, ctx->records.ensure(L.totalBlocks));
+		VXB_CUDA(ctx, ctx->emitList.ensure(L.totalBlocks));
+		VXB_CUDA(ctx, ctx->bigList.ensure(L.totalBlocks));
+		VXB_CUDA(ctx, ctx->transList.ensure(L.totalBlocks));
+		VXB_CUDA(ctx, ctx->blockRecs.ensure(L.totalBlocks));
+		VXB_CUDA(ctx, ctx->ntScratch.ensure(L.totalBlocks * 256));
+
+		const uint64_t vol = sharded ? (uint64_t)n * n * n / sh.world * 2 : (uint64_t)n * n * n;
+		if (!ctx->capV) ctx->capV = std::max<uint64_t>(1u << 20, vol / 24);
+		if (!ctx->capI) ctx->capI = ctx->capV * 6;
+		if (!ctx->capTV) ctx->capTV = std::max<uint64_t>(1u << 18, ctx->capV / 8);
+		if (!ctx->capTI) ctx->capTI = ctx->capTV * 6;
+		if (!ctx->capC) ctx->capC = ctx->capV + ctx->capV / 4;
+
+		dev.grid.dist = ctx->dDist; dev.grid.mat = ctx->dMat; dev.grid.blend = ctx->dBlend; dev.grid.n = (int)n;
+		dev.n = (int)n; dev.levels = levels; dev.lastLevel = levels - 1; dev.computed = computed;
+		dev.scanFlags = ctx->scanFlags.p; dev.blockInfo = ctx->blockInfo.p;
+		dev.consPages = ctx->consPages.p;
+		dev.consValid = ctx->validFlags.p + L.validOff[0];
+		for (int l = 1; l < levels; ++l)
+		{
+			dev.cachePages[l] = ctx->cachePages.p + L.pageOff[l]; dev.cacheValid[l] = ctx->validFlags.p + L.validOff[l];
+			dev.mixInfo[l] = ctx->mixInfo.p + L.mixOff[l];
+			dev.mixCount[l] = ctx->mixCount.p + L.mixOff[l];
+		}
+		dev.coarseLo = coarseLo; dev.coarseDone = ctx->coarseDone.p;
+		memset(&scanLat, 0, sizeof(scanLat));
+		scanLat.lo = VXB_LATTICE_LO; scanLat.levels = levels;
+		for (int l = VXB_LATTICE_LO; l < levels; ++l) { dev.coarseLattice[l] = ctx->coarseLatticeBase + ctx->coarseLatticeOff[l]; scanLat.p[l] = dev.coarseLattice[l]; }
+		dev.coarseMaps = ctx->coarseMaps.p;
+		dev.latticeLo = VXB_LATTICE_LO;
+		dev.worklist = ctx->worklist.p;
+		dev.records = ctx->records.p; dev.rcap = (unsigned)L.totalBlocks;
+		dev.counters = ctx->counters.p; dev.lut = ctx->lut.p;
+		dev.transitions = (flags & VXB_FLAG_NO_TRANSITIONS) ? 0 : 1;
+		dev.emitList = ctx->emitList.p; dev.bigList = ctx->bigList.p; dev.transList = ctx->transList.p; dev.ntScratch = ctx->ntScratch.p;
+		dev.blockRecs = ctx->blockRecs.p;
+		dev.lattice1 = ctx->haveLattice1 ? ctx->latticePtr : nullptr;
+		dev.incremental = dev.ranged = region ? 1 : 0;
+		if (region)
+			for (int l = 0; l < levels; ++l)
+			{
+				for (int a = 0; a < 3; ++a) { dev.rangeMin[l][a] = region->rangeMin[l][a]; dev.rangeMax[l][a] = region->rangeMax[l][a]; }
+				dev.idStart[l] = region->idStart[l];
+			}
+		memset(&peers, 0, sizeof(peers));
+		memset(&peerLat, 0, sizeof(peerLat));
+		if (!sharded) return VXB_OK;
 		if (!sh.on) return fail(ctx, VXB_ERR_STATE, "vxb_polygonize_sharded: call vxb_shard_configure first");
 		if (sh.sbLevel != coarseLo - 1 || coarseLo >= levels) return fail(ctx, VXB_ERR_STATE, "vxb_polygonize_sharded: the grid changed since vxb_shard_configure");
 		dev.shardWorld = (int)sh.world; dev.shardRank = (int)sh.rank; dev.shardLayers = (int)sh.groupLayers;
 		dev.sbLevel = sh.sbLevel; dev.sbMine = sh.sbMine.p; dev.sbWeight = sh.sbWeight.p;
 		// the pages of the super-block level live in the buffer the peers write into
-		dev.cachePages[sh.sbLevel] = reinterpret_cast<unsigned short*>(sh.pagesBuf);
-		dev.cacheValid[sh.sbLevel] = sh.pagesBuf + sh.pagesBytes;
+		dev.cachePages[sh.sbLevel] = sh.pages(sh.pagesBuf);
+		dev.cacheValid[sh.sbLevel] = sh.valid(sh.pagesBuf);
 		for (uint32_t p = 0; p < sh.world; ++p)
 		{
 			if (p == sh.rank) continue;
 			if (!sh.peerSet[p]) return fail(ctx, VXB_ERR_STATE, "vxb_polygonize_sharded: a peer's page buffer is not set (vxb_shard_set_peer / vxb_shard_import)");
 			peers.pages[peers.count] = sh.peerPages[p]; peers.valid[peers.count] = sh.peerValid[p];
-			peers.peerSlots[peers.count] = reinterpret_cast<unsigned long long*>(sh.peerLattice[p] + sh.latticeBytes);
-			peerLat.base[peers.count] = sh.peerLattice[p];
+			peers.peerSlots[peers.count] = sh.slots(sh.peerPages[p]);
+			peerLat.base[peers.count] = sh.lattices(sh.peerPages[p]);
 			++peers.count;
 		}
 		peerLat.count = peers.count;
-		{
-			unsigned char* area = sh.pagesBuf + sh.pagesBytes + sh.validBytes + sh.latticeBytes;
-			peers.mySlots = reinterpret_cast<unsigned long long*>(area);
-			peers.epoch = reinterpret_cast<unsigned long long*>(area + 64);
-			peers.arrived = reinterpret_cast<unsigned int*>(area + 128);
-			peers.rank = (int)sh.rank;
-		}
-		if (shardPhase == 3 && sh.world > 1 && (!sh.comm || !ncclApi().ok)) return fail(ctx, VXB_ERR_STATE, "vxb_polygonize_sharded: phase 3 needs vxb_shard_nccl_init");
+		peers.mySlots = sh.slots(sh.pagesBuf);
+		peers.epoch = sh.epoch();
+		peers.arrived = sh.arrived();
+		peers.rank = (int)sh.rank;
+		if (phase == kShardWhole && sh.world > 1 && (!sh.comm || !ncclApi().ok)) return fail(ctx, VXB_ERR_STATE, "vxb_polygonize_sharded: phase 3 needs vxb_shard_nccl_init");
+		return VXB_OK;
 	}
-	const int scanWorld = sharded ? (int)sh.world : 1, scanRank = sharded ? (int)sh.rank : 0, scanGroup = sharded ? (int)sh.groupLayers : (int)nb0;
 
+	// the scan, the coarse levels' lattices and the block info
+	int enqueueScan(Launcher& launch)
+	{
+		const size_t nb0 = ctx->n / 16;
+		const int scanWorld = sharded ? (int)sh.world : 1, scanRank = sharded ? (int)sh.rank : 0, scanGroup = sharded ? (int)sh.groupLayers : (int)nb0;
+		VXB_CUDA(ctx, cudaMemsetAsync(ctx->counters.p, 0, sizeof(VxbCounters), st));
+		if (!region) VXB_CUDA(ctx, cudaMemsetAsync(ctx->validFlags.p, 0, L.validBytes, st)); // incremental runs keep the caches (:362-364)
+		if (sharded) VXB_CUDA(ctx, cudaMemsetAsync(sh.valid(sh.pagesBuf), 0, sh.validBytes, st));
+		if (L.coarseBlocks) VXB_CUDA(ctx, cudaMemsetAsync(ctx->coarseDone.p, 0, L.coarseBlocks, st));
+		// incremental runs: only the block layers of the level-0 dirty box changed since the last run
+		const int zBase = region ? std::max(0, region->rangeMin[0][2]) : 0;
+		const size_t myLayers = region ? (size_t)std::max(0, std::min((int)nb0, region->rangeMax[0][2]) - zBase) : nb0 / scanWorld;
+		if (!myLayers) return VXB_OK;
+		const int perCta = nb0 >= 32 ? 32 : 8;
+		const dim3 grid((unsigned)((nb0 + perCta - 1) / perCta), (unsigned)nb0, (unsigned)myLayers);
+		unsigned char* lattice1 = ctx->haveLattice1 ? ctx->latticePtr : nullptr;
+		launch(0, st, perCta == 32 ? vxb_scan_kernel<32> : vxb_scan_kernel<8>, grid, VXB_THREADS, 0,
+			ctx->dDist, (int)ctx->n, ctx->scanFlags.p, lattice1, scanGroup, scanWorld, scanRank, zBase);
+		if (VXB_LATTICE_LO < computed)
+		{
+			// the sample lattices of levels >= 2: needed only by vxb_block_kernel<2>, so a single-GPU run computes them on the
+			// second stream next to the block walk and the level-0 kernel; a sharded rank does the rows of its own planes here
+			const bool cubeRows = sharded && ctx->cube.active; // the volumes are split over the ranks: own rows here, then published
+			const cudaStream_t ls = (cubeRows || kernelTimes || phase == kShardScan) ? st : ctx->stream2;
+			if (ls != st) { VXB_CUDA(ctx, cudaEventRecord(ctx->evLatticeFork, st)); VXB_CUDA(ctx, cudaStreamWaitEvent(ls, ctx->evLatticeFork, 0)); }
+			launch(1, ls, vxb_coarse_lattice_kernel, (unsigned)ctx->smCount * 4, 256, 0, reinterpret_cast<const signed char*>(ctx->dDist), (int)ctx->n, scanLat,
+				cubeRows ? (int)sh.groupLayers * 16 : 1, cubeRows ? (int)sh.world : 0, cubeRows ? (int)sh.rank : 0);
+			if (ls != st) { VXB_CUDA(ctx, cudaEventRecord(ctx->evLatticeJoin, ls)); latticeForked = true; }
+		}
+		// the lattice planes of my layers -> every peer (ordered before the peers' coarse levels by the exchanges)
+		if (sharded && ctx->cube.active && peerLat.count && VXB_LATTICE_LO < ctx->levels)
+			launch(8, st, vxb_publish_lattice_kernel, (unsigned)ctx->smCount, VXB_THREADS, 0, dev, peerLat, ctx->coarseLatticeBase);
+		const size_t mine = myLayers * nb0 * nb0;
+		const unsigned g2 = (unsigned)std::min<size_t>((mine + 255) / 256, (size_t)ctx->smCount * 8);
+		launch(1, st, vxb_block_info_kernel, g2, 256, 0, ctx->dDist, (int)ctx->n, ctx->scanFlags.p, ctx->blockInfo.p, mine, scanGroup, scanWorld, scanRank, zBase);
+		return VXB_OK;
+	}
+
+	// the sign-mix pyramid, level 0 and the levels below the coarse ones; a sharded run plans its share first and publishes
+	// its pages to the peers last
+	int enqueueLevels(Launcher& launch)
+	{
+		const int levels = ctx->levels;
+		auto selectLevel = [&](int l) {
+			const size_t b = blocksAt(l);
+			launch(1, st, vxb_select_kernel, (unsigned)std::min<size_t>((b + 255) / 256, (size_t)ctx->smCount * 8), 256, 0, dev, l);
+			return b;
+		};
+		if (levels > 1)
+		{
+			// sign-mix pyramid: the block walk of levels >= 2 and (sharded runs) the weights of the super-blocks
+			size_t threadsA = 0;
+			for (int l = 1; l < levels && l <= 2; ++l) threadsA += L.blocks[l];
+			launch(1, st, vxb_pyramid_kernel, (unsigned)((threadsA + 255) / 256), 256, 0, dev);
+			if (levels > 3) launch(1, st, vxb_pyramid_top_kernel, 1, 1024, 0, dev);
+		}
+		if (sharded) launch(1, st, vxb_plan_kernel, 1, 1024, 0, dev);
+		if (selectLevel(0))
+			launch(3, st, vxb_block_kernel<0>, ctx->persistentGrid(ctx->gridBlock[0]), VXB_THREADS, sizeof(VxbBlockSmem<0>), ctx->tmapDist19, ctx->tmapDist19, dev, 0);
+		launch(Launcher::kNoKind, st, vxb_mark_split_kernel, 1, 1, 0, dev); // level 0 is complete: the flat kernels work behind the split
+		for (int l = 1; l < ctx->coarseLo && l < computed; ++l)
+		{
+			if (!selectLevel(l)) continue;
+			if (l >= VXB_LATTICE_LO) joinLattice();
+			launch(2, st, vxb_block_kernel<1>, ctx->persistentGrid(ctx->gridBlock[1]), VXB_THREADS, sizeof(VxbBlockSmem<1>), ctx->tmap, ctx->tmap1, dev, l);
+		}
+		if (sharded && peers.count) launch(9, st, vxb_publish_kernel, (unsigned)ctx->smCount * 4, VXB_THREADS, 0, dev, peers);
+		VXB_CUDA(ctx, cudaGetLastError());
+		return VXB_OK;
+	}
+
+	// the coarse levels, the big blocks, vertices, triangles and transition cells, and the directory
+	int enqueueTail(Launcher& launch)
+	{
+		const unsigned flatGrid = ctx->persistentGrid(ctx->smCount * 8);
+		if (computed > ctx->coarseLo)
+		{
+			joinLattice(); // the lattices are complete
+			launch(2, st, vxb_block_kernel<2>, ctx->persistentGrid(ctx->gridBlock[2]), VXB_THREADS, sizeof(VxbBlockSmem<2>), ctx->tmap, ctx->tmap1, dev, ctx->coarseLo);
+		}
+		// blocks too large for the shared-memory path of vxb_block_kernel (> 1024 non-trivial cells / > 2048 level-0 vertices)
+		launch(2, st, vxb_big_block_kernel, ctx->persistentGrid(ctx->gridBigBlock), VXB_THREADS, sizeof(VxbBigBlockSmem), ctx->tmap, ctx->tmap1, dev);
+		// vertices + triangles of everything but the level-0 blocks done inside vxb_block_kernel<0>, next to the transition
+		// cells (which need the block records and the material pages only)
+		const bool transitions = dev.transitions && computed > 1;
+		const bool fork = transitions && !kernelTimes;
+		if (fork) { VXB_CUDA(ctx, cudaEventRecord(ctx->evFork, st)); VXB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->evFork, 0)); }
+		launch(4, st, vxb_vertex_kernel, flatGrid, VXB_THREADS, 0, dev);
+		launch(5, st, vxb_triangle_kernel, flatGrid, VXB_THREADS, 0, dev);
+		if (transitions)
+		{
+			const cudaStream_t ts = fork ? ctx->stream2 : st;
+			launch(6, ts, vxb_transition_kernel, ctx->persistentGrid(ctx->gridTransition), VXB_TR_THREADS, 0, dev);
+			launch(6, ts, vxb_transition_vertex_kernel, flatGrid, VXB_THREADS, 0, dev);
+			if (fork) { VXB_CUDA(ctx, cudaEventRecord(ctx->evJoin, ctx->stream2)); VXB_CUDA(ctx, cudaStreamWaitEvent(st, ctx->evJoin, 0)); }
+		}
+		joinLattice();
+		launch(7, st, vxb_finish_kernel, (unsigned)ctx->smCount * 2, VXB_THREADS, 0, dev);
+		VXB_CUDA(ctx, cudaGetLastError());
+		return VXB_OK;
+	}
+
+	// a whole sharded step exchanges after the scan and after the levels (one rank has nothing to exchange)
+	int enqueueAll(Launcher& launch)
+	{
+		const bool exchanges = phase == kShardWhole && sh.world > 1;
+		int rc = enqueueScan(launch);
+		if (rc == VXB_OK && exchanges)
+		{
+			// exchange 0: all-gather of the block info; every rank's layers are one contiguous chunk (rank-major layout)
+			const size_t chunk = blocksAtLevel(ctx->n, 0) / sh.world;
+			launch.bracket(8, [&] { rc = ncclApi().allGather(ctx->blockInfo.p + chunk * sh.rank, ctx->blockInfo.p, chunk, /*ncclUint8*/ 1, sh.comm, st); });
+			if (rc != 0) return failNccl(ctx, "ncclAllGather (block info)", rc);
+		}
+		if (rc == VXB_OK) rc = enqueueLevels(launch);
+		// exchange 1: the pages were written straight into the peers' buffers by vxb_publish_kernel, whose last CTA announced
+		// this step's epoch to every peer; waiting for the peers' epochs orders every rank's coarse levels after every rank's
+		// publication (a device-side barrier over the mapped buffers: ~5 us instead of a ~40 us one-word all-gather)
+		if (rc == VXB_OK && exchanges) launch(9, st, vxb_peer_wait_kernel, 1, 32, 0, peers, (int)sh.world);
+		if (rc == VXB_OK) rc = enqueueTail(launch);
+		return rc;
+	}
+
+	// every kernel argument of the run, its flags and the launch limit: a re-upload into other buffers, grown arenas or
+	// other flags make a new key
+	std::vector<unsigned char> graphKey() const
+	{
+		std::vector<unsigned char> key(sizeof(VxbDev) + sizeof(VxbPeers) + sizeof(VxbPeerLattices) + 3 * sizeof(CUtensorMap) + 64, 0);
+		unsigned char* k = key.data();
+		memcpy(k, &dev, sizeof(VxbDev)); k += sizeof(VxbDev);
+		memcpy(k, &peers, sizeof(VxbPeers)); k += sizeof(VxbPeers);
+		memcpy(k, &peerLat, sizeof(VxbPeerLattices)); k += sizeof(VxbPeerLattices);
+		const CUtensorMap* maps[3] = { &ctx->tmap, &ctx->tmap1, &ctx->tmapDist19 };
+		for (const CUtensorMap* mp : maps) { memcpy(k, mp, sizeof(CUtensorMap)); k += sizeof(CUtensorMap); }
+		const void* ptrs[4] = { ctx->dDist, ctx->scanFlags.p, ctx->blockInfo.p, ctx->haveLattice1 ? ctx->latticePtr : nullptr };
+		memcpy(k, ptrs, sizeof(ptrs)); k += sizeof(ptrs);
+		const int scalars[7] = { computed, (int)L.validBytes, (int)(ctx->n / 16), (int)ctx->n, (int)phase, (int)flags, (int)ctx->launchLimit };
+		memcpy(k, scalars, sizeof(scalars));
+		return key;
+	}
+
+	// vxb_result_info, the statistics, and what later runs need to know about this one
+	void finish(const VxbCounters& hc)
+	{
+		// the directory stays on the device (it is part of the result resident in HBM); vxb_result_download fetches and
+		// sorts it into the reference's block order on demand
+		ctx->lastDev = dev; ctx->directoryFetched = false; ctx->sortedRecords.clear();
+
+		vxb_result_info& info = ctx->info;
+		info.levels_total = (uint32_t)ctx->levels; info.levels_computed = (uint32_t)computed;
+		info.block_count = hc.records; info.pad = 0;
+		info.vertex_span = hc.vertices; info.index_span = hc.indices;
+		info.trans_vertex_span = hc.transVertices; info.trans_index_span = hc.transIndices;
+		info.vertex_total = hc.vertices; info.index_total = (uint64_t)hc.indices - 3ull * hc.degenerate;
+		info.trans_vertex_total = hc.transVertices; info.trans_index_total = hc.transIndices;
+		// statistics (TransVoxelImpl.cpp:528-531): BlocksCalculated counts every block of every computed level;
+		// TrivialCells only those of processed (not skipped) blocks.  The statistics of a sharded run are the SUM over the
+		// ranks (modulo 2^32): rank 0 carries the terms that do not depend on the work split.
+		uint64_t blocksCalculated = 0, processedCells = (uint64_t)hc.nonSkippedLevel0 * 4096ull;
+		if (!sharded || sh.rank == 0)
+			for (int l = 0; l < computed; ++l)
+			{
+				blocksCalculated += blocksAt(l);
+				if (l) processedCells += blocksAt(l) * 4096ull;
+			}
+		info.stats[0] = (uint32_t)blocksCalculated;
+		info.stats[1] = (uint32_t)(processedCells - hc.nonTrivial);
+		info.stats[2] = hc.nonTrivial;
+		info.stats[3] = hc.degenerate;
+		for (int i = 0; i < 16; ++i) info.stats[4 + i] = hc.perCase[i];
+		for (int i = 0; i < 8; ++i) info.used_materials[i] = hc.usedMaterials[i];
+		ctx->haveResult = true;
+		ctx->resultSharded = sharded; ctx->resultRegion = region != nullptr;
+		if (!region && !sharded) { ctx->haveFullRun = (computed == ctx->levels); ctx->nextId = (uint32_t)L.totalBlocks; }
+		else if (sharded) ctx->haveFullRun = false;
+	}
+};
+
+// A run has no host decision inside its sequence, so it is captured once into a CUDA graph and replayed while its key
+// stays the same; a replay reports the launch counts of the captured run.  A failed capture turns graphs off for good:
+// then nothing is enqueued, the counts are reset for the plain launches that follow, and *replayed stays false.
+template <typename Enqueue>
+int launchGraph(vxb_context* ctx, const std::vector<unsigned char>& key, Enqueue enqueue, Launcher& launch, bool* replayed)
+{
+	if (!ctx->graphExec || key != ctx->graphKey)
+	{
+		if (ctx->graphExec) { cudaGraphExecDestroy(ctx->graphExec); ctx->graphExec = nullptr; }
+		cudaGraph_t graph = nullptr;
+		cudaError_t ce = cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal);
+		if (ce == cudaSuccess)
+		{
+			const int rc = enqueue(launch);
+			ce = cudaStreamEndCapture(ctx->stream, &graph);
+			if (rc != VXB_OK && ce == cudaSuccess) ce = cudaErrorUnknown;
+		}
+		if (ce == cudaSuccess) ce = cudaGraphInstantiate(&ctx->graphExec, graph, 0);
+		if (graph) cudaGraphDestroy(graph);
+		if (ce != cudaSuccess) { ctx->graphExec = nullptr; ctx->graphDisabled = true; cudaGetLastError(); }
+		else { ctx->graphKey = key; ctx->graphLaunches = launch.total; memcpy(ctx->graphKindLaunches, ctx->kindLaunches, sizeof(ctx->kindLaunches)); }
+	}
+	if (!ctx->graphExec) { launch.reset(); return VXB_OK; }
+	VXB_CUDA(ctx, cudaGraphLaunch(ctx->graphExec, ctx->stream));
+	launch.total = ctx->graphLaunches;
+	memcpy(ctx->kindLaunches, ctx->graphKindLaunches, sizeof(ctx->kindLaunches));
+	*replayed = true;
+	return VXB_OK;
+}
+
+int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, const Region* region, RunPhase phase = kRunSingle)
+{
+	if (!ctx) return VXB_ERR_ARGUMENT;
+	Run r{ ctx, ctx->shard, ctx->stream, region, phase, flags, phase != kRunSingle };
+	int rc = r.prepare(maxLevels);
+	if (rc != VXB_OK) return rc;
+	const cudaStream_t st = ctx->stream;
 	VxbCounters hc;
 	for (int attempt = 0; attempt < 6; ++attempt)
 	{
@@ -1424,257 +1683,37 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 		VXB_CUDA(ctx, ctx->tvlist.ensure(ctx->capTV));
 		VXB_CUDA(ctx, ctx->cellRecs.ensure(ctx->capC));
 		VXB_CUDA(ctx, ctx->cellBlock.ensure(ctx->capC));
+		VxbDev& dev = r.dev;
 		dev.verts = ctx->verts.p; dev.idx = ctx->idx.p; dev.tverts = ctx->tverts.p; dev.tidx = ctx->tidx.p;
 		dev.vcap = (unsigned)ctx->capV; dev.icap = (unsigned)ctx->capI; dev.tvcap = (unsigned)ctx->capTV; dev.ticap = (unsigned)ctx->capTI;
 		dev.vlist = ctx->vlist.p; dev.cellRecs = ctx->cellRecs.p; dev.cellBlock = ctx->cellBlock.p; dev.ccap = (unsigned)ctx->capC; dev.tvlist = ctx->tvlist.p;
 
-		KernelTimer timer{ ctx, kernelTimes };
-		uint32_t launches = 0;
-		for (int k = 0; k < 10; ++k) ctx->kindLaunches[k] = 0;
-		const unsigned flatGrid = ctx->persistentGrid(ctx->smCount * 8);
-		cudaStream_t st = ctx->stream;
-
-		bool latticeForked = false;
-		auto joinLattice = [&]() { if (latticeForked) { cudaStreamWaitEvent(st, ctx->evVerts, 0); latticeForked = false; } };
-		// ---- the pieces of a run; a full run is all of them in order, a sharded run has an exchange after the first two ----
-		auto scanPart = [&]() -> int
+		Launcher launch(ctx, r.kernelTimes);
+		r.latticeForked = false;
+		// phases 0 and 1 of a sharded run end at an exchange the caller makes: no sync, no result
+		if (phase == kShardScan || phase == kShardLevels)
 		{
-			VXB_CUDA(ctx, cudaMemsetAsync(ctx->counters.p, 0, sizeof(VxbCounters), st));
-			if (!incremental) VXB_CUDA(ctx, cudaMemsetAsync(ctx->validFlags.p, 0, validBytes, st)); // incremental runs keep the caches (:362-364)
-			if (sharded) VXB_CUDA(ctx, cudaMemsetAsync(sh.pagesBuf + sh.pagesBytes, 0, sh.validBytes, st));
-			if (coarseBlocks) VXB_CUDA(ctx, cudaMemsetAsync(ctx->coarseDone.p, 0, coarseBlocks, st));
-			// incremental runs: only the block layers of the level-0 dirty box changed since the last run
-			const int zBase = incremental ? std::max(0, region->rangeMin[0][2]) : 0;
-			const size_t myLayers = incremental ? (size_t)std::max(0, std::min((int)nb0, region->rangeMax[0][2]) - zBase) : nb0 / scanWorld;
-			if (!myLayers) return VXB_OK;
-			const int perCta = nb0 >= 32 ? 32 : 8;
-			const dim3 grid((unsigned)((nb0 + perCta - 1) / perCta), (unsigned)nb0, (unsigned)myLayers);
-			timer.begin(0);
-			if (perCta == 32) vxb_scan_kernel<32><<<grid, VXB_THREADS, 0, st>>>(ctx->dDist, (int)n, ctx->scanFlags.p, ctx->haveLattice1 ? ctx->latticePtr : nullptr, scanGroup, scanWorld, scanRank, zBase);
-			else vxb_scan_kernel<8><<<grid, VXB_THREADS, 0, st>>>(ctx->dDist, (int)n, ctx->scanFlags.p, ctx->haveLattice1 ? ctx->latticePtr : nullptr, scanGroup, scanWorld, scanRank, zBase);
-			timer.end(); ++launches; ++ctx->kindLaunches[0];
-			if (VXB_LATTICE_LO < computed)
-			{
-				// the sample lattices of levels >= 2: needed only by vxb_block_kernel<2>, so a single-GPU run computes them on the
-				// second stream next to the block walk and the level-0 kernel; a sharded rank does the rows of its own planes here
-				const bool cubeRows = sharded && ctx->cube.active; // the volumes are split over the ranks: own rows here, then published
-				cudaStream_t ls = (cubeRows || kernelTimes || shardPhase == 0) ? st : ctx->stream2;
-				if (ls != st)
-				{
-					VXB_CUDA(ctx, cudaEventRecord(ctx->evDecide0, st));
-					VXB_CUDA(ctx, cudaStreamWaitEvent(ls, ctx->evDecide0, 0));
-				}
-				timer.begin(1);
-				vxb_coarse_lattice_kernel<<<(unsigned)ctx->smCount * 4, 256, 0, ls>>>(reinterpret_cast<const signed char*>(ctx->dDist), (int)n, scanLat,
-					cubeRows ? (int)sh.groupLayers * 16 : 1, cubeRows ? (int)sh.world : 0, cubeRows ? (int)sh.rank : 0);
-				timer.end(); ++launches; ++ctx->kindLaunches[1];
-				if (ls != st) { VXB_CUDA(ctx, cudaEventRecord(ctx->evVerts, ls)); latticeForked = true; } // joined before the first kernel that reads a lattice
-			}
-			if (sharded && ctx->cube.active && peerLat.count && VXB_LATTICE_LO < levels)
-			{
-				// the lattice planes of my layers -> every peer (ordered before the peers' coarse levels by the exchanges)
-				timer.begin(8);
-				vxb_publish_lattice_kernel<<<(unsigned)ctx->smCount, VXB_THREADS, 0, st>>>(dev, peerLat, ctx->coarseLatticeBase);
-				timer.end(); ++launches; ++ctx->kindLaunches[8];
-			}
-			const size_t mine = myLayers * nb0 * nb0;
-			const unsigned g2 = (unsigned)std::min<size_t>((mine + 255) / 256, (size_t)ctx->smCount * 8);
-			timer.begin(1);
-			vxb_block_info_kernel<<<g2, 256, 0, st>>>(ctx->dDist, (int)n, ctx->scanFlags.p, ctx->blockInfo.p, mine, scanGroup, scanWorld, scanRank, zBase);
-			timer.end(); ++launches; ++ctx->kindLaunches[1];
-			return VXB_OK;
-		};
-		auto selectLevel = [&](int l) {
-			const size_t b = region ? region->count[l] : blocksAtLevel(n, l);
-			const unsigned gs = (unsigned)std::min<size_t>((b + 255) / 256, (size_t)ctx->smCount * 8);
-			timer.begin(1);
-			vxb_select_kernel<<<gs, 256, 0, st>>>(dev, l);
-			timer.end(); ++launches; ++ctx->kindLaunches[1];
-			return b;
-		};
-		auto levelPart = [&]() -> int
-		{
-			if (levels > 1)
-			{
-				// sign-mix pyramid: the block walk of levels >= 2 and (sharded runs) the weights of the super-blocks
-				size_t threadsA = 0;
-				for (int l = 1; l < levels && l <= 2; ++l) threadsA += blocksAtLevel(n, l);
-				timer.begin(1);
-				vxb_pyramid_kernel<<<(unsigned)((threadsA + 255) / 256), 256, 0, st>>>(dev);
-				if (levels > 3) { vxb_pyramid_top_kernel<<<1, 1024, 0, st>>>(dev); ++launches; ++ctx->kindLaunches[1]; }
-				timer.end(); ++launches; ++ctx->kindLaunches[1];
-			}
-			if (sharded) { timer.begin(1); vxb_plan_kernel<<<1, 1024, 0, st>>>(dev); timer.end(); ++launches; ++ctx->kindLaunches[1]; }
-			if (selectLevel(0))
-			{
-				timer.begin(3);
-				vxb_block_kernel<0><<<ctx->persistentGrid(ctx->gridBlock[0]),VXB_THREADS, sizeof(VxbBlockSmem<0>), st>>>(ctx->tmapDist19, ctx->tmapDist19, dev, 0);
-				timer.end(); ++launches; ++ctx->kindLaunches[3];
-			}
-			vxb_mark_split_kernel<<<1, 1, 0, st>>>(dev); ++launches; // level 0 is complete: the flat kernels work behind the split
-			for (int l = 1; l < coarseLo && l < computed; ++l)
-			{
-				if (!selectLevel(l)) continue;
-				if (l >= VXB_LATTICE_LO) joinLattice();
-				timer.begin(2);
-				vxb_block_kernel<1><<<ctx->persistentGrid(ctx->gridBlock[1]),VXB_THREADS, sizeof(VxbBlockSmem<1>), st>>>(ctx->tmap, ctx->tmap1, dev, l);
-				timer.end(); ++launches; ++ctx->kindLaunches[2];
-			}
-			if (sharded && peers.count) { timer.begin(9); vxb_publish_kernel<<<(unsigned)ctx->smCount * 4, VXB_THREADS, 0, st>>>(dev, peers); timer.end(); ++launches; ++ctx->kindLaunches[9]; }
-			VXB_CUDA(ctx, cudaGetLastError());
-			return VXB_OK;
-		};
-		auto tailPart = [&]() -> int
-		{
-			if (computed > coarseLo)
-			{
-				joinLattice(); // the lattices are complete
-				timer.begin(2);
-				vxb_block_kernel<2><<<ctx->persistentGrid(ctx->gridBlock[2]),VXB_THREADS, sizeof(VxbBlockSmem<2>), st>>>(ctx->tmap, ctx->tmap1, dev, coarseLo);
-				timer.end(); ++launches; ++ctx->kindLaunches[2];
-			}
-			// blocks too large for the shared-memory path of vxb_block_kernel (> 1024 non-trivial cells / > 2048 level-0 vertices)
-			timer.begin(2);
-			vxb_big_block_kernel<<<ctx->persistentGrid(ctx->gridBigBlock),VXB_THREADS, sizeof(VxbBigBlockSmem), st>>>(ctx->tmap, ctx->tmap1, dev);
-			timer.end(); ++launches; ++ctx->kindLaunches[2];
-			// vertices + triangles of everything but the level-0 blocks done inside vxb_block_kernel<0>, next to the transition
-			// cells (which need the block records and the material pages only)
-			const bool fork = dev.transitions && computed > 1 && !kernelTimes;
-			if (fork)
-			{
-				VXB_CUDA(ctx, cudaEventRecord(ctx->evFork, st));
-				VXB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->evFork, 0));
-			}
-			timer.begin(4);
-			vxb_vertex_kernel<<<flatGrid, VXB_THREADS, 0, st>>>(dev);
-			timer.end(); ++launches; ++ctx->kindLaunches[4];
-			timer.begin(5);
-			vxb_triangle_kernel<<<flatGrid, VXB_THREADS, 0, st>>>(dev);
-			timer.end(); ++launches; ++ctx->kindLaunches[5];
-			if (dev.transitions && computed > 1)
-			{
-				cudaStream_t ts = fork ? ctx->stream2 : st;
-				timer.begin(6);
-				vxb_transition_kernel<<<ctx->persistentGrid(ctx->gridTransition),VXB_TR_THREADS, 0, ts>>>(dev);
-				vxb_transition_vertex_kernel<<<flatGrid, VXB_THREADS, 0, ts>>>(dev);
-				timer.end(); launches += 2; ctx->kindLaunches[6] += 2;
-				if (fork)
-				{
-					VXB_CUDA(ctx, cudaEventRecord(ctx->evJoin, ctx->stream2));
-					VXB_CUDA(ctx, cudaStreamWaitEvent(st, ctx->evJoin, 0));
-				}
-			}
-			joinLattice();
-			timer.begin(7);
-			vxb_finish_kernel<<<(unsigned)ctx->smCount * 2, VXB_THREADS, 0, st>>>(dev);
-			timer.end(); ++launches; ++ctx->kindLaunches[7];
-			VXB_CUDA(ctx, cudaGetLastError());
-			return VXB_OK;
-		};
-		auto exchange = [&](int which) -> int
-		{
-			if (sh.world == 1) return VXB_OK; // one rank: nothing to exchange
-			const NcclApi& nccl = ncclApi();
-			timer.begin(8 + which);
-			++ctx->kindLaunches[8 + which];
-			if (which == 0)
-			{
-				// all-gather of the block info: every rank's layers are one contiguous chunk (rank-major layout)
-				const size_t chunk = blocks0 / sh.world;
-				const int r = nccl.allGather(ctx->blockInfo.p + chunk * sh.rank, ctx->blockInfo.p, chunk, /*ncclUint8*/ 1, sh.comm, st);
-				if (r != 0) return failNccl(ctx, "ncclAllGather (block info)", r);
-			}
-			else
-			{
-				// the pages were written straight into the peers' buffers by vxb_publish_kernel, whose last CTA announced this
-				// step's epoch to every peer; waiting for the peers' epochs orders every rank's coarse levels after every rank's
-				// publication (a device-side barrier over the mapped buffers: ~5 us instead of a ~40 us one-word all-gather)
-				vxb_peer_wait_kernel<<<1, 32, 0, st>>>(peers, (int)sh.world);
-				++launches;
-			}
-			timer.end();
-			return VXB_OK;
-		};
-		auto enqueueAll = [&]() -> int
-		{
-			int r = scanPart();
-			if (r == VXB_OK && shardPhase == 3) r = exchange(0);
-			if (r == VXB_OK) r = levelPart();
-			if (r == VXB_OK && shardPhase == 3) r = exchange(1);
-			if (r == VXB_OK) r = tailPart();
-			return r;
-		};
-
-		if (shardPhase == 0)
-		{
-			VXB_CUDA(ctx, cudaEventRecord(ctx->evBegin, st));
-			const int r = scanPart();
-			VXB_CUDA(ctx, cudaGetLastError());
-			sh.phaseLaunches = launches;
-			return r;
+			if (phase == kShardScan) VXB_CUDA(ctx, cudaEventRecord(ctx->evBegin, st));
+			rc = phase == kShardScan ? r.enqueueScan(launch) : r.enqueueLevels(launch);
+			if (phase == kShardScan) VXB_CUDA(ctx, cudaGetLastError());
+			ctx->shard.phaseLaunches = (phase == kShardScan ? 0 : ctx->shard.phaseLaunches) + launch.total;
+			return rc;
 		}
-		if (shardPhase == 1)
-		{
-			const int r = levelPart();
-			sh.phaseLaunches += launches;
-			return r;
-		}
-		if (shardPhase != 2) VXB_CUDA(ctx, cudaEventRecord(ctx->evBegin, st));
-		// A run has no host decision inside the sequence, so it is captured once into a CUDA graph and replayed; the key is
-		// every kernel argument (a re-upload into other buffers, grown arenas, other flags => new capture).
+		if (phase != kShardTail) VXB_CUDA(ctx, cudaEventRecord(ctx->evBegin, st));
 		bool replayed = false;
-		if ((shardPhase == -1 || shardPhase == 3) && !incremental && !kernelTimes && !ctx->graphDisabled)
-		{
-			std::vector<unsigned char> key(sizeof(VxbDev) + sizeof(VxbPeers) + sizeof(VxbPeerLattices) + 3 * sizeof(CUtensorMap) + 64, 0);
-			unsigned char* k = key.data();
-			memcpy(k, &dev, sizeof(VxbDev)); k += sizeof(VxbDev);
-			memcpy(k, &peers, sizeof(VxbPeers)); k += sizeof(VxbPeers);
-			memcpy(k, &peerLat, sizeof(VxbPeerLattices)); k += sizeof(VxbPeerLattices);
-			const CUtensorMap* maps[3] = { &ctx->tmap, &ctx->tmap1, &ctx->tmapDist19 };
-			for (const CUtensorMap* mp : maps) { memcpy(k, mp, sizeof(CUtensorMap)); k += sizeof(CUtensorMap); }
-			const void* ptrs[4] = { ctx->dDist, ctx->scanFlags.p, ctx->blockInfo.p, ctx->haveLattice1 ? ctx->latticePtr : nullptr };
-			memcpy(k, ptrs, sizeof(ptrs)); k += sizeof(ptrs);
-			const int scalars[7] = { computed, (int)validBytes, (int)nb0, (int)n, shardPhase, (int)flags, (int)ctx->launchLimit };
-			memcpy(k, scalars, sizeof(scalars));
-			if (!ctx->graphExec || key != ctx->graphKey)
-			{
-				if (ctx->graphExec) { cudaGraphExecDestroy(ctx->graphExec); ctx->graphExec = nullptr; }
-				cudaGraph_t graph = nullptr;
-				cudaError_t ce = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
-				if (ce == cudaSuccess)
-				{
-					const int rc = enqueueAll();
-					ce = cudaStreamEndCapture(st, &graph);
-					if (rc != VXB_OK && ce == cudaSuccess) ce = cudaErrorUnknown;
-				}
-				if (ce == cudaSuccess) ce = cudaGraphInstantiate(&ctx->graphExec, graph, 0);
-				if (graph) cudaGraphDestroy(graph);
-				if (ce != cudaSuccess) { ctx->graphExec = nullptr; ctx->graphDisabled = true; cudaGetLastError(); } // fall back to plain launches for good
-				else { ctx->graphKey = key; ctx->graphLaunches = launches; }
-				launches = 0;
-			}
-			if (ctx->graphExec)
-			{
-				VXB_CUDA(ctx, cudaGraphLaunch(ctx->graphExec, st));
-				launches = ctx->graphLaunches;
-				replayed = true;
-			}
-		}
-		if (!replayed)
-		{
-			const int rc = (shardPhase == 2) ? tailPart() : enqueueAll();
-			if (rc != VXB_OK) return rc;
-			if (shardPhase == 2) launches += sh.phaseLaunches;
-		}
+		if (phase != kShardTail && !region && !r.kernelTimes && !ctx->graphDisabled)
+			if ((rc = launchGraph(ctx, r.graphKey(), [&](Launcher& l) { return r.enqueueAll(l); }, launch, &replayed)) != VXB_OK) return rc;
+		if (!replayed && (rc = phase == kShardTail ? r.enqueueTail(launch) : r.enqueueAll(launch)) != VXB_OK) return rc;
+		if (phase == kShardTail) launch.total += ctx->shard.phaseLaunches;
 		VXB_CUDA(ctx, cudaGetLastError());
 		VXB_CUDA(ctx, cudaEventRecord(ctx->evEnd, st));
 		VXB_CUDA(ctx, cudaMemcpyAsync(&hc, ctx->counters.p, sizeof(hc), cudaMemcpyDeviceToHost, st));
 		VXB_CUDA(ctx, cudaStreamSynchronize(st));
 		float ms = 0.f;
 		VXB_CUDA(ctx, cudaEventElapsedTime(&ms, ctx->evBegin, ctx->evEnd));
-		timer.collect();
+		launch.collectTimes();
 		ctx->info.device_ms = ms;
-		ctx->info.kernel_launches = launches;
+		ctx->info.kernel_launches = launch.total;
 
 		const bool overflow = hc.vertices > ctx->capV || hc.indices > ctx->capI || hc.transVertices > ctx->capTV || hc.transIndices > ctx->capTI || hc.cells > ctx->capC;
 		if (!overflow) break;
@@ -1685,46 +1724,15 @@ static int runPolygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags, c
 		if (hc.transIndices > ctx->capTI) ctx->capTI = (uint64_t)hc.transIndices + hc.transIndices / 8 + 1024;
 		if (hc.cells > ctx->capC) ctx->capC = (uint64_t)hc.cells + hc.cells / 8 + 1024;
 		// a sharded run is collective: the caller repeats it on every rank
-		if (sharded) return fail(ctx, VXB_ERR_CAPACITY, "vxb_polygonize_sharded: output arenas overflowed; capacities were grown, repeat the run on every rank");
+		if (r.sharded) return fail(ctx, VXB_ERR_CAPACITY, "vxb_polygonize_sharded: output arenas overflowed; capacities were grown, repeat the run on every rank");
 	}
-
-	// the directory stays on the device (it is part of the result resident in HBM); vxb_result_download fetches and
-	// sorts it into the reference's block order on demand
-	ctx->lastCounters = hc;
-	ctx->lastDev = dev;
-	ctx->directoryFetched = false;
-	ctx->sortedRecords.clear();
-
-	vxb_result_info& info = ctx->info;
-	info.levels_total = (uint32_t)levels; info.levels_computed = (uint32_t)computed;
-	info.block_count = hc.records; info.pad = 0;
-	info.vertex_span = hc.vertices; info.index_span = hc.indices;
-	info.trans_vertex_span = hc.transVertices; info.trans_index_span = hc.transIndices;
-	info.vertex_total = hc.vertices; info.index_total = (uint64_t)hc.indices - 3ull * hc.degenerate;
-	info.trans_vertex_total = hc.transVertices; info.trans_index_total = hc.transIndices;
-	// statistics (TransVoxelImpl.cpp:528-531): BlocksCalculated counts every block of every computed level;
-	// TrivialCells only those of processed (not skipped) blocks.  The statistics of a sharded run are the SUM over the
-	// ranks (modulo 2^32): rank 0 carries the terms that do not depend on the work split.
-	uint64_t blocksCalculated = 0, processedCells = (uint64_t)hc.nonSkippedLevel0 * 4096ull;
-	for (int l = 0; l < computed; ++l)
-	{
-		const size_t b = region ? region->count[l] : blocksAtLevel(n, l);
-		if (sharded && sh.rank != 0) continue;
-		blocksCalculated += b;
-		if (l) processedCells += b * 4096ull;
-	}
-	info.stats[0] = (uint32_t)blocksCalculated;
-	info.stats[1] = (uint32_t)(processedCells - hc.nonTrivial);
-	info.stats[2] = hc.nonTrivial;
-	info.stats[3] = hc.degenerate;
-	for (int i = 0; i < 16; ++i) info.stats[4 + i] = hc.perCase[i];
-	for (int i = 0; i < 8; ++i) info.used_materials[i] = hc.usedMaterials[i];
-	ctx->haveResult = true;
-	ctx->resultSharded = sharded; ctx->resultRegion = region != nullptr;
-	if (!region && !sharded) { ctx->haveFullRun = (computed == levels); ctx->nextId = (uint32_t)totalBlocks; }
-	else if (sharded) ctx->haveFullRun = false;
+	r.finish(hc);
 	return VXB_OK;
 }
+}
+
+extern "C"
+{
 
 int vxb_polygonize(vxb_context* ctx, uint32_t maxLevels, uint32_t flags)
 {
@@ -1794,16 +1802,11 @@ int vxb_shard_configure(vxb_context* ctx, uint32_t rank, uint32_t world, uint32_
 	const size_t sb = blocksAtLevel(n, sh.sbLevel);
 	VXB_CUDA(ctx, sh.sbMine.ensure(sb));
 	VXB_CUDA(ctx, sh.sbWeight.ensure(sb));
-	VXB_CUDA(ctx, sh.barrierBuf.ensure(8));
-	VXB_CUDA(ctx, cudaMemset(sh.barrierBuf.p, 0, 64));
 	sh.pagesBytes = sb * 4096 * sizeof(unsigned short);
 	sh.validBytes = (sb + 255) & ~(size_t)255;
-	{
-		size_t offs[VXB_MAX_LEVELS];
-		sh.latticeBytes = coarseLatticeLayout(n, ctx->levels, offs);
-	}
-	sh.latticeBytes = (sh.latticeBytes + 255) & ~(size_t)255;
-	sh.bufBytes = sh.pagesBytes + sh.validBytes + sh.latticeBytes + 256; // pages | valid | lattices | barrier area (8 slots, epoch, CTA counter)
+	size_t offs[VXB_MAX_LEVELS];
+	sh.latticeBytes = (coarseLatticeLayout(n, ctx->levels, offs) + 255) & ~(size_t)255;
+	sh.bufBytes = sh.barrierOffset() + sh.barrierBytes;
 	const VmmApi& api = vmmApi();
 	if (api.ok)
 	{
@@ -1824,7 +1827,7 @@ int vxb_shard_configure(vxb_context* ctx, uint32_t rank, uint32_t world, uint32_
 	{
 		VXB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&sh.pagesBuf), sh.bufBytes));
 	}
-	VXB_CUDA(ctx, cudaMemset(sh.pagesBuf + sh.pagesBytes + sh.validBytes + sh.latticeBytes, 0, 256));
+	VXB_CUDA(ctx, cudaMemset(sh.barrier(sh.pagesBuf), 0, sh.barrierBytes));
 	sh.on = true;
 	// virtual ranks over one shared upload: no shared even-lattice copy => level 1 gathers its tiles.  The coarse levels'
 	// lattices move into the buffer the peers map (buildTensorMap -> buildCoarseLattices).
@@ -1852,7 +1855,7 @@ int vxb_shard_buffers_get(vxb_context* ctx, vxb_shard_buffers* out)
 	out->chunk_bytes = blocks0 / sh.world;
 	out->pages = sh.pagesBuf;
 	out->pages_bytes = sh.pagesBytes;
-	out->valid = sh.pagesBuf + sh.pagesBytes;
+	out->valid = sh.valid(sh.pagesBuf);
 	out->valid_bytes = sh.validBytes;
 	out->super_level = (uint32_t)sh.sbLevel;
 	return VXB_OK;
@@ -1865,7 +1868,6 @@ int vxb_shard_set_peer(vxb_context* ctx, uint32_t peer, void* pages, void* valid
 	if (!sh.on || peer >= sh.world || peer == sh.rank || !pages || !valid) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_shard_set_peer: not configured, or bad peer / pointer");
 	sh.peerPages[peer] = static_cast<unsigned short*>(pages);
 	sh.peerValid[peer] = static_cast<unsigned char*>(valid);
-	sh.peerLattice[peer] = static_cast<unsigned char*>(pages) + sh.pagesBytes + sh.validBytes; // one buffer: pages | valid | lattices
 	sh.peerSet[peer] = true;
 	return VXB_OK;
 }
@@ -1896,7 +1898,7 @@ int vxb_shard_import(vxb_context* ctx, uint32_t peer, int fd)
 	VXB_CU(ctx, api.addressReserve(&va, sh.bufBytes, 0, 0, 0));
 	const int r = mapRange(ctx, va, sh.bufBytes, h, sh.peerMapped);
 	if (r != VXB_OK) return r;
-	return vxb_shard_set_peer(ctx, peer, reinterpret_cast<void*>(va), reinterpret_cast<unsigned char*>(va) + sh.pagesBytes);
+	return vxb_shard_set_peer(ctx, peer, reinterpret_cast<void*>(va), sh.valid(reinterpret_cast<void*>(va)));
 }
 
 int vxb_shard_nccl_unique_id(vxb_nccl_id* id)
@@ -1923,7 +1925,7 @@ int vxb_polygonize_sharded(vxb_context* ctx, uint32_t phase, uint32_t flags)
 {
 	if (!ctx) return VXB_ERR_ARGUMENT;
 	if (phase > 3) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_polygonize_sharded: phase is 0, 1, 2 (the pieces around the two exchanges) or 3 (everything, NCCL inside)");
-	return runPolygonize(ctx, 0, flags, nullptr, (int)phase);
+	return runPolygonize(ctx, 0, flags, nullptr, (RunPhase)phase);
 }
 
 int vxb_region_info_get(vxb_context* ctx, vxb_region_info* out)
@@ -2182,14 +2184,10 @@ struct vxb_mesh
 
 namespace
 {
-void releaseMesh(vxb_mesh* m)
+void deleteMesh(vxb_mesh* m)
 {
-	for (vxb_mesh::Arenas& a : m->set) a.release();
-	m->dir.release(); m->scratch.release();
-	m->keys.release(); m->vals.release(); m->keysOut.release(); m->valsOut.release(); m->jobSrc.release(); m->jobDst.release();
-	m->items.release(); m->prefix.release(); m->cubTemp.release(); m->counts.release();
-	m->drawCmd.release(); m->drawTCmd.release(); m->drawInfo.release(); m->drawTInfo.release(); m->drawCounts.release();
 	for (cudaEvent_t e : m->ev) if (e) cudaEventDestroy(e);
+	delete m; // the buffers free themselves
 }
 
 uint64_t grownCapacity(uint64_t live) { return (std::max<uint64_t>(live + live / 2, 1024) + 3) & ~(uint64_t)3; }
@@ -2214,7 +2212,7 @@ int vxb_mesh_create(vxb_context* ctx, const uint64_t capacity[4], vxb_mesh** out
 		for (int a = 0; a < 4; ++a) m->cap[a] = (capacity[a] + 3) & ~(uint64_t)3;
 		e = m->set[0].ensure(m->cap);
 	}
-	if (e != cudaSuccess) { releaseMesh(m); delete m; return fail(ctx, VXB_ERR_CUDA, "vxb_mesh_create", e); }
+	if (e != cudaSuccess) { deleteMesh(m); return fail(ctx, VXB_ERR_CUDA, "vxb_mesh_create", e); }
 	ctx->meshes.push_back(m);
 	*out = m;
 	return VXB_OK;
@@ -2227,8 +2225,7 @@ void vxb_mesh_destroy(vxb_mesh* m)
 	cudaSetDevice(ctx->device);
 	cudaStreamSynchronize(ctx->stream);
 	ctx->meshes.erase(std::remove(ctx->meshes.begin(), ctx->meshes.end(), m), ctx->meshes.end());
-	releaseMesh(m);
-	delete m;
+	deleteMesh(m);
 }
 
 int vxb_mesh_apply(vxb_mesh* m)
@@ -2250,10 +2247,11 @@ int vxb_mesh_apply(vxb_mesh* m)
 	VxbMeshRange g;
 	memset(&g, 0, sizeof(g));
 	g.erase = region ? 1 : 0;
-	size_t slots = 0;
+	const LevelLayout L = levelLayout(n, levels, ctx->coarseLo);
+	const size_t slots = L.totalBlocks;
 	for (int l = 0; l < levels; ++l)
 	{
-		g.levelBase[l] = (unsigned)slots; slots += blocksAtLevel(n, l);
+		g.levelBase[l] = (unsigned)L.blockBase[l];
 		g.nb[l] = (int)((n >> 4) >> l);
 		if (region)
 		{
