@@ -271,7 +271,7 @@ int vxb_region_info_get(vxb_context* ctx, vxb_region_info* out);
  * address the cube exactly like a single-GPU grid.  A fourth channel holds the even-lattice copy the level-1 tiles read.
  *
  * Work.  Every rank streams its OWN pieces once (vxb_scan_kernel: flags per 16^3 block); ONE ncclAllGather makes the
- * 1-byte-per-block info complete everywhere (exchange 0).  From it every rank derives the same work split: the
+ * 4-byte-per-block info complete everywhere (exchange 0).  From it every rank derives the same work split: the
  * "super-blocks" (blocks of the last level with more than 4096 blocks) in coordinate order, cut where the running count of
  * surface-crossing level-0 blocks passes total * r / world.  A rank polygonizes every level up to the super-block
  * level inside its super-blocks - the material votes of a cell only read its own children (:763-837), so this chain is
@@ -296,7 +296,7 @@ int vxb_region_info_get(vxb_context* ctx, vxb_region_info* out);
 typedef struct vxb_nccl_id { char internal[128]; } vxb_nccl_id;   /* = ncclUniqueId */
 typedef struct vxb_shard_buffers
 {
-	void* block_info;             /* device: one byte per level-0 block, rank-major (the layout of the all-gather) */
+	void* block_info;             /* device: one 32-bit word per level-0 block, rank-major (the layout of the all-gather) */
 	uint64_t block_info_bytes;
 	uint64_t chunk_bytes;         /* block_info_bytes / world */
 	void* pages;                  /* device: {material id, blend} of every cell of every super-block, block-major (z,y,x) */
@@ -434,6 +434,12 @@ int vxb_set_capacity(vxb_context* ctx, uint64_t vertices, uint64_t indices, uint
  * for their children need.  With a few CTAs each one walks many work items, so small grids exercise the code that
  * runs only from a CTA's second item on.  The output does not depend on it. */
 int vxb_set_launch_limit(vxb_context* ctx, uint32_t ctas);
+
+/* Test hook: the block walk of the last completed run at `level`: *items = the blocks it selected as work items of the
+ * per-block kernel, *emitted = the blocks that kernel found a non-trivial cell in (and emitted).  Levels from the first
+ * coarse level on are walked inside the coarse kernel, which selects no list: *items is 0 there.  Sharded runs: this
+ * rank's counts.  Either pointer may be NULL. */
+int vxb_run_work_items(vxb_context* ctx, uint32_t level, uint32_t* items, uint32_t* emitted);
 
 /* Per-kernel device time of the last vxb_polygonize run with VXB_FLAG_KERNEL_TIMES, for bench.py's roofline line:
  * which = 0: vxb_scan_kernel (streams the level-0 distance volume once), 1: block info, sign-mix pyramid + selection kernels,

@@ -265,6 +265,7 @@ def load_library():
         "vxb_result_download": (C.c_int, [vp, vp, vp, vp, vp, vp]),
         "vxb_set_capacity": (C.c_int, [vp, u64, u64, u64, u64]),
         "vxb_set_launch_limit": (C.c_int, [vp, u32]),
+        "vxb_run_work_items": (C.c_int, [vp, u32, C.POINTER(u32), C.POINTER(u32)]),
         "vxb_kernel_ms": (C.c_int, [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(u32)]),
         "vxb_result_unmapped_materials": (u64, [vp, vp, u64]),
         "vxb_mesh_create": (C.c_int, [vp, vp, C.POINTER(vp)]),
@@ -286,7 +287,7 @@ def load_library():
 
 EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream", "vxb_exchange_stream", "vxb_grid_upload_dense",
                     "vxb_grid_upload_blocks", "vxb_grid_upload_packed", "vxb_pack_dense_bound", "vxb_pack_dense", "vxb_grid_set_device", "vxb_grid_device_pointers", "vxb_set_materials",
-                    "vxb_polygonize", "vxb_polygonize_region", "vxb_region_info_get", "vxb_grid_update_blocks", "vxb_result_info_get", "vxb_result_download", "vxb_set_capacity", "vxb_set_launch_limit", "vxb_kernel_ms",
+                    "vxb_polygonize", "vxb_polygonize_region", "vxb_region_info_get", "vxb_grid_update_blocks", "vxb_result_info_get", "vxb_result_download", "vxb_set_capacity", "vxb_set_launch_limit", "vxb_run_work_items", "vxb_kernel_ms",
                     "vxb_result_unmapped_materials", "vxb_host_alloc", "vxb_host_free", "vxb_polygonize_sharded", "vxb_shard_configure",
                     "vxb_shard_buffers_get", "vxb_shard_set_peer", "vxb_shard_export", "vxb_shard_import", "vxb_shard_nccl_unique_id",
                     "vxb_shard_nccl_init", "vxb_grid_fill", "vxb_grid_inject_surface", "vxb_grid_inject_material", "vxb_grid_pack",
@@ -613,6 +614,12 @@ class Context:
     def set_launch_limit(self, ctas=0):
         """Test hook: at most `ctas` CTAs for the persistent kernels (0 = the default, occupancy-sized grids)."""
         self._check(self.L.vxb_set_launch_limit(self.h, ctas), "vxb_set_launch_limit")
+
+    def run_work_items(self, level):
+        """Test hook: (work items selected, blocks emitted) at `level` in the last completed run."""
+        items, emitted = C.c_uint32(0), C.c_uint32(0)
+        self._check(self.L.vxb_run_work_items(self.h, level, C.byref(items), C.byref(emitted)), "vxb_run_work_items")
+        return items.value, emitted.value
 
     def polygonize(self, max_levels=0, flags=0):
         self._check(self.L.vxb_polygonize(self.h, max_levels, flags), "vxb_polygonize")

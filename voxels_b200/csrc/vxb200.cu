@@ -108,7 +108,7 @@ struct vxb_context
 		}
 	} hostOffsets, hostRecords;
 	DevBuf<unsigned int> scanFlags;
-	DevBuf<unsigned char> blockInfo;
+	DevBuf<unsigned int> blockInfo;
 	DevBuf<unsigned int> consPages;
 	DevBuf<unsigned char> validFlags; // consValid + cacheValid[l] packed
 	DevBuf<unsigned short> cachePages;
@@ -128,6 +128,7 @@ struct vxb_context
 	bool haveLattice1 = false, latticeOff = false;
 	int gridBlock[3] = { 0, 0, 0 }, gridBigBlock = 0, gridTransition = 0;
 	uint32_t launchLimit = 0;      // vxb_set_launch_limit: cap on the persistent kernels' grids (0 = none)
+	uint32_t runWork[VXB_MAX_LEVELS] = { 0 }, runEmit[VXB_MAX_LEVELS] = { 0 }; // vxb_run_work_items: the last run's counters
 	unsigned persistentGrid(int grid) const { return launchLimit ? std::min<unsigned>((unsigned)grid, launchLimit) : (unsigned)grid; }
 	DevBuf<unsigned char> mixInfo, coarseDone;
 	DevBuf<unsigned short> mixCount;
@@ -1319,6 +1320,15 @@ int vxb_set_launch_limit(vxb_context* ctx, uint32_t ctas)
 	return VXB_OK;
 }
 
+int vxb_run_work_items(vxb_context* ctx, uint32_t level, uint32_t* items, uint32_t* emitted)
+{
+	if (!ctx || level >= VXB_MAX_LEVELS) return VXB_ERR_ARGUMENT;
+	if (!ctx->haveResult) return fail(ctx, VXB_ERR_STATE, "vxb_run_work_items: no run has completed");
+	if (items) *items = ctx->runWork[level];
+	if (emitted) *emitted = ctx->runEmit[level];
+	return VXB_OK;
+}
+
 } // extern "C"
 
 namespace
@@ -1564,7 +1574,7 @@ struct Run
 		{
 			// exchange 0: all-gather of the block info; every rank's layers are one contiguous chunk (rank-major layout)
 			const size_t chunk = blocksAtLevel(ctx->n, 0) / sh.world;
-			launch.bracket(8, [&] { rc = ncclApi().allGather(ctx->blockInfo.p + chunk * sh.rank, ctx->blockInfo.p, chunk, /*ncclUint8*/ 1, sh.comm, st); });
+			launch.bracket(8, [&] { rc = ncclApi().allGather(ctx->blockInfo.p + chunk * sh.rank, ctx->blockInfo.p, chunk * sizeof(unsigned int), /*ncclUint8*/ 1, sh.comm, st); });
 			if (rc != 0) return failNccl(ctx, "ncclAllGather (block info)", rc);
 		}
 		if (rc == VXB_OK) rc = enqueueLevels(launch);
@@ -1624,6 +1634,8 @@ struct Run
 		info.stats[3] = hc.degenerate;
 		for (int i = 0; i < 16; ++i) info.stats[4 + i] = hc.perCase[i];
 		for (int i = 0; i < 8; ++i) info.used_materials[i] = hc.usedMaterials[i];
+		memcpy(ctx->runWork, hc.workCount, sizeof(ctx->runWork));
+		memcpy(ctx->runEmit, hc.emitCount, sizeof(ctx->runEmit));
 		ctx->haveResult = true;
 		ctx->resultSharded = sharded; ctx->resultRegion = region != nullptr;
 		if (!region && !sharded) { ctx->haveFullRun = (computed == ctx->levels); ctx->nextId = (uint32_t)L.totalBlocks; }
@@ -1851,8 +1863,8 @@ int vxb_shard_buffers_get(vxb_context* ctx, vxb_shard_buffers* out)
 	VXB_CUDA(ctx, ctx->blockInfo.ensure(blocks0));
 	memset(out, 0, sizeof(*out));
 	out->block_info = ctx->blockInfo.p;
-	out->block_info_bytes = blocks0;
-	out->chunk_bytes = blocks0 / sh.world;
+	out->block_info_bytes = blocks0 * sizeof(unsigned int);
+	out->chunk_bytes = blocks0 / sh.world * sizeof(unsigned int);
 	out->pages = sh.pagesBuf;
 	out->pages_bytes = sh.pagesBytes;
 	out->valid = sh.valid(sh.pagesBuf);

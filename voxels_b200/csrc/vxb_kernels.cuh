@@ -2,9 +2,9 @@
 //
 // Pipeline per vxb_polygonize call (reference: TransVoxelRun::Execute, TransVoxelImpl.cpp:468-538):
 //   vxb_scan_kernel          streams the level-0 distance volume ONCE (coalesced 16-byte loads) and
-//                            reduces, per 16^3 block, sign/zero/lattice flags + a run-count bound
-//                            (VoxelGrid::CompressBlock's BF_Empty rule, VoxelGrid.cpp:610-672).
-//   vxb_block_info_kernel    turns the raw flags into BF_Empty / sign-mix bits (exact slow path when
+//                            reduces, per 16^3 block, sign/zero/lattice flags, the signs of its low faces + a
+//                            run-count bound (VoxelGrid::CompressBlock's BF_Empty rule, VoxelGrid.cpp:610-672).
+//   vxb_block_info_kernel    turns the raw flags into BF_Empty / sign-mix / low-face bits (exact slow path when
 //                            the run-count bound is inconclusive).
 //   vxb_select_kernel        per LOD level, the block walk (GenerateBlockListForLevel :385-466 + AreBlockAndNeighborsEmpty
 //                            :1511-1527): appends the blocks that can produce output or side effects.
@@ -17,12 +17,36 @@
 #define VXB_TILE_PITCH 32
 #define VXB_TILE_BYTES (17 * 17 * VXB_TILE_PITCH)
 
-// blockInfo bits (per level-0 block)
+// blockInfo bits (one word per level-0 block)
 #define VXB_BI_NEG 1u
 #define VXB_BI_NONNEG 2u
 #define VXB_BI_EMPTY 4u
 #define VXB_BI_NEG_E 8u      // level-1 lattice (even coordinates)
 #define VXB_BI_NONNEG_E 16u
+// low-face summaries: a (has a negative sample, has a non-negative one) bit pair at these shifts for the samples of the block
+// with local coordinate 0 on the named axes - the planes x = 0, y = 0, z = 0 and the lines x = y = 0, x = z = 0, y = z = 0 -
+// and the sign of the corner sample (0, 0, 0).  They are what the cells of the -x / -y / -z neighbours (and of the edge and
+// corner neighbours) sample of this block.
+#define VXB_BI_LOW_X 8
+#define VXB_BI_LOW_Y 10
+#define VXB_BI_LOW_Z 12
+#define VXB_BI_LOW_XY 14
+#define VXB_BI_LOW_XZ 16
+#define VXB_BI_LOW_YZ 18
+#define VXB_BI_CORNER_NEG (1u << 20)
+// the same summaries in vxb_scan_kernel's flag word (its bits 8-19 hold the in-row change count): the six pairs at bits
+// 20-31 (blockInfo's bits 8-19 shifted up by 12), the corner at bit 5
+#define VXB_SF_LOW_SHIFT 12
+#define VXB_SF_CORNER_NEG 32u
+
+// (neg, nonneg) of the samples of a block with local coordinate 0 on the axes set in `axes` (bit 0 = x, 1 = y, 2 = z; not 0)
+__device__ __forceinline__ unsigned vxb_bi_low(unsigned bi, int axes)
+{
+	if (axes == 7) return (bi & VXB_BI_CORNER_NEG) ? VXB_BI_NEG : VXB_BI_NONNEG;
+	const int shift = axes == 1 ? VXB_BI_LOW_X : axes == 2 ? VXB_BI_LOW_Y : axes == 4 ? VXB_BI_LOW_Z
+		: axes == 3 ? VXB_BI_LOW_XY : axes == 5 ? VXB_BI_LOW_XZ : VXB_BI_LOW_YZ;
+	return (bi >> shift) & 3u;
+}
 
 struct VxbCounters
 {
@@ -68,7 +92,7 @@ struct VxbDev
 	VxbGrid grid;
 	int n, levels, lastLevel;
 	unsigned int* scanFlags;
-	unsigned char* blockInfo;
+	unsigned int* blockInfo;                    // [nb0^3] VXB_BI_* (rank-major in sharded runs)
 	unsigned int* consPages;                    // [nb0^3][128]
 	unsigned char* consValid;                   // [nb0^3]
 	unsigned short* cachePages[VXB_MAX_LEVELS]; // level l >= 1: [nb_l^3][4096] {id, blend}
@@ -143,7 +167,7 @@ __device__ __forceinline__ int vxb_layer_slot(const VxbDev& d, int z)
 	return owner * perRank + (g / d.shardWorld) * d.shardLayers + z % d.shardLayers;
 }
 
-__device__ __forceinline__ const unsigned char* vxb_binfo_row(const VxbDev& d, int y, int z)
+__device__ __forceinline__ const unsigned int* vxb_binfo_row(const VxbDev& d, int y, int z)
 {
 	const int nb0 = d.n >> 4;
 	return d.blockInfo + ((size_t)vxb_layer_slot(d, z) * nb0 + y) * nb0;
@@ -286,6 +310,7 @@ __global__ void __launch_bounds__(VXB_THREADS, (J == 32 ? 3 : 4)) vxb_scan_kerne
 	__syncthreads();
 
 	unsigned neg = 0, pos = 0, zero = 0, negE = 0, nonnegE = 0, changes = 0;
+	unsigned low = 0; // the low-face summaries, at their bits of the flag word (VXB_SF_*)
 	if (bx0 + j < nb)
 	{
 		const uint4* src = reinterpret_cast<const uint4*>(dist + (((size_t)bz * 16) * n + (size_t)by * 16) * n + (size_t)(bx0 + j) * 16);
@@ -327,6 +352,17 @@ __global__ void __launch_bounds__(VXB_THREADS, (J == 32 ? 3 : 4)) vxb_scan_kerne
 					pos |= ~w[q] & 0x80808080u & ~zb;
 					if (even) { negE |= w[q] & 0x00800080u; nonnegE |= ~w[q] & 0x00800080u; }
 				}
+				{
+					// low faces (zero counts as non-negative, as in the case code): byte 0 of every row is on the plane x = 0,
+					// the rows with y = 0 / z = 0 are on those planes
+					const unsigned s0 = (w[0] & 0x80u) ? VXB_BI_NEG : VXB_BI_NONNEG;
+					const unsigned sr = (((w[0] | w[1] | w[2] | w[3]) & 0x80808080u) ? VXB_BI_NEG : 0u)
+						| (((w[0] & w[1] & w[2] & w[3] & 0x80808080u) != 0x80808080u) ? VXB_BI_NONNEG : 0u);
+					low |= s0 << (VXB_BI_LOW_X + VXB_SF_LOW_SHIFT);
+					if (y == 0) low |= (sr << (VXB_BI_LOW_Y + VXB_SF_LOW_SHIFT)) | (s0 << (VXB_BI_LOW_XY + VXB_SF_LOW_SHIFT));
+					if (z == 0) low |= (sr << (VXB_BI_LOW_Z + VXB_SF_LOW_SHIFT)) | (s0 << (VXB_BI_LOW_XZ + VXB_SF_LOW_SHIFT));
+					if ((y | z) == 0) low |= (sr << (VXB_BI_LOW_YZ + VXB_SF_LOW_SHIFT)) | ((w[0] & 0x80u) ? VXB_SF_CORNER_NEG : 0u);
+				}
 				if (!flat)
 				{
 #pragma unroll
@@ -344,7 +380,8 @@ __global__ void __launch_bounds__(VXB_THREADS, (J == 32 ? 3 : 4)) vxb_scan_kerne
 			}
 		}
 	}
-	unsigned f = (neg ? 1u : 0u) | (pos ? 2u : 0u) | (zero ? 4u : 0u) | (negE ? 8u : 0u) | (nonnegE ? 16u : 0u);
+	// bits 0-4: flags, 5 and 20-31: low faces; bits 8-19 take the in-row change count (<= 256 rows x 15 = 3840) below
+	unsigned f = (neg ? 1u : 0u) | (pos ? 2u : 0u) | (zero ? 4u : 0u) | (negE ? 8u : 0u) | (nonnegE ? 16u : 0u) | low;
 #pragma unroll
 	for (int o = J; o < 32; o <<= 1) { f |= __shfl_xor_sync(0xFFFFFFFFu, f, o); changes += __shfl_xor_sync(0xFFFFFFFFu, changes, o); } // lanes of the same block
 	if ((tid & 31) < J) { atomicOr(&sFlags[j], f); atomicAdd(&sChanges[j], changes); }
@@ -354,7 +391,7 @@ __global__ void __launch_bounds__(VXB_THREADS, (J == 32 ? 3 : 4)) vxb_scan_kerne
 }
 
 // K1b: raw flags -> blockInfo.  One thread per level-0 block.
-__global__ void vxb_block_info_kernel(const signed char* __restrict__ dist, int n, const unsigned int* __restrict__ scanFlags, unsigned char* __restrict__ blockInfo,
+__global__ void vxb_block_info_kernel(const signed char* __restrict__ dist, int n, const unsigned int* __restrict__ scanFlags, unsigned int* __restrict__ blockInfo,
 	size_t total /* blocks of this rank: whole layers, z-major */, int groupLayers, int world, int rank, int zBase /* as vxb_scan_kernel */)
 {
 	const int nb = n >> 4;
@@ -367,7 +404,7 @@ __global__ void vxb_block_info_kernel(const signed char* __restrict__ dist, int 
 		const size_t b = (size_t)tz * layerBlocks + q % layerBlocks;
 		const unsigned f = scanFlags[b];
 		const bool neg = f & 1, pos = f & 2, zero = f & 4;
-		const unsigned changes = f >> 8; // value changes inside 16-byte rows (lower bound of run ends)
+		const unsigned changes = (f >> 8) & 0xFFFu; // value changes inside 16-byte rows (lower bound of run ends)
 		bool empty = (neg != pos) && !zero; // every sample non-zero with one strict sign
 		if (empty)
 		{
@@ -391,14 +428,15 @@ __global__ void vxb_block_info_kernel(const signed char* __restrict__ dist, int 
 				}
 			}
 		}
-		blockInfo[world == 1 ? b : (size_t)rank * total + q] = (unsigned char)((neg ? VXB_BI_NEG : 0) | ((pos || zero) ? VXB_BI_NONNEG : 0) | (empty ? VXB_BI_EMPTY : 0)
-			| ((f & 8) ? VXB_BI_NEG_E : 0) | ((f & 16) ? VXB_BI_NONNEG_E : 0));
+		blockInfo[world == 1 ? b : (size_t)rank * total + q] = (neg ? VXB_BI_NEG : 0u) | ((pos || zero) ? VXB_BI_NONNEG : 0u) | (empty ? VXB_BI_EMPTY : 0u)
+			| ((f & 8) ? VXB_BI_NEG_E : 0u) | ((f & 16) ? VXB_BI_NONNEG_E : 0u)
+			| ((f >> VXB_SF_LOW_SHIFT) & (0xFFFu << VXB_BI_LOW_X)) | ((f & VXB_SF_CORNER_NEG) ? VXB_BI_CORNER_NEG : 0u);
 	}
 }
 
 // K1c: sign-mix pyramid over the level-0 blockInfo: mixInfo[l][b] = OR of (NEG, NONNEG) over the (2^l)^3 level-0 blocks that
 // block b of level l covers; mixCount[l][b] = how many of them hold both signs (the weight of a super-block in sharded runs).
-// vxb_pyramid_kernel: levels 1 and 2 straight from blockInfo, one thread per block (8 / 64 byte reads).
+// vxb_pyramid_kernel: levels 1 and 2 straight from blockInfo, one thread per block (8 / 64 word reads).
 // vxb_pyramid_top_kernel: levels >= 3 from their eight children, level by level, in ONE CTA (<= 4681 blocks in total).
 __global__ void __launch_bounds__(256) vxb_pyramid_kernel(const VxbDev d)
 {
@@ -417,7 +455,7 @@ __global__ void __launch_bounds__(256) vxb_pyramid_kernel(const VxbDev d)
 	unsigned u = 0, mixed = 0;
 	for (int z = 0; z < span; ++z) for (int y = 0; y < span; ++y)
 	{
-		const unsigned char* row = vxb_binfo_row(d, by * span + y, bz * span + z) + bx * span;
+		const unsigned int* row = vxb_binfo_row(d, by * span + y, bz * span + z) + bx * span;
 		for (int x = 0; x < span; ++x) { u |= row[x]; mixed += (row[x] & 3u) == 3u; }
 	}
 	d.mixInfo[level][q] = (unsigned char)(u & 3u);
@@ -638,31 +676,61 @@ __global__ void vxb_select_kernel(VxbDev d, int level)
 				if (!skip)
 				{
 					counted = true;
-					// cells of this block sample it and the first plane of its +1 neighbours (superset test)
-					unsigned u = 0;
-					for (int z = 0; z < 2; ++z) for (int y = 0; y < 2; ++y) for (int x = 0; x < 2; ++x)
+					// Exact test: the cells of this block sample the 17^3 points [0, 16]^3 - the block itself, the low plane of
+					// its +x / +y / +z neighbours, the low line of its three edge neighbours and the low corner of the +xyz one
+					// (a neighbour beyond the far grid edge adds nothing: its samples clamp onto points already counted).  Those points form
+					// a connected lattice whose every edge is an edge of one of the block's cells, so when they hold both signs
+					// some edge joins a negative sample to a non-negative one and its cell is non-trivial; without both signs
+					// no cell is.  A block that fails the test has no non-trivial cell and vxb_block_kernel<0> would write
+					// nothing for it: no page, no statistics, no histogram.
+					const bool hx = bx + 1 < nb, hy = by + 1 < nb, hz = bz + 1 < nb;
+					const unsigned* r00 = vxb_binfo_row(d, by, bz);
+					unsigned u = r00[bx] & 3u;
+					if (hx) u |= vxb_bi_low(r00[bx + 1], 1);
+					if (hy)
 					{
-						const int cx = min(bx + x, nb - 1), cy = min(by + y, nb - 1), cz = min(bz + z, nb - 1);
-						u |= vxb_binfo_row(d, cy, cz)[cx];
+						const unsigned* r10 = vxb_binfo_row(d, by + 1, bz);
+						u |= vxb_bi_low(r10[bx], 2);
+						if (hx) u |= vxb_bi_low(r10[bx + 1], 3);
 					}
-					take = (u & VXB_BI_NEG) && (u & VXB_BI_NONNEG);
+					if (hz)
+					{
+						const unsigned* r01 = vxb_binfo_row(d, by, bz + 1);
+						u |= vxb_bi_low(r01[bx], 4);
+						if (hx) u |= vxb_bi_low(r01[bx + 1], 5);
+						if (hy)
+						{
+							const unsigned* r11 = vxb_binfo_row(d, by + 1, bz + 1);
+							u |= vxb_bi_low(r11[bx], 6);
+							if (hx) u |= vxb_bi_low(r11[bx + 1], 7);
+						}
+					}
+					take = u == (VXB_BI_NEG | VXB_BI_NONNEG);
 				}
 			}
 			else if (level == 1)
 			{
-				// sign mix on the even lattice over the covered level-0 blocks + the far halo plane (superset);
-				// blocks on the far grid edge sample the clamped coordinate n-1, which is off the lattice.
+				// sign mix (superset) of the block's samples: the even lattice of the eight covered level-0 blocks, and of
+				// the +2 level-0 neighbours the samples at their local coordinate 0 on the +2 axes - the low plane, line or
+				// corner summary, which covers all of them.  Blocks on the far grid edge sample the clamped coordinate n-1,
+				// which is off the lattice: there every block of the neighbourhood adds its whole sign flags.
 				unsigned u = 0; bool anyChild = false;
 				const bool edge = (bx == nb - 1) || (by == nb - 1) || (bz == nb - 1);
-				for (int z = 0; z < 3; ++z) for (int y = 0; y < 3; ++y) for (int x = 0; x < 3; ++x)
-				{
-					const int cx = min(2 * bx + x, nb0 - 1), cy = min(2 * by + y, nb0 - 1), cz = min(2 * bz + z, nb0 - 1);
-					const size_t cb = ((size_t)cz * nb0 + cy) * nb0 + cx;
-					const unsigned bi = vxb_binfo_row(d, cy, cz)[cx];
-					u |= (bi >> 3) & 3u;
-					if (edge) u |= bi & 3u;
-					if (x < 2 && y < 2 && z < 2 && d.consValid[cb]) anyChild = true;
-				}
+#pragma unroll
+				for (int z = 0; z < 3; ++z)
+#pragma unroll
+					for (int y = 0; y < 3; ++y)
+#pragma unroll
+						for (int x = 0; x < 3; ++x)
+						{
+							const int cx = min(2 * bx + x, nb0 - 1), cy = min(2 * by + y, nb0 - 1), cz = min(2 * bz + z, nb0 - 1);
+							const size_t cb = ((size_t)cz * nb0 + cy) * nb0 + cx;
+							const unsigned bi = vxb_binfo_row(d, cy, cz)[cx];
+							const int far = (x == 2 ? 1 : 0) | (y == 2 ? 2 : 0) | (z == 2 ? 4 : 0);
+							u |= far ? vxb_bi_low(bi, far) : (bi >> 3) & 3u;
+							if (edge) u |= bi & 3u;
+							if (!far && d.consValid[cb]) anyChild = true;
+						}
 				take = (u == 3u) || anyChild;
 			}
 			else take = vxb_coarse_block_needed(d, level, bx, by, bz);
