@@ -414,6 +414,56 @@ int vxb_mesh_device_arenas(vxb_mesh* mesh, const vxb_block_record** records, con
 /* vxb_result_select_lod over the mesh's blocks; the lists are the mesh's own (the context's stay as they are) */
 int vxb_mesh_select_lod(vxb_mesh* mesh, const float camera[3], float base_distance, vxb_draw_lists* out);
 
+/* ---- ray queries against the mesh: picking, line of sight, projectile hits, without leaving HBM ------------------------
+ * Rays are cast against the LEVEL-0 regular triangles of the mesh (the full-detail surface, the one edits change); levels >= 1
+ * and transition meshes are not part of the query.
+ *   The hit     over every level-0 triangle that passes the test below, the one with the least t; ties go to the lower slot,
+ *               then to the lower triangle.  A pure function of the mesh (content and order) and the ray: it does not depend
+ *               on the launch configuration, on the variant or on the other rays of the batch.  Both faces are hit (no
+ *               back-face culling).  A miss: slot = VXB_RAY_MISS, t = +inf, every other field zero.
+ *   The test    Moeller-Trumbore in float32, in exactly this order (no fused multiply-add, IEEE division and square root):
+ *                 p0, p1, p2 = pos of vertices index[3k], index[3k+1], index[3k+2] (+ vertex_offset)
+ *                 e1 = p1 - p0; e2 = p2 - p0; s = o - p0                                   (per component)
+ *                 pv = d x e2: pvx = dy*e2z - dz*e2y; pvy = dz*e2x - dx*e2z; pvz = dx*e2y - dy*e2x
+ *                 det = (e1x*pvx + e1y*pvy) + e1z*pvz; inv = 1 / det
+ *                 u = ((sx*pvx + sy*pvy) + sz*pvz) * inv
+ *                 qv = s x e1 (same pattern): qvx = sy*e1z - sz*e1y; qvy = sz*e1x - sx*e1z; qvz = sx*e1y - sy*e1x
+ *                 v = ((dx*qvx + dy*qvy) + dz*qvz) * inv
+ *                 t = ((e2x*qvx + e2y*qvy) + e2z*qvz) * inv
+ *                 hit iff det != 0 && u >= 0 && u <= 1 && v >= 0 && u + v <= 1 && t >= t_min && t <= t_max
+ *               (positive comparisons: a NaN - a tiny det makes inv infinite and u NaN - fails the test).
+ *   position    o_i + t * d_i
+ *   normal      w = (1 - u) - v; n_i = (w*n0_i + u*n1_i) + v*n2_i; len = sqrt((nx*nx + ny*ny) + nz*nz); n_i / len if len > 0,
+ *               else (0, 0, 0)
+ * A level-0 triangle lies in the closed box of its block.  The walk tests the triangles of every block whose box, grown by
+ * 1/16 voxel, meets the segment; an accepted hit lies within rounding of its triangle (far less than 1/16 voxel unless det
+ * is close to zero), so this is every triangle that can pass the test.
+ * Refusals: VXB_ERR_STATE before the first vxb_mesh_apply; VXB_ERR_ARGUMENT for a NULL pointer with count > 0; count = 0 does
+ * nothing.  The HOST variant also refuses with VXB_ERR_ARGUMENT, naming the ray index in vxb_last_error and writing nothing to
+ * `hits`, a ray with a non-finite origin or direction, a zero direction, a NaN or non-finite t_min, a NaN t_max or
+ * t_min > t_max.  The DEVICE variant cannot read the rays before it runs: there such a ray is a miss.
+ * The first cast after an apply (or after the mesh changed grid size) also rebuilds a per-mesh map from level-0 block
+ * coordinates to slots ((n/16)^3 x 4 bytes: 1 MB at 1024^3), stream-ordered before the cast. */
+/* One ray in OUTPUT (Y-up) coordinates, the space of the vertices and of vxb_mesh_select_lod's camera.  The direction
+ * need not be unit length; t is in units of it.  The ray is the segment origin + t * direction, t in [t_min, t_max]
+ * (both inclusive; t_max may be +inf). */
+typedef struct vxb_ray { float origin[3]; float t_min; float direction[3]; float t_max; } vxb_ray;          /* 32 bytes */
+#define VXB_RAY_MISS 0xFFFFFFFFu   /* a macro, not an enum: ISO C limits enumerators to the range of int */
+typedef struct vxb_ray_hit
+{
+	float t, u, v;          /* ray parameter; barycentrics of the triangle's 2nd and 3rd vertex */
+	uint32_t slot;          /* mesh directory slot of the block (vxb_mesh_device_arenas / vxb_mesh_download order); VXB_RAY_MISS */
+	uint32_t block_id;      /* vxb_block_record.id of that block */
+	uint32_t triangle;      /* k: the triangle is indices [index_offset + 3k, index_offset + 3k + 3) of the block */
+	float position[3];      /* origin + t * direction */
+	float normal[3];        /* the vertex normals blended at (u, v), normalised; (0,0,0) when the blend is zero */
+} vxb_ray_hit;                                                                                               /* 48 bytes */
+/* HOST memory; blocks until the hits are written. */
+int vxb_mesh_raycast(vxb_mesh* mesh, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits);
+/* DEVICE memory; enqueued on vxb_stream(ctx) after everything queued there (an apply included), returns without waiting.
+ * The mesh's state at the call is what the cast sees: a later apply is queued after it. */
+int vxb_mesh_raycast_device(vxb_mesh* mesh, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits);
+
 /* GetMaterial(id) == nullptr handling (TransVoxelImpl.cpp:1364-1368: textures stay zero, one LS_Error log per
  * vertex): after vxb_result_download the material ids of those vertices, in the reference's logging order
  * (level, block, regular vertices, then transition faces), can be read here.  Returns the count; copies at

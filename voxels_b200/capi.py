@@ -163,6 +163,24 @@ class DrawLists(C.Structure):
 DRAW_COMMAND_DTYPE = np.dtype([("index_count", "<u4"), ("instance_count", "<u4"), ("first_index", "<u4"), ("base_vertex", "<i4"), ("first_instance", "<u4")])
 DRAW_INFO_DTYPE = np.dtype([("block_id", "<u4"), ("level", "<u4"), ("block_adj", "<u4"), ("face", "<u4")])
 
+# vxb_ray / vxb_ray_hit (include/vxb200.h "ray queries")
+VXB_RAY_MISS = 0xFFFFFFFF
+RAY_DTYPE = np.dtype([("origin", "<f4", 3), ("t_min", "<f4"), ("direction", "<f4", 3), ("t_max", "<f4")])
+RAY_HIT_DTYPE = np.dtype([("t", "<f4"), ("u", "<f4"), ("v", "<f4"), ("slot", "<u4"), ("block_id", "<u4"), ("triangle", "<u4"),
+                          ("position", "<f4", 3), ("normal", "<f4", 3)])
+assert RAY_DTYPE.itemsize == 32 and RAY_HIT_DTYPE.itemsize == 48
+
+
+def make_rays(origins, directions, t_min=0.0, t_max=np.inf):
+    """A RAY_DTYPE array from [count, 3] origins and directions (OUTPUT, Y-up coordinates); t_min / t_max: scalars or [count]."""
+    o = np.asarray(origins, np.float32).reshape(-1, 3)
+    d = np.asarray(directions, np.float32).reshape(-1, 3)
+    rays = np.zeros(len(o), RAY_DTYPE)
+    rays["origin"], rays["direction"] = o, d
+    rays["t_min"], rays["t_max"] = np.float32(t_min) if np.isscalar(t_min) else np.asarray(t_min, np.float32), \
+        np.float32(t_max) if np.isscalar(t_max) else np.asarray(t_max, np.float32)
+    return rays
+
 
 class MeshInfo(C.Structure):
     """vxb_mesh_info (include/vxb200.h)."""
@@ -275,6 +293,8 @@ def load_library():
         "vxb_mesh_download": (C.c_int, [vp, vp, vp, vp, vp, vp]),
         "vxb_mesh_device_arenas": (C.c_int, [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
         "vxb_mesh_select_lod": (C.c_int, [vp, vp, C.c_float, C.POINTER(DrawLists)]),
+        "vxb_mesh_raycast": (C.c_int, [vp, vp, u32, vp]),
+        "vxb_mesh_raycast_device": (C.c_int, [vp, vp, u32, vp]),
         "vxb_host_alloc": (vp, [C.c_size_t]),
         "vxb_host_free": (None, [vp]),
     }
@@ -295,7 +315,7 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_grid_upload_packed_streamed", "vxb_result_download_begin", "vxb_result_download_end",
                     "vxb_grid_fill_program", "vxb_grid_inject_program", "vxb_grid_program_stats",
                     "vxb_mesh_create", "vxb_mesh_destroy", "vxb_mesh_apply", "vxb_mesh_info_get", "vxb_mesh_download",
-                    "vxb_mesh_device_arenas", "vxb_mesh_select_lod"]
+                    "vxb_mesh_device_arenas", "vxb_mesh_select_lod", "vxb_mesh_raycast", "vxb_mesh_raycast_device"]
 
 
 def nccl_unique_id():
@@ -453,6 +473,26 @@ class Mesh:
                 _device_to_numpy(lists.regular_info, lists.regular_count, DRAW_INFO_DTYPE),
                 _device_to_numpy(lists.transition, lists.transition_count, DRAW_COMMAND_DTYPE),
                 _device_to_numpy(lists.transition_info, lists.transition_count, DRAW_INFO_DTYPE))
+
+    def raycast_rc(self, rays, hits=None):
+        """vxb_mesh_raycast's return code for a RAY_DTYPE array; the hits go to `hits` (a RAY_HIT_DTYPE array, or None for a
+        NULL pointer)."""
+        rays = np.ascontiguousarray(rays, RAY_DTYPE) if rays is not None else None
+        return self.L.vxb_mesh_raycast(self.h, _ptr(rays), 0 if rays is None else len(rays), _ptr(hits))
+
+    def raycast(self, origins, directions=None, t_min=0.0, t_max=np.inf):
+        """Casts rays against the mesh's level-0 triangles (vxb_mesh_raycast): `origins` / `directions` are [count, 3] in OUTPUT
+        (Y-up) coordinates, or `origins` is a RAY_DTYPE array and `directions` None.  Returns a RAY_HIT_DTYPE array."""
+        rays = np.ascontiguousarray(origins if directions is None else make_rays(origins, directions, t_min, t_max), RAY_DTYPE)
+        hits = np.zeros(len(rays), RAY_HIT_DTYPE)
+        self.ctx._check(self.L.vxb_mesh_raycast(self.h, _ptr(rays), len(rays), _ptr(hits)), "vxb_mesh_raycast")
+        return hits
+
+    def raycast_device(self, rays_ptr, count, hits_ptr):
+        """vxb_mesh_raycast_device: `count` vxb_ray at the device address `rays_ptr`, hits to `hits_ptr` (e.g. torch tensors'
+        data_ptr()); enqueued on the context's stream, returns without waiting."""
+        self.ctx._check(self.L.vxb_mesh_raycast_device(self.h, None if rays_ptr is None else C.c_void_p(rays_ptr), count,
+                                                       None if hits_ptr is None else C.c_void_p(hits_ptr)), "vxb_mesh_raycast_device")
 
 
 class Context:

@@ -8,6 +8,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <memory>
@@ -31,9 +32,11 @@
 #include "vxb_grid.cuh"
 #include "vxb_draw.cuh"
 #include "vxb_mesh.cuh"
+#include "vxb_ray.cuh"
 
 static_assert(sizeof(VxbVertex) == 48, "PolygonVertex layout");
 static_assert(sizeof(vxb_block_record) == 128, "record layout");
+static_assert(sizeof(vxb_ray) == 32 && sizeof(vxb_ray_hit) == 48, "ray layouts");
 
 namespace
 {
@@ -2192,6 +2195,13 @@ struct vxb_mesh
 	uint64_t serial = 0;                        // vxb_context::runSerial of that run
 	uint32_t n = 0;
 	vxb_mesh_info info;
+	// ray casts (vxb_ray.cuh): the level-0 coord_id -> slot map, built for the applied run `mapSerial` on a grid of `mapN`
+	DevBuf<unsigned int> rayMap;
+	bool mapBuilt = false;
+	uint64_t mapSerial = 0;
+	uint32_t mapN = 0;
+	DevBuf<vxb_ray> rayIn;                      // vxb_mesh_raycast's device staging, grown as needed
+	DevBuf<vxb_ray_hit> rayOut;
 };
 
 namespace
@@ -2203,6 +2213,52 @@ void deleteMesh(vxb_mesh* m)
 }
 
 uint64_t grownCapacity(uint64_t live) { return (std::max<uint64_t>(live + live / 2, 1024) + 3) & ~(uint64_t)3; }
+
+// The map for the applied run (rebuilt after every apply: each one has a new serial) and the cast, both on ctx->stream.
+int enqueueRaycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits)
+{
+	vxb_context* ctx = m->ctx;
+	cudaStream_t st = ctx->stream;
+	const uint32_t nb = m->n / 16;
+	if (!m->mapBuilt || m->mapSerial != m->serial || m->mapN != m->n)
+	{
+		const size_t cells = (size_t)nb * nb * nb;
+		if (cells > m->rayMap.count)
+		{
+			VXB_CUDA(ctx, cudaStreamSynchronize(st)); // a cast still queued may read the old map
+			VXB_CUDA(ctx, m->rayMap.ensure(cells));
+		}
+		VXB_CUDA(ctx, cudaMemsetAsync(m->rayMap.p, 0xFF, cells * sizeof(unsigned int), st));
+		const unsigned level0 = m->info.level_blocks[0];
+		if (level0) vxb_ray_map_kernel<<<(level0 + 255) / 256, 256, 0, st>>>(m->dir.p, level0, m->rayMap.p);
+		VXB_CUDA(ctx, cudaGetLastError());
+		m->mapBuilt = true; m->mapSerial = m->serial; m->mapN = m->n;
+	}
+	VxbRayMesh rm;
+	rm.dir = m->dir.p; rm.map = m->rayMap.p; rm.verts = m->set[m->active].v.p; rm.idx = m->set[m->active].i.p; rm.nb = (int)nb;
+	const unsigned warpsPerCta = VXB_RAY_THREADS / 32;
+	const unsigned ctas = std::min<unsigned>((count + warpsPerCta - 1) / warpsPerCta, (unsigned)std::max(ctx->smCount, 1) * 8);
+	vxb_raycast_kernel<<<ctas, VXB_RAY_THREADS, 0, st>>>(rm, rays, count, hits);
+	VXB_CUDA(ctx, cudaGetLastError());
+	return VXB_OK;
+}
+
+// the host variant's argument rule (include/vxb200.h): the index of the first invalid ray, or -1
+long long invalidRay(const vxb_ray* rays, uint32_t count, const char** why)
+{
+	for (uint32_t r = 0; r < count; ++r)
+	{
+		const vxb_ray& x = rays[r];
+		bool finite = true;
+		for (int a = 0; a < 3; ++a) finite = finite && std::isfinite(x.origin[a]) && std::isfinite(x.direction[a]);
+		if (!finite) { *why = "non-finite origin or direction"; return r; }
+		if (x.direction[0] == 0.f && x.direction[1] == 0.f && x.direction[2] == 0.f) { *why = "zero direction"; return r; }
+		if (!std::isfinite(x.t_min)) { *why = "t_min is NaN or infinite"; return r; }
+		if (std::isnan(x.t_max)) { *why = "t_max is NaN"; return r; }
+		if (x.t_min > x.t_max) { *why = "t_min > t_max"; return r; }
+	}
+	return -1;
+}
 }
 
 extern "C"
@@ -2450,6 +2506,46 @@ int vxb_mesh_select_lod(vxb_mesh* m, const float camera[3], float baseDistance, 
 	if (r != VXB_OK) return r;
 	if (out) *out = m->drawLists;
 	return VXB_OK;
+}
+
+int vxb_mesh_raycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (count && (!rays || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_raycast: NULL rays or hits");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_raycast: nothing applied yet");
+	if (!count) return VXB_OK;
+	const char* why = "";
+	const long long bad = invalidRay(rays, count, &why);
+	if (bad >= 0)
+	{
+		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_raycast: ray %lld: %s", bad, why);
+		return fail(ctx, VXB_ERR_ARGUMENT, buf);
+	}
+	cudaSetDevice(ctx->device);
+	cudaStream_t st = ctx->stream;
+	if (count > m->rayIn.count || count > m->rayOut.count)
+	{
+		VXB_CUDA(ctx, cudaStreamSynchronize(st)); // nothing queued may still use the staging being replaced
+		VXB_CUDA(ctx, m->rayIn.ensure(count)); VXB_CUDA(ctx, m->rayOut.ensure(count));
+	}
+	VXB_CUDA(ctx, cudaMemcpyAsync(m->rayIn.p, rays, sizeof(vxb_ray) * count, cudaMemcpyHostToDevice, st));
+	const int r = enqueueRaycast(m, m->rayIn.p, count, m->rayOut.p);
+	if (r != VXB_OK) return r;
+	VXB_CUDA(ctx, cudaMemcpyAsync(hits, m->rayOut.p, sizeof(vxb_ray_hit) * count, cudaMemcpyDeviceToHost, st));
+	VXB_CUDA(ctx, cudaStreamSynchronize(st));
+	return VXB_OK;
+}
+
+int vxb_mesh_raycast_device(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (count && (!rays || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_raycast_device: NULL rays or hits");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_raycast_device: nothing applied yet");
+	if (!count) return VXB_OK;
+	cudaSetDevice(ctx->device);
+	return enqueueRaycast(m, rays, count, hits);
 }
 
 } // extern "C"

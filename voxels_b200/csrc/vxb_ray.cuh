@@ -1,0 +1,226 @@
+// Ray casts against the level-0 triangles of the resident mesh (include/vxb200.h "vxb_mesh_raycast").
+//
+// Level-0 vertices lie on the cell edges of their own block (t in [0, 256], exact dyadic positions), so every level-0
+// triangle lies in the closed box of its block.  A ray therefore only needs the triangles of the blocks whose box it meets.
+// The walk visits those blocks with a 3-D DDA (Amanatides-Woo) over the level-0 block lattice, made conservative:
+//
+//   tested set   every block whose closed box grown by VXB_RAY_EPS meets the clipped segment (te <= tx below).  A triangle
+//                the test accepts has its hit point within rounding (about 1e-3 voxel at n = 4096 for a well-conditioned
+//                test) of the triangle, hence inside the grown box of its block; so no accepted hit is lost to the walk.
+//   anchoring    a tested block is handled at the DDA cell whose parameter interval [t0, t1) holds the block's grown-box
+//                entry te (the last cell's interval is closed).  The intervals of the visited cells partition the clipped
+//                segment exactly (each t1 is the next cell's t0, the same float), so every tested block is handled exactly
+//                once.  The ray point at te is within VXB_RAY_EPS (+ rounding) of the block and inside the anchor cell (up to
+//                rounding), so the block is one of the anchor cell's 27 neighbours: lane k of the warp evaluates neighbour k.
+//                This covers rays in a block face plane (two columns), along a block edge (four) and through corners (eight).
+//   stop         after cell c, every block not handled yet has te >= t1(c).  te = (plane - o) / d is two correctly rounded
+//                operations, so the true entry is at least t1 - 2^-22 |t1|, and a hit in that block (inside its grown box) has
+//                t >= that.  With the margin 2^-20 |t1|, t1 > best + margin proves t > best for every remaining hit: no hit
+//                can tie or beat the best one, and the walk ends.
+#pragma once
+
+#include <math_constants.h>
+
+#define VXB_RAY_EPS 0.0625f        // growth of a block's box in voxels (1/16: a multiple of 2^-4, so 16 b +- eps is exact)
+#define VXB_RAY_MARGIN_EXP (-20)   // stop margin: 2^-20 |t1| (te is within 2^-22 |te| of its true value, see above)
+#define VXB_RAY_THREADS 256
+
+// the dense level-0 map: coord_id -> mesh directory slot (VXB_RAY_MISS where no block is), after a memset to 0xFF
+__global__ void __launch_bounds__(256) vxb_ray_map_kernel(const vxb_block_record* __restrict__ dir, unsigned count, unsigned* __restrict__ map)
+{
+	const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < count) map[__ldg(&dir[i].coord_id)] = i;
+}
+
+struct VxbRayMesh
+{
+	const vxb_block_record* dir;   // mesh directory (level 0 first)
+	const unsigned* map;           // nb^3 slots, grid (Z-up) coord_id order
+	const VxbVertex* verts;
+	const unsigned* idx;
+	int nb;                        // level-0 blocks per axis
+};
+
+// entry / exit parameters of the slab [lo, hi] along one axis; d == 0 (either sign): all t, or none when o is outside
+VXB_FN void vxb_ray_slab(float o, float d, float lo, float hi, float& tin, float& tout)
+{
+	if (d == 0.f)
+	{
+		if (!(o >= lo && o <= hi)) { tin = CUDART_INF_F; tout = -CUDART_INF_F; }
+		return;
+	}
+	float a = VXB_DIV(lo - o, d), b = VXB_DIV(hi - o, d);
+	if (d < 0.f) { const float s = a; a = b; b = s; }
+	tin = fmaxf(tin, a); tout = fminf(tout, b);
+}
+
+// the grown box of block index b along one axis
+VXB_FN float vxb_ray_lo(int b) { return (float)(16 * b) - VXB_RAY_EPS; }
+VXB_FN float vxb_ray_hi(int b) { return (float)(16 * b + 16) + VXB_RAY_EPS; }
+
+// the next cell boundary crossed along one axis (ungrown planes); +inf when the step would leave the grid
+VXB_FN float vxb_ray_next(int c, float o, float d, int nb)
+{
+	if (d > 0.f && c + 1 < nb) return VXB_DIV((float)(16 * (c + 1)) - o, d);
+	if (d < 0.f && c > 0) return VXB_DIV((float)(16 * c) - o, d);
+	return CUDART_INF_F;
+}
+
+VXB_FN bool vxb_ray_valid(const vxb_ray& r)
+{
+	const bool finite = isfinite(r.origin[0]) && isfinite(r.origin[1]) && isfinite(r.origin[2]) && isfinite(r.direction[0]) &&
+		isfinite(r.direction[1]) && isfinite(r.direction[2]) && isfinite(r.t_min) && !isnan(r.t_max);
+	const bool nonzero = r.direction[0] != 0.f || r.direction[1] != 0.f || r.direction[2] != 0.f;
+	return finite && nonzero && r.t_min <= r.t_max;
+}
+
+// (t, slot, triangle) ordered by the tie rule: least t, then lower slot, then lower triangle
+VXB_FN bool vxb_ray_before(float t, unsigned s, unsigned k, float t2, unsigned s2, unsigned k2)
+{
+	return t < t2 || (t == t2 && (s < s2 || (s == s2 && k < k2)));
+}
+
+// One warp per ray, persistent over the batch.  Rays and hits in OUTPUT (Y-up) coordinates; block coordinates of the map
+// are grid (Z-up): output (x, y, z) = grid (x, z, y).
+__global__ void __launch_bounds__(VXB_RAY_THREADS) vxb_raycast_kernel(const VxbRayMesh m, const vxb_ray* __restrict__ rays, unsigned count,
+	vxb_ray_hit* __restrict__ hits)
+{
+	const unsigned lane = threadIdx.x & 31;
+	const unsigned warps = gridDim.x * (VXB_RAY_THREADS / 32);
+	const int nb = m.nb;
+	const float n = (float)(16 * nb);
+	// this lane's neighbour offset (lanes 27..31 have none)
+	const int ox = (int)(lane % 3) - 1, oy = (int)((lane / 3) % 3) - 1, oz = (int)(lane / 9) - 1;
+	for (unsigned r = blockIdx.x * (VXB_RAY_THREADS / 32) + (threadIdx.x >> 5); r < count; r += warps)
+	{
+		const vxb_ray ray = rays[r];
+		const float px = ray.origin[0], py = ray.origin[1], pz = ray.origin[2];
+		const float dx = ray.direction[0], dy = ray.direction[1], dz = ray.direction[2];
+		const float tMin = ray.t_min, tMax = ray.t_max;
+		float bt = CUDART_INF_F, bu = 0.f, bv = 0.f;   // this lane's best hit
+		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
+		// ---- clip to the grown grid box [-eps, n + eps]^3 (the union of the grown block boxes, computed with the same planes) ----
+		float T0 = tMin, T1 = tMax;
+		bool live = vxb_ray_valid(ray);
+		if (live)
+		{
+			vxb_ray_slab(px, dx, -VXB_RAY_EPS, n + VXB_RAY_EPS, T0, T1);
+			vxb_ray_slab(py, dy, -VXB_RAY_EPS, n + VXB_RAY_EPS, T0, T1);
+			vxb_ray_slab(pz, dz, -VXB_RAY_EPS, n + VXB_RAY_EPS, T0, T1);
+			live = T0 <= T1;
+		}
+		if (live)
+		{
+			// the first cell: the block of the clipped entry point, clamped into the grid
+			int cx = min(max((int)floorf((px + T0 * dx) * 0.0625f), 0), nb - 1);
+			int cy = min(max((int)floorf((py + T0 * dy) * 0.0625f), 0), nb - 1);
+			int cz = min(max((int)floorf((pz + T0 * dz) * 0.0625f), 0), nb - 1);
+			float nx = vxb_ray_next(cx, px, dx, nb), ny = vxb_ray_next(cy, py, dy, nb), nz = vxb_ray_next(cz, pz, dz, nb);
+			float t0 = T0;
+			for (;;)
+			{
+				const float tn = fminf(nx, fminf(ny, nz));
+				const bool last = !(tn < T1);
+				const float t1 = last ? T1 : fmaxf(tn, t0);
+				// ---- the neighbours anchored in [t0, t1) ----
+				const int bx = cx + ox, by = cy + oy, bz = cz + oz;
+				bool cand = false;
+				unsigned slot = VXB_RAY_MISS;
+				if (lane < 27 && bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb)
+				{
+					float te = T0, tx = T1;
+					vxb_ray_slab(px, dx, vxb_ray_lo(bx), vxb_ray_hi(bx), te, tx);
+					vxb_ray_slab(py, dy, vxb_ray_lo(by), vxb_ray_hi(by), te, tx);
+					vxb_ray_slab(pz, dz, vxb_ray_lo(bz), vxb_ray_hi(bz), te, tx);
+					if (te <= tx && te >= t0 && (te < t1 || last))
+					{
+						slot = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
+						cand = slot != VXB_RAY_MISS;
+					}
+				}
+				unsigned todo = __ballot_sync(0xFFFFFFFFu, cand);
+				const bool tested = todo != 0;
+				while (todo)
+				{
+					const unsigned src = __ffs(todo) - 1;
+					todo &= todo - 1;
+					const unsigned s = __shfl_sync(0xFFFFFFFFu, slot, src);
+					const vxb_block_record* rec = m.dir + s;
+					const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
+					for (unsigned k = lane; k < tris; k += 32)
+					{
+						const unsigned* ip = m.idx + io + 3 * k;
+						const float* a = m.verts[vo + __ldg(ip)].pos;
+						const float* b = m.verts[vo + __ldg(ip + 1)].pos;
+						const float* c = m.verts[vo + __ldg(ip + 2)].pos;
+						const float p0x = __ldg(a), p0y = __ldg(a + 1), p0z = __ldg(a + 2);
+						const float e1x = __ldg(b) - p0x, e1y = __ldg(b + 1) - p0y, e1z = __ldg(b + 2) - p0z;
+						const float e2x = __ldg(c) - p0x, e2y = __ldg(c + 1) - p0y, e2z = __ldg(c + 2) - p0z;
+						const float sx = px - p0x, sy = py - p0y, sz = pz - p0z;
+						// Moeller-Trumbore exactly as include/vxb200.h states it (-fmad=false: no contraction)
+						const float pvx = dy * e2z - dz * e2y, pvy = dz * e2x - dx * e2z, pvz = dx * e2y - dy * e2x;
+						const float det = (e1x * pvx + e1y * pvy) + e1z * pvz;
+						const float inv = VXB_DIV(1.f, det);
+						const float u = ((sx * pvx + sy * pvy) + sz * pvz) * inv;
+						const float qvx = sy * e1z - sz * e1y, qvy = sz * e1x - sx * e1z, qvz = sx * e1y - sy * e1x;
+						const float v = ((dx * qvx + dy * qvy) + dz * qvz) * inv;
+						const float t = ((e2x * qvx + e2y * qvy) + e2z * qvz) * inv;
+						// positive comparisons only: a NaN fails
+						if (det != 0.f && u >= 0.f && u <= 1.f && v >= 0.f && u + v <= 1.f && t >= tMin && t <= tMax &&
+							vxb_ray_before(t, s, k, bt, bs, bk))
+						{
+							bt = t; bs = s; bk = k; bu = u; bv = v;
+						}
+					}
+				}
+				if (last) break;
+				if (tested)
+				{
+					float w = bt;
+					for (int o = 16; o > 0; o >>= 1) w = fminf(w, __shfl_xor_sync(0xFFFFFFFFu, w, o));
+					if (t1 > w + ldexpf(fabsf(t1), VXB_RAY_MARGIN_EXP)) break;
+				}
+				// ---- step across the nearest boundary (ties: x, then y, then z; the others follow with empty intervals) ----
+				if (nx == tn) { cx += dx > 0.f ? 1 : -1; nx = vxb_ray_next(cx, px, dx, nb); }
+				else if (ny == tn) { cy += dy > 0.f ? 1 : -1; ny = vxb_ray_next(cy, py, dy, nb); }
+				else { cz += dz > 0.f ? 1 : -1; nz = vxb_ray_next(cz, pz, dz, nb); }
+				t0 = t1;
+			}
+		}
+		// ---- the winner by the tie rule; its lane writes the hit ----
+		float wt = bt; unsigned ws = bs, wk = bk;
+		for (int o = 16; o > 0; o >>= 1)
+		{
+			const float t2 = __shfl_xor_sync(0xFFFFFFFFu, wt, o);
+			const unsigned s2 = __shfl_xor_sync(0xFFFFFFFFu, ws, o), k2 = __shfl_xor_sync(0xFFFFFFFFu, wk, o);
+			if (vxb_ray_before(t2, s2, k2, wt, ws, wk)) { wt = t2; ws = s2; wk = k2; }
+		}
+		const unsigned winner = __ffs(__ballot_sync(0xFFFFFFFFu, bs == ws && bk == wk)) - 1;
+		if (lane == winner)
+		{
+			vxb_ray_hit h;
+			h.u = 0.f; h.v = 0.f; h.slot = VXB_RAY_MISS; h.block_id = 0; h.triangle = 0;
+			h.t = CUDART_INF_F;
+			h.position[0] = h.position[1] = h.position[2] = 0.f;
+			h.normal[0] = h.normal[1] = h.normal[2] = 0.f;
+			if (bs != VXB_RAY_MISS)
+			{
+				const vxb_block_record* rec = m.dir + bs;
+				const unsigned vo = __ldg(&rec->vertex_offset);
+				const unsigned* ip = m.idx + __ldg(&rec->index_offset) + 3 * bk;
+				const float* n0 = m.verts[vo + __ldg(ip)].nrm;
+				const float* n1 = m.verts[vo + __ldg(ip + 1)].nrm;
+				const float* n2 = m.verts[vo + __ldg(ip + 2)].nrm;
+				h.t = bt; h.u = bu; h.v = bv; h.slot = bs; h.block_id = __ldg(&rec->id); h.triangle = bk;
+				h.position[0] = px + bt * dx; h.position[1] = py + bt * dy; h.position[2] = pz + bt * dz;
+				const float w = (1.f - bu) - bv;
+				const float nxv = (w * __ldg(n0) + bu * __ldg(n1)) + bv * __ldg(n2);
+				const float nyv = (w * __ldg(n0 + 1) + bu * __ldg(n1 + 1)) + bv * __ldg(n2 + 1);
+				const float nzv = (w * __ldg(n0 + 2) + bu * __ldg(n1 + 2)) + bv * __ldg(n2 + 2);
+				const float len = VXB_SQRT((nxv * nxv + nyv * nyv) + nzv * nzv);
+				if (len > 0.f) { h.normal[0] = VXB_DIV(nxv, len); h.normal[1] = VXB_DIV(nyv, len); h.normal[2] = VXB_DIV(nzv, len); }
+			}
+			hits[r] = h;
+		}
+	}
+}
