@@ -464,6 +464,100 @@ int vxb_mesh_raycast(vxb_mesh* mesh, const vxb_ray* rays, uint32_t count, vxb_ra
  * The mesh's state at the call is what the cast sees: a later apply is queued after it. */
 int vxb_mesh_raycast_device(vxb_mesh* mesh, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits);
 
+/* ---- collision queries against the mesh: sphere sweeps and closest points, for character controllers and cameras -------
+ * Like the ray queries: the LEVEL-0 regular triangles only, both faces, OUTPUT (Y-up) coordinates, a pure function of the
+ * mesh (content and order) and of the query (not of the launch, the variant or the rest of the batch), float32 with no fused
+ * multiply-add, IEEE division and square root, in exactly the order written here.  x.y = (xx*yx + xy*yy) + xz*yz with the
+ * left operand as written; a x b = (ay*bz - az*by, az*bx - ax*bz, ax*by - ay*bx).
+ *   Closest point of triangle (a, b, c) (p0, p1, p2 as for the rays) to a point p: Ericson's ClosestPtPointTriangle, the
+ *   regions tested in this order, the first that holds gives point, u (weight of b) and v (weight of c):
+ *     ab = b - a; ac = c - a; ap = p - a; d1 = ab.ap; d2 = ac.ap
+ *     A    d1 <= 0 && d2 <= 0                                  point = a, u = 0, v = 0
+ *          bp = p - b; d3 = ab.bp; d4 = ac.bp
+ *     B    d3 >= 0 && d4 <= d3                                 point = b, u = 1, v = 0
+ *          vc = d1*d4 - d3*d2
+ *     AB   vc <= 0 && d1 >= 0 && d3 <= 0                       w = d1 / (d1 - d3); point_i = a_i + w*ab_i, u = w, v = 0
+ *          cp = p - c; d5 = ab.cp; d6 = ac.cp
+ *     C    d6 >= 0 && d5 <= d6                                 point = c, u = 0, v = 1
+ *          vb = d5*d2 - d1*d6
+ *     AC   vb <= 0 && d2 >= 0 && d6 <= 0                       w = d2 / (d2 - d6); point_i = a_i + w*ac_i, u = 0, v = w
+ *          va = d3*d6 - d5*d4
+ *     BC   va <= 0 && (d4 - d3) >= 0 && (d5 - d6) >= 0         w = (d4 - d3) / ((d4 - d3) + (d5 - d6));
+ *                                                              point_i = b_i + w*(c_i - b_i), u = 1 - w, v = w
+ *     face otherwise                                           den = 1 / ((va + vb) + vc); u = vb*den; v = vc*den;
+ *                                                              point_i = (a_i + ab_i*u) + ac_i*v
+ *   and dd = (qx*qx + qy*qy) + qz*qz with q = p - point.
+ *   Normal: the ray hit's blended normal at (u, v).
+ *
+ *   vxb_mesh_closest_point: for a query point p and max_distance m, every level-0 triangle with dd <= m*m (inclusive, m*m
+ *     in float) is a candidate; the result is the one with the least dd, then the lower slot, then the lower triangle, with
+ *     distance = sqrt(dd).  A miss: slot = VXB_RAY_MISS, distance = +inf, every other field zero.  This is the query for
+ *     resolving penetration (the depth is r - distance for a sphere of radius r at p).
+ *
+ *   vxb_mesh_sphere_cast: a sphere of radius r whose centre moves along c(t) = o_i + t*d_i, t in [t_min, t_max] (a vxb_ray,
+ *     the same validity rules).  With c0_i = o_i + t_min*d_i, rr = r*r and dd_d = (dx*dx + dy*dy) + dz*dz, each triangle's
+ *     contact t is:
+ *       started in contact   the closest point of the triangle to c0 has dd <= rr: t = t_min, and the hit's flags have
+ *                            VXB_SPHERE_STARTED_IN_CONTACT.
+ *       otherwise            the least of these, each +inf when it fails:
+ *         face     e1 = b - a; e2 = c - a; n = e1 x e2; len = sqrt((nx*nx + ny*ny) + nz*nz); side = (c0 - a).n;
+ *                  k = side >= 0 ? r : -r; o'_i = o_i - k*(n_i / len); Moeller-Trumbore of the ray (o', d) exactly as for the
+ *                  ray queries, giving det, u, v, t, accepted iff (side >= 0 ? det > 0 : det < 0) && u >= 0 && u <= 1 &&
+ *                  v >= 0 && u + v <= 1 && t >= t_min && t <= t_max (the plane offset by r toward the side the sphere
+ *                  starts on, approached; a zero-area triangle makes len 0 and fails)
+ *         edges    ab, bc, ca in turn, for the edge q0 -> q1: e = q1 - q0; w = o - q0; ee = e.e; de = d x e; we = w x e;
+ *                  A = de.de; B = de.we; g = d.we; disc = ee * (rr*A - g*g); t = (-B - sqrt(disc)) / A;
+ *                  s = ((wx + t*dx)*ex + (wy + t*dy)*ey) + (wz + t*dz)*ez;
+ *                  accepted iff A > 0 && disc >= 0 && s >= 0 && s <= ee && t >= t_min && t <= t_max
+ *         vertices a, b, c in turn, for the vertex q: w = o - q; B = w.d; x = w x d; disc = rr*dd_d - x.x;
+ *                  t = (-B - sqrt(disc)) / dd_d; accepted iff dd_d > 0 && disc >= 0 && t >= t_min && t <= t_max
+ *                            (both discriminants are the Lagrange-identity forms, which keep their precision for
+ *                            origins far from the triangle).
+ *     A triangle with a finite contact t is a candidate; the hit is the one with the least t, then the lower slot, then the
+ *     lower triangle.  Sweeps that start in contact with several triangles therefore report the lowest slot, not the deepest
+ *     penetration: use vxb_mesh_closest_point for that.  center_i = o_i + t*d_i; point, u and v are the closest point of
+ *     the triangle to center (the contact point; center - point is the contact normal); normal as for the closest point.
+ *     A miss: slot = VXB_RAY_MISS, t = +inf, every other field zero.
+ *
+ * The walk of the sweeps is the ray cast's block walk with the block boxes grown by r + 1/16 voxel instead of 1/16: a
+ * contact puts the centre within r of its triangle's block.  VXB_SPHERE_RADIUS_MAX caps r and max_distance at 15 voxels so
+ * that every block within reach of a point stays within one block of that point's block (27 neighbours, as for the rays).
+ * Refusals: as for the ray queries (VXB_ERR_STATE before the first vxb_mesh_apply; VXB_ERR_ARGUMENT for a NULL pointer with
+ * count > 0; count = 0 does nothing; the same map rebuild), and VXB_ERR_ARGUMENT on both variants for a radius outside
+ * 0 < r <= 15 or a max_distance outside 0 <= m <= 15 (NaN and infinities included).  The HOST variants refuse an invalid
+ * sweep (the ray rules) or a point with a non-finite coordinate, naming its index in vxb_last_error; the DEVICE variants
+ * return a miss for it.  A refused call writes nothing to `hits`. */
+#define VXB_SPHERE_RADIUS_MAX 15.0f          /* sweeps and closest-point queries reach at most this far (voxels) */
+#define VXB_SPHERE_STARTED_IN_CONTACT 1u     /* vxb_sphere_hit.flags */
+typedef struct vxb_sphere_hit
+{
+	float t;                /* centre = origin + t * direction at the first contact */
+	uint32_t slot;          /* as vxb_ray_hit; VXB_RAY_MISS */
+	uint32_t block_id;
+	uint32_t triangle;
+	float center[3];        /* origin + t * direction */
+	float point[3];         /* the contact point: the closest point of the triangle to `center` */
+	float normal[3];        /* the vertex normals blended at (u, v), the ray hit's formula */
+	float u, v;             /* barycentrics of `point` (2nd and 3rd vertex) */
+	uint32_t flags;         /* VXB_SPHERE_STARTED_IN_CONTACT */
+} vxb_sphere_hit;                                                                                            /* 64 bytes */
+typedef struct vxb_closest_hit
+{
+	float distance;         /* |query - point|; +inf on a miss */
+	uint32_t slot;          /* as vxb_ray_hit; VXB_RAY_MISS */
+	uint32_t block_id;
+	uint32_t triangle;
+	float point[3];         /* the closest point of the level-0 surface within max_distance */
+	float normal[3];        /* the vertex normals blended at (u, v), the ray hit's formula */
+	float u, v;             /* barycentrics of `point` (2nd and 3rd vertex) */
+} vxb_closest_hit;                                                                                           /* 48 bytes */
+/* HOST memory; block until the hits are written.  `points` is count x 3 floats. */
+int vxb_mesh_sphere_cast(vxb_mesh* mesh, float radius, const vxb_ray* rays, uint32_t count, vxb_sphere_hit* hits);
+int vxb_mesh_closest_point(vxb_mesh* mesh, float max_distance, const float* points, uint32_t count, vxb_closest_hit* hits);
+/* DEVICE memory; enqueued on vxb_stream(ctx) like vxb_mesh_raycast_device: they see the mesh as of their place in the queue. */
+int vxb_mesh_sphere_cast_device(vxb_mesh* mesh, float radius, const vxb_ray* rays, uint32_t count, vxb_sphere_hit* hits);
+int vxb_mesh_closest_point_device(vxb_mesh* mesh, float max_distance, const float* points, uint32_t count, vxb_closest_hit* hits);
+
 /* GetMaterial(id) == nullptr handling (TransVoxelImpl.cpp:1364-1368: textures stay zero, one LS_Error log per
  * vertex): after vxb_result_download the material ids of those vertices, in the reference's logging order
  * (level, block, regular vertices, then transition faces), can be read here.  Returns the count; copies at

@@ -182,6 +182,16 @@ def make_rays(origins, directions, t_min=0.0, t_max=np.inf):
     return rays
 
 
+# vxb_sphere_hit / vxb_closest_hit (include/vxb200.h "collision queries")
+VXB_SPHERE_RADIUS_MAX = 15.0
+VXB_SPHERE_STARTED_IN_CONTACT = 1
+SPHERE_HIT_DTYPE = np.dtype([("t", "<f4"), ("slot", "<u4"), ("block_id", "<u4"), ("triangle", "<u4"), ("center", "<f4", 3),
+                             ("point", "<f4", 3), ("normal", "<f4", 3), ("u", "<f4"), ("v", "<f4"), ("flags", "<u4")])
+CLOSEST_HIT_DTYPE = np.dtype([("distance", "<f4"), ("slot", "<u4"), ("block_id", "<u4"), ("triangle", "<u4"), ("point", "<f4", 3),
+                              ("normal", "<f4", 3), ("u", "<f4"), ("v", "<f4")])
+assert SPHERE_HIT_DTYPE.itemsize == 64 and CLOSEST_HIT_DTYPE.itemsize == 48
+
+
 class MeshInfo(C.Structure):
     """vxb_mesh_info (include/vxb200.h)."""
     _fields_ = [("levels", C.c_uint32), ("block_count", C.c_uint32), ("level_blocks", C.c_uint32 * 12), ("vertex_span", C.c_uint64),
@@ -295,6 +305,10 @@ def load_library():
         "vxb_mesh_select_lod": (C.c_int, [vp, vp, C.c_float, C.POINTER(DrawLists)]),
         "vxb_mesh_raycast": (C.c_int, [vp, vp, u32, vp]),
         "vxb_mesh_raycast_device": (C.c_int, [vp, vp, u32, vp]),
+        "vxb_mesh_sphere_cast": (C.c_int, [vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_sphere_cast_device": (C.c_int, [vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_closest_point": (C.c_int, [vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_closest_point_device": (C.c_int, [vp, C.c_float, vp, u32, vp]),
         "vxb_host_alloc": (vp, [C.c_size_t]),
         "vxb_host_free": (None, [vp]),
     }
@@ -315,7 +329,8 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_grid_upload_packed_streamed", "vxb_result_download_begin", "vxb_result_download_end",
                     "vxb_grid_fill_program", "vxb_grid_inject_program", "vxb_grid_program_stats",
                     "vxb_mesh_create", "vxb_mesh_destroy", "vxb_mesh_apply", "vxb_mesh_info_get", "vxb_mesh_download",
-                    "vxb_mesh_device_arenas", "vxb_mesh_select_lod", "vxb_mesh_raycast", "vxb_mesh_raycast_device"]
+                    "vxb_mesh_device_arenas", "vxb_mesh_select_lod", "vxb_mesh_raycast", "vxb_mesh_raycast_device",
+                    "vxb_mesh_sphere_cast", "vxb_mesh_sphere_cast_device", "vxb_mesh_closest_point", "vxb_mesh_closest_point_device"]
 
 
 def nccl_unique_id():
@@ -493,6 +508,50 @@ class Mesh:
         data_ptr()); enqueued on the context's stream, returns without waiting."""
         self.ctx._check(self.L.vxb_mesh_raycast_device(self.h, None if rays_ptr is None else C.c_void_p(rays_ptr), count,
                                                        None if hits_ptr is None else C.c_void_p(hits_ptr)), "vxb_mesh_raycast_device")
+
+    def sphere_cast_rc(self, radius, rays, hits=None, count=None):
+        """vxb_mesh_sphere_cast's return code for a RAY_DTYPE array (or None for a NULL pointer); the hits go to `hits` (a
+        SPHERE_HIT_DTYPE array, or None for a NULL pointer); `count` defaults to len(rays)."""
+        rays = np.ascontiguousarray(rays, RAY_DTYPE) if rays is not None else None
+        n = (0 if rays is None else len(rays)) if count is None else count
+        return self.L.vxb_mesh_sphere_cast(self.h, radius, _ptr(rays), n, _ptr(hits))
+
+    def sphere_cast(self, radius, origins, directions=None, t_min=0.0, t_max=np.inf):
+        """Sweeps a sphere of `radius` voxels along each segment against the mesh's level-0 triangles (vxb_mesh_sphere_cast):
+        `origins` / `directions` are [count, 3] in OUTPUT (Y-up) coordinates, or `origins` is a RAY_DTYPE array and
+        `directions` None.  Returns a SPHERE_HIT_DTYPE array."""
+        rays = np.ascontiguousarray(origins if directions is None else make_rays(origins, directions, t_min, t_max), RAY_DTYPE)
+        hits = np.zeros(len(rays), SPHERE_HIT_DTYPE)
+        self.ctx._check(self.L.vxb_mesh_sphere_cast(self.h, radius, _ptr(rays), len(rays), _ptr(hits)), "vxb_mesh_sphere_cast")
+        return hits
+
+    def sphere_cast_device(self, radius, rays_ptr, count, hits_ptr):
+        """vxb_mesh_sphere_cast_device: `count` vxb_ray at the device address `rays_ptr`, hits to `hits_ptr`; enqueued on the
+        context's stream, returns without waiting."""
+        self.ctx._check(self.L.vxb_mesh_sphere_cast_device(self.h, radius, None if rays_ptr is None else C.c_void_p(rays_ptr), count,
+                                                           None if hits_ptr is None else C.c_void_p(hits_ptr)), "vxb_mesh_sphere_cast_device")
+
+    def closest_points_rc(self, max_distance, points, hits=None, count=None):
+        """vxb_mesh_closest_point's return code for [count, 3] float32 points (or None for a NULL pointer); the hits go to
+        `hits` (a CLOSEST_HIT_DTYPE array, or None for a NULL pointer); `count` defaults to len(points)."""
+        pts = np.ascontiguousarray(points, np.float32).reshape(-1, 3) if points is not None else None
+        n = (0 if pts is None else len(pts)) if count is None else count
+        return self.L.vxb_mesh_closest_point(self.h, max_distance, _ptr(pts), n, _ptr(hits))
+
+    def closest_points(self, points, max_distance):
+        """The nearest level-0 surface point within `max_distance` voxels of each of the [count, 3] `points` (OUTPUT, Y-up
+        coordinates), vxb_mesh_closest_point.  Returns a CLOSEST_HIT_DTYPE array."""
+        pts = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
+        hits = np.zeros(len(pts), CLOSEST_HIT_DTYPE)
+        self.ctx._check(self.L.vxb_mesh_closest_point(self.h, max_distance, _ptr(pts), len(pts), _ptr(hits)), "vxb_mesh_closest_point")
+        return hits
+
+    def closest_points_device(self, max_distance, points_ptr, count, hits_ptr):
+        """vxb_mesh_closest_point_device: `count` points (3 floats each) at the device address `points_ptr`, hits to
+        `hits_ptr`; enqueued on the context's stream, returns without waiting."""
+        self.ctx._check(self.L.vxb_mesh_closest_point_device(self.h, max_distance, None if points_ptr is None else C.c_void_p(points_ptr),
+                                                             count, None if hits_ptr is None else C.c_void_p(hits_ptr)),
+                        "vxb_mesh_closest_point_device")
 
 
 class Context:

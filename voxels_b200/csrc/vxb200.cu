@@ -33,10 +33,12 @@
 #include "vxb_draw.cuh"
 #include "vxb_mesh.cuh"
 #include "vxb_ray.cuh"
+#include "vxb_collide.cuh"
 
 static_assert(sizeof(VxbVertex) == 48, "PolygonVertex layout");
 static_assert(sizeof(vxb_block_record) == 128, "record layout");
 static_assert(sizeof(vxb_ray) == 32 && sizeof(vxb_ray_hit) == 48, "ray layouts");
+static_assert(sizeof(vxb_sphere_hit) == 64 && sizeof(vxb_closest_hit) == 48, "collision layouts");
 
 namespace
 {
@@ -2200,8 +2202,11 @@ struct vxb_mesh
 	bool mapBuilt = false;
 	uint64_t mapSerial = 0;
 	uint32_t mapN = 0;
-	DevBuf<vxb_ray> rayIn;                      // vxb_mesh_raycast's device staging, grown as needed
+	DevBuf<vxb_ray> rayIn;                      // the host variants' device staging (rays and sweeps), grown as needed
 	DevBuf<vxb_ray_hit> rayOut;
+	DevBuf<vxb_sphere_hit> sphereOut;
+	DevBuf<float> pointIn;                      // 3 floats per closest-point query
+	DevBuf<vxb_closest_hit> closestOut;
 };
 
 namespace
@@ -2214,8 +2219,9 @@ void deleteMesh(vxb_mesh* m)
 
 uint64_t grownCapacity(uint64_t live) { return (std::max<uint64_t>(live + live / 2, 1024) + 3) & ~(uint64_t)3; }
 
-// The map for the applied run (rebuilt after every apply: each one has a new serial) and the cast, both on ctx->stream.
-int enqueueRaycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits)
+// The level-0 map for the applied run (rebuilt after every apply: each one has a new serial), queued on ctx->stream, and the
+// kernels' view of the mesh.
+int ensureMap(vxb_mesh* m, VxbRayMesh& rm)
 {
 	vxb_context* ctx = m->ctx;
 	cudaStream_t st = ctx->stream;
@@ -2225,7 +2231,7 @@ int enqueueRaycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit
 		const size_t cells = (size_t)nb * nb * nb;
 		if (cells > m->rayMap.count)
 		{
-			VXB_CUDA(ctx, cudaStreamSynchronize(st)); // a cast still queued may read the old map
+			VXB_CUDA(ctx, cudaStreamSynchronize(st)); // a query still queued may read the old map
 			VXB_CUDA(ctx, m->rayMap.ensure(cells));
 		}
 		VXB_CUDA(ctx, cudaMemsetAsync(m->rayMap.p, 0xFF, cells * sizeof(unsigned int), st));
@@ -2234,12 +2240,76 @@ int enqueueRaycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit
 		VXB_CUDA(ctx, cudaGetLastError());
 		m->mapBuilt = true; m->mapSerial = m->serial; m->mapN = m->n;
 	}
-	VxbRayMesh rm;
 	rm.dir = m->dir.p; rm.map = m->rayMap.p; rm.verts = m->set[m->active].v.p; rm.idx = m->set[m->active].i.p; rm.nb = (int)nb;
-	const unsigned warpsPerCta = VXB_RAY_THREADS / 32;
-	const unsigned ctas = std::min<unsigned>((count + warpsPerCta - 1) / warpsPerCta, (unsigned)std::max(ctx->smCount, 1) * 8);
-	vxb_raycast_kernel<<<ctas, VXB_RAY_THREADS, 0, st>>>(rm, rays, count, hits);
-	VXB_CUDA(ctx, cudaGetLastError());
+	return VXB_OK;
+}
+
+// CTAs of a persistent one-warp-per-query launch
+unsigned queryCtas(const vxb_context* ctx, uint32_t count, unsigned threads)
+{
+	const unsigned warpsPerCta = threads / 32;
+	return std::min<unsigned>((count + warpsPerCta - 1) / warpsPerCta, (unsigned)std::max(ctx->smCount, 1) * 8);
+}
+
+int enqueueRaycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits)
+{
+	VxbRayMesh rm;
+	const int e = ensureMap(m, rm);
+	if (e != VXB_OK) return e;
+	vxb_raycast_kernel<<<queryCtas(m->ctx, count, VXB_RAY_THREADS), VXB_RAY_THREADS, 0, m->ctx->stream>>>(rm, rays, count, hits);
+	VXB_CUDA(m->ctx, cudaGetLastError());
+	return VXB_OK;
+}
+
+int enqueueSphereCast(vxb_mesh* m, float radius, const vxb_ray* rays, uint32_t count, vxb_sphere_hit* hits)
+{
+	VxbRayMesh rm;
+	const int e = ensureMap(m, rm);
+	if (e != VXB_OK) return e;
+	vxb_sphere_cast_kernel<<<queryCtas(m->ctx, count, VXB_COLLIDE_THREADS), VXB_COLLIDE_THREADS, 0, m->ctx->stream>>>(rm, radius, rays, count, hits);
+	VXB_CUDA(m->ctx, cudaGetLastError());
+	return VXB_OK;
+}
+
+int enqueueClosestPoint(vxb_mesh* m, float maxDistance, const float* points, uint32_t count, vxb_closest_hit* hits)
+{
+	VxbRayMesh rm;
+	const int e = ensureMap(m, rm);
+	if (e != VXB_OK) return e;
+	vxb_closest_point_kernel<<<queryCtas(m->ctx, count, VXB_COLLIDE_THREADS), VXB_COLLIDE_THREADS, 0, m->ctx->stream>>>(rm, maxDistance, points, count, hits);
+	VXB_CUDA(m->ctx, cudaGetLastError());
+	return VXB_OK;
+}
+
+// the batch arguments of the collision queries (include/vxb200.h): 0 < radius <= 15, 0 <= max_distance <= 15; NaN fails
+bool validRadius(float r) { return r > 0.f && r <= VXB_SPHERE_RADIUS_MAX; }
+bool validMaxDistance(float d) { return d >= 0.f && d <= VXB_SPHERE_RADIUS_MAX; }
+
+// the index of the first query point with a non-finite coordinate, or -1
+long long invalidPoint(const float* points, uint32_t count)
+{
+	for (uint32_t q = 0; q < count; ++q)
+		if (!std::isfinite(points[3 * q]) || !std::isfinite(points[3 * q + 1]) || !std::isfinite(points[3 * q + 2])) return q;
+	return -1;
+}
+
+// A host variant's round trip on ctx->stream: queries to the staging `in`, the enqueued query, hits back; blocks.
+template <class In, class Out, class Enqueue>
+int hostQuery(vxb_mesh* m, DevBuf<In>& in, size_t inPerQuery, DevBuf<Out>& out, const In* queries, uint32_t count, Out* hits, Enqueue&& enqueue)
+{
+	vxb_context* ctx = m->ctx;
+	cudaSetDevice(ctx->device);
+	cudaStream_t st = ctx->stream;
+	if (count * inPerQuery > in.count || count > out.count)
+	{
+		VXB_CUDA(ctx, cudaStreamSynchronize(st)); // nothing queued may still use the staging being replaced
+		VXB_CUDA(ctx, in.ensure(count * inPerQuery)); VXB_CUDA(ctx, out.ensure(count));
+	}
+	VXB_CUDA(ctx, cudaMemcpyAsync(in.p, queries, sizeof(In) * inPerQuery * count, cudaMemcpyHostToDevice, st));
+	const int r = enqueue(in.p, out.p);
+	if (r != VXB_OK) return r;
+	VXB_CUDA(ctx, cudaMemcpyAsync(hits, out.p, sizeof(Out) * count, cudaMemcpyDeviceToHost, st));
+	VXB_CUDA(ctx, cudaStreamSynchronize(st));
 	return VXB_OK;
 }
 
@@ -2522,19 +2592,8 @@ int vxb_mesh_raycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_h
 		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_raycast: ray %lld: %s", bad, why);
 		return fail(ctx, VXB_ERR_ARGUMENT, buf);
 	}
-	cudaSetDevice(ctx->device);
-	cudaStream_t st = ctx->stream;
-	if (count > m->rayIn.count || count > m->rayOut.count)
-	{
-		VXB_CUDA(ctx, cudaStreamSynchronize(st)); // nothing queued may still use the staging being replaced
-		VXB_CUDA(ctx, m->rayIn.ensure(count)); VXB_CUDA(ctx, m->rayOut.ensure(count));
-	}
-	VXB_CUDA(ctx, cudaMemcpyAsync(m->rayIn.p, rays, sizeof(vxb_ray) * count, cudaMemcpyHostToDevice, st));
-	const int r = enqueueRaycast(m, m->rayIn.p, count, m->rayOut.p);
-	if (r != VXB_OK) return r;
-	VXB_CUDA(ctx, cudaMemcpyAsync(hits, m->rayOut.p, sizeof(vxb_ray_hit) * count, cudaMemcpyDeviceToHost, st));
-	VXB_CUDA(ctx, cudaStreamSynchronize(st));
-	return VXB_OK;
+	return hostQuery(m, m->rayIn, 1, m->rayOut, rays, count, hits,
+		[&](const vxb_ray* in, vxb_ray_hit* out) { return enqueueRaycast(m, in, count, out); });
 }
 
 int vxb_mesh_raycast_device(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits)
@@ -2546,6 +2605,67 @@ int vxb_mesh_raycast_device(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vx
 	if (!count) return VXB_OK;
 	cudaSetDevice(ctx->device);
 	return enqueueRaycast(m, rays, count, hits);
+}
+
+int vxb_mesh_sphere_cast(vxb_mesh* m, float radius, const vxb_ray* rays, uint32_t count, vxb_sphere_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!validRadius(radius)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_sphere_cast: radius must be in (0, 15]");
+	if (count && (!rays || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_sphere_cast: NULL rays or hits");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_sphere_cast: nothing applied yet");
+	if (!count) return VXB_OK;
+	const char* why = "";
+	const long long bad = invalidRay(rays, count, &why);
+	if (bad >= 0)
+	{
+		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_sphere_cast: sweep %lld: %s", bad, why);
+		return fail(ctx, VXB_ERR_ARGUMENT, buf);
+	}
+	return hostQuery(m, m->rayIn, 1, m->sphereOut, rays, count, hits,
+		[&](const vxb_ray* in, vxb_sphere_hit* out) { return enqueueSphereCast(m, radius, in, count, out); });
+}
+
+int vxb_mesh_sphere_cast_device(vxb_mesh* m, float radius, const vxb_ray* rays, uint32_t count, vxb_sphere_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!validRadius(radius)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_sphere_cast_device: radius must be in (0, 15]");
+	if (count && (!rays || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_sphere_cast_device: NULL rays or hits");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_sphere_cast_device: nothing applied yet");
+	if (!count) return VXB_OK;
+	cudaSetDevice(ctx->device);
+	return enqueueSphereCast(m, radius, rays, count, hits);
+}
+
+int vxb_mesh_closest_point(vxb_mesh* m, float maxDistance, const float* points, uint32_t count, vxb_closest_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!validMaxDistance(maxDistance)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_point: max_distance must be in [0, 15]");
+	if (count && (!points || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_point: NULL points or hits");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_closest_point: nothing applied yet");
+	if (!count) return VXB_OK;
+	const long long bad = invalidPoint(points, count);
+	if (bad >= 0)
+	{
+		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_closest_point: point %lld: non-finite coordinate", bad);
+		return fail(ctx, VXB_ERR_ARGUMENT, buf);
+	}
+	return hostQuery(m, m->pointIn, 3, m->closestOut, points, count, hits,
+		[&](const float* in, vxb_closest_hit* out) { return enqueueClosestPoint(m, maxDistance, in, count, out); });
+}
+
+int vxb_mesh_closest_point_device(vxb_mesh* m, float maxDistance, const float* points, uint32_t count, vxb_closest_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!validMaxDistance(maxDistance)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_point_device: max_distance must be in [0, 15]");
+	if (count && (!points || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_point_device: NULL points or hits");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_closest_point_device: nothing applied yet");
+	if (!count) return VXB_OK;
+	cudaSetDevice(ctx->device);
+	return enqueueClosestPoint(m, maxDistance, points, count, hits);
 }
 
 } // extern "C"

@@ -17,6 +17,20 @@
 //                operations, so the true entry is at least t1 - 2^-22 |t1|, and a hit in that block (inside its grown box) has
 //                t >= that.  With the margin 2^-20 |t1|, t1 > best + margin proves t > best for every remaining hit: no hit
 //                can tie or beat the best one, and the walk ends.
+//
+// Sphere sweeps (vxb_collide.cuh) run the same walk with the boxes grown by g = r + VXB_RAY_EPS instead of VXB_RAY_EPS:
+//   tested set   a contact the sweep's tests accept puts the centre within r (+ rounding) of its triangle, hence of the
+//                triangle's block, hence inside that block's box grown by r + eps.  A sweep that starts in contact has
+//                c(t_min) there too, so the block's te is the clipped start.  The planes 16 b -+ g are now rounded (g is any
+//                float), but a rounded plane moves by 2^-24 |16 b| at most, far inside the eps slack, so the box the walk uses
+//                still holds every such centre; the proof above needs nothing else of the planes.
+//   anchoring    the centre at te is within g (+ rounding) of the block and inside the anchor cell (up to rounding) along
+//                every axis where it lies inside the grid.  Where it lies outside the grid (the clip box is grown by g too),
+//                the cell index is clamped to 0 or nb - 1, and only that block is within g of the centre along that axis.
+//                With r <= VXB_SPHERE_RADIUS_MAX = 15, g + rounding < 16 = one block: the block is still one of the anchor
+//                cell's 27 neighbours.  A larger radius would need a wider neighbourhood, which is why the radius is capped.
+//   stop         unchanged: te is still two correctly rounded operations from the (rounded) plane, and a contact inside the
+//                grown box has t >= the true te.
 #pragma once
 
 #include <math_constants.h>
@@ -54,9 +68,9 @@ VXB_FN void vxb_ray_slab(float o, float d, float lo, float hi, float& tin, float
 	tin = fmaxf(tin, a); tout = fminf(tout, b);
 }
 
-// the grown box of block index b along one axis
-VXB_FN float vxb_ray_lo(int b) { return (float)(16 * b) - VXB_RAY_EPS; }
-VXB_FN float vxb_ray_hi(int b) { return (float)(16 * b + 16) + VXB_RAY_EPS; }
+// the box of block index b along one axis, grown by g
+VXB_FN float vxb_ray_lo(int b, float g) { return (float)(16 * b) - g; }
+VXB_FN float vxb_ray_hi(int b, float g) { return (float)(16 * b + 16) + g; }
 
 // the next cell boundary crossed along one axis (ungrown planes); +inf when the step would leave the grid
 VXB_FN float vxb_ray_next(int c, float o, float d, int nb)
@@ -80,17 +94,130 @@ VXB_FN bool vxb_ray_before(float t, unsigned s, unsigned k, float t2, unsigned s
 	return t < t2 || (t == t2 && (s < s2 || (s == s2 && k < k2)));
 }
 
-// One warp per ray, persistent over the batch.  Rays and hits in OUTPUT (Y-up) coordinates; block coordinates of the map
-// are grid (Z-up): output (x, y, z) = grid (x, z, y).
+
+// the positions of triangle k of the block at (vertex offset vo, index offset io)
+VXB_FN void vxb_ray_triangle(const VxbRayMesh& m, unsigned vo, unsigned io, unsigned k, float3& a, float3& b, float3& c)
+{
+	const unsigned* ip = m.idx + io + 3 * k;
+	const float* pa = m.verts[vo + __ldg(ip)].pos;
+	const float* pb = m.verts[vo + __ldg(ip + 1)].pos;
+	const float* pc = m.verts[vo + __ldg(ip + 2)].pos;
+	a = make_float3(__ldg(pa), __ldg(pa + 1), __ldg(pa + 2));
+	b = make_float3(__ldg(pb), __ldg(pb + 1), __ldg(pb + 2));
+	c = make_float3(__ldg(pc), __ldg(pc + 1), __ldg(pc + 2));
+}
+
+// The vertex normals of triangle k of slot s blended at (u, v) and normalised, the hit normal of include/vxb200.h:
+// w = (1 - u) - v; n_i = (w*n0_i + u*n1_i) + v*n2_i; n_i / sqrt((nx*nx + ny*ny) + nz*nz), or (0, 0, 0) when that is 0.
+VXB_FN void vxb_ray_blend_normal(const VxbRayMesh& m, unsigned s, unsigned k, float u, float v, float* out)
+{
+	const vxb_block_record* rec = m.dir + s;
+	const unsigned vo = __ldg(&rec->vertex_offset);
+	const unsigned* ip = m.idx + __ldg(&rec->index_offset) + 3 * k;
+	const float* n0 = m.verts[vo + __ldg(ip)].nrm;
+	const float* n1 = m.verts[vo + __ldg(ip + 1)].nrm;
+	const float* n2 = m.verts[vo + __ldg(ip + 2)].nrm;
+	const float w = (1.f - u) - v;
+	const float nxv = (w * __ldg(n0) + u * __ldg(n1)) + v * __ldg(n2);
+	const float nyv = (w * __ldg(n0 + 1) + u * __ldg(n1 + 1)) + v * __ldg(n2 + 1);
+	const float nzv = (w * __ldg(n0 + 2) + u * __ldg(n1 + 2)) + v * __ldg(n2 + 2);
+	const float len = VXB_SQRT((nxv * nxv + nyv * nyv) + nzv * nzv);
+	out[0] = out[1] = out[2] = 0.f;
+	if (len > 0.f) { out[0] = VXB_DIV(nxv, len); out[1] = VXB_DIV(nyv, len); out[2] = VXB_DIV(nzv, len); }
+}
+
+// The lane holding the warp's least (t, slot, triangle) by the tie rule (every lane takes part; each candidate is held by
+// one lane, and a warp of misses - slot = triangle = VXB_RAY_MISS everywhere - yields lane 0).
+VXB_FN unsigned vxb_ray_winner(float t, unsigned s, unsigned k)
+{
+	float wt = t; unsigned ws = s, wk = k;
+	for (int o = 16; o > 0; o >>= 1)
+	{
+		const float t2 = __shfl_xor_sync(0xFFFFFFFFu, wt, o);
+		const unsigned s2 = __shfl_xor_sync(0xFFFFFFFFu, ws, o), k2 = __shfl_xor_sync(0xFFFFFFFFu, wk, o);
+		if (vxb_ray_before(t2, s2, k2, wt, ws, wk)) { wt = t2; ws = s2; wk = k2; }
+	}
+	return __ffs(__ballot_sync(0xFFFFFFFFu, s == ws && k == wk)) - 1;
+}
+
+// The conservative block walk of the proof at the top, for one segment per warp (every lane calls it with the same ray):
+// the boxes are grown by `grow` (VXB_RAY_EPS for rays, r + VXB_RAY_EPS for sweeps).  `block(s)` is called by the whole warp
+// once for every block of the tested set that has a map entry, in walk order; it tests the block's triangles (strided over
+// the lanes) and lowers this lane's best parameter `best`, which the stop rule reads.  Rays and blocks in OUTPUT (Y-up)
+// coordinates; block coordinates of the map are grid (Z-up): output (x, y, z) = grid (x, z, y).
+template <class Block>
+VXB_FN void vxb_ray_walk(const VxbRayMesh& m, const vxb_ray& ray, const float grow, const float& best, Block&& block)
+{
+	const unsigned lane = threadIdx.x & 31;
+	const int nb = m.nb;
+	const float n = (float)(16 * nb);
+	// this lane's neighbour offset (lanes 27..31 have none)
+	const int ox = (int)(lane % 3) - 1, oy = (int)((lane / 3) % 3) - 1, oz = (int)(lane / 9) - 1;
+	const float px = ray.origin[0], py = ray.origin[1], pz = ray.origin[2];
+	const float dx = ray.direction[0], dy = ray.direction[1], dz = ray.direction[2];
+	// ---- clip to the grown grid box [-g, n + g]^3 (the union of the grown block boxes, computed with the same planes) ----
+	float T0 = ray.t_min, T1 = ray.t_max;
+	if (!vxb_ray_valid(ray)) return;
+	vxb_ray_slab(px, dx, -grow, n + grow, T0, T1);
+	vxb_ray_slab(py, dy, -grow, n + grow, T0, T1);
+	vxb_ray_slab(pz, dz, -grow, n + grow, T0, T1);
+	if (!(T0 <= T1)) return;
+	// the first cell: the block of the clipped entry point, clamped into the grid
+	int cx = min(max((int)floorf((px + T0 * dx) * 0.0625f), 0), nb - 1);
+	int cy = min(max((int)floorf((py + T0 * dy) * 0.0625f), 0), nb - 1);
+	int cz = min(max((int)floorf((pz + T0 * dz) * 0.0625f), 0), nb - 1);
+	float nx = vxb_ray_next(cx, px, dx, nb), ny = vxb_ray_next(cy, py, dy, nb), nz = vxb_ray_next(cz, pz, dz, nb);
+	float t0 = T0;
+	for (;;)
+	{
+		const float tn = fminf(nx, fminf(ny, nz));
+		const bool last = !(tn < T1);
+		const float t1 = last ? T1 : fmaxf(tn, t0);
+		// ---- the neighbours anchored in [t0, t1) ----
+		const int bx = cx + ox, by = cy + oy, bz = cz + oz;
+		bool cand = false;
+		unsigned slot = VXB_RAY_MISS;
+		if (lane < 27 && bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb)
+		{
+			float te = T0, tx = T1;
+			vxb_ray_slab(px, dx, vxb_ray_lo(bx, grow), vxb_ray_hi(bx, grow), te, tx);
+			vxb_ray_slab(py, dy, vxb_ray_lo(by, grow), vxb_ray_hi(by, grow), te, tx);
+			vxb_ray_slab(pz, dz, vxb_ray_lo(bz, grow), vxb_ray_hi(bz, grow), te, tx);
+			if (te <= tx && te >= t0 && (te < t1 || last))
+			{
+				slot = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
+				cand = slot != VXB_RAY_MISS;
+			}
+		}
+		unsigned todo = __ballot_sync(0xFFFFFFFFu, cand);
+		const bool tested = todo != 0;
+		while (todo)
+		{
+			const unsigned src = __ffs(todo) - 1;
+			todo &= todo - 1;
+			block(__shfl_sync(0xFFFFFFFFu, slot, src));
+		}
+		if (last) break;
+		if (tested)
+		{
+			float w = best;
+			for (int o = 16; o > 0; o >>= 1) w = fminf(w, __shfl_xor_sync(0xFFFFFFFFu, w, o));
+			if (t1 > w + ldexpf(fabsf(t1), VXB_RAY_MARGIN_EXP)) break;
+		}
+		// ---- step across the nearest boundary (ties: x, then y, then z; the others follow with empty intervals) ----
+		if (nx == tn) { cx += dx > 0.f ? 1 : -1; nx = vxb_ray_next(cx, px, dx, nb); }
+		else if (ny == tn) { cy += dy > 0.f ? 1 : -1; ny = vxb_ray_next(cy, py, dy, nb); }
+		else { cz += dz > 0.f ? 1 : -1; nz = vxb_ray_next(cz, pz, dz, nb); }
+		t0 = t1;
+	}
+}
+
+// One warp per ray, persistent over the batch.  Rays and hits in OUTPUT (Y-up) coordinates.
 __global__ void __launch_bounds__(VXB_RAY_THREADS) vxb_raycast_kernel(const VxbRayMesh m, const vxb_ray* __restrict__ rays, unsigned count,
 	vxb_ray_hit* __restrict__ hits)
 {
 	const unsigned lane = threadIdx.x & 31;
 	const unsigned warps = gridDim.x * (VXB_RAY_THREADS / 32);
-	const int nb = m.nb;
-	const float n = (float)(16 * nb);
-	// this lane's neighbour offset (lanes 27..31 have none)
-	const int ox = (int)(lane % 3) - 1, oy = (int)((lane / 3) % 3) - 1, oz = (int)(lane / 9) - 1;
 	for (unsigned r = blockIdx.x * (VXB_RAY_THREADS / 32) + (threadIdx.x >> 5); r < count; r += warps)
 	{
 		const vxb_ray ray = rays[r];
@@ -99,104 +226,34 @@ __global__ void __launch_bounds__(VXB_RAY_THREADS) vxb_raycast_kernel(const VxbR
 		const float tMin = ray.t_min, tMax = ray.t_max;
 		float bt = CUDART_INF_F, bu = 0.f, bv = 0.f;   // this lane's best hit
 		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		// ---- clip to the grown grid box [-eps, n + eps]^3 (the union of the grown block boxes, computed with the same planes) ----
-		float T0 = tMin, T1 = tMax;
-		bool live = vxb_ray_valid(ray);
-		if (live)
-		{
-			vxb_ray_slab(px, dx, -VXB_RAY_EPS, n + VXB_RAY_EPS, T0, T1);
-			vxb_ray_slab(py, dy, -VXB_RAY_EPS, n + VXB_RAY_EPS, T0, T1);
-			vxb_ray_slab(pz, dz, -VXB_RAY_EPS, n + VXB_RAY_EPS, T0, T1);
-			live = T0 <= T1;
-		}
-		if (live)
-		{
-			// the first cell: the block of the clipped entry point, clamped into the grid
-			int cx = min(max((int)floorf((px + T0 * dx) * 0.0625f), 0), nb - 1);
-			int cy = min(max((int)floorf((py + T0 * dy) * 0.0625f), 0), nb - 1);
-			int cz = min(max((int)floorf((pz + T0 * dz) * 0.0625f), 0), nb - 1);
-			float nx = vxb_ray_next(cx, px, dx, nb), ny = vxb_ray_next(cy, py, dy, nb), nz = vxb_ray_next(cz, pz, dz, nb);
-			float t0 = T0;
-			for (;;)
+		vxb_ray_walk(m, ray, VXB_RAY_EPS, bt, [&](const unsigned s) {
+			const vxb_block_record* rec = m.dir + s;
+			const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
+			for (unsigned k = lane; k < tris; k += 32)
 			{
-				const float tn = fminf(nx, fminf(ny, nz));
-				const bool last = !(tn < T1);
-				const float t1 = last ? T1 : fmaxf(tn, t0);
-				// ---- the neighbours anchored in [t0, t1) ----
-				const int bx = cx + ox, by = cy + oy, bz = cz + oz;
-				bool cand = false;
-				unsigned slot = VXB_RAY_MISS;
-				if (lane < 27 && bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb)
+				float3 p0, p1, p2;
+				vxb_ray_triangle(m, vo, io, k, p0, p1, p2);
+				const float e1x = p1.x - p0.x, e1y = p1.y - p0.y, e1z = p1.z - p0.z;
+				const float e2x = p2.x - p0.x, e2y = p2.y - p0.y, e2z = p2.z - p0.z;
+				const float sx = px - p0.x, sy = py - p0.y, sz = pz - p0.z;
+				// Moeller-Trumbore exactly as include/vxb200.h states it (-fmad=false: no contraction)
+				const float pvx = dy * e2z - dz * e2y, pvy = dz * e2x - dx * e2z, pvz = dx * e2y - dy * e2x;
+				const float det = (e1x * pvx + e1y * pvy) + e1z * pvz;
+				const float inv = VXB_DIV(1.f, det);
+				const float u = ((sx * pvx + sy * pvy) + sz * pvz) * inv;
+				const float qvx = sy * e1z - sz * e1y, qvy = sz * e1x - sx * e1z, qvz = sx * e1y - sy * e1x;
+				const float v = ((dx * qvx + dy * qvy) + dz * qvz) * inv;
+				const float t = ((e2x * qvx + e2y * qvy) + e2z * qvz) * inv;
+				// positive comparisons only: a NaN fails
+				if (det != 0.f && u >= 0.f && u <= 1.f && v >= 0.f && u + v <= 1.f && t >= tMin && t <= tMax &&
+					vxb_ray_before(t, s, k, bt, bs, bk))
 				{
-					float te = T0, tx = T1;
-					vxb_ray_slab(px, dx, vxb_ray_lo(bx), vxb_ray_hi(bx), te, tx);
-					vxb_ray_slab(py, dy, vxb_ray_lo(by), vxb_ray_hi(by), te, tx);
-					vxb_ray_slab(pz, dz, vxb_ray_lo(bz), vxb_ray_hi(bz), te, tx);
-					if (te <= tx && te >= t0 && (te < t1 || last))
-					{
-						slot = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
-						cand = slot != VXB_RAY_MISS;
-					}
+					bt = t; bs = s; bk = k; bu = u; bv = v;
 				}
-				unsigned todo = __ballot_sync(0xFFFFFFFFu, cand);
-				const bool tested = todo != 0;
-				while (todo)
-				{
-					const unsigned src = __ffs(todo) - 1;
-					todo &= todo - 1;
-					const unsigned s = __shfl_sync(0xFFFFFFFFu, slot, src);
-					const vxb_block_record* rec = m.dir + s;
-					const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
-					for (unsigned k = lane; k < tris; k += 32)
-					{
-						const unsigned* ip = m.idx + io + 3 * k;
-						const float* a = m.verts[vo + __ldg(ip)].pos;
-						const float* b = m.verts[vo + __ldg(ip + 1)].pos;
-						const float* c = m.verts[vo + __ldg(ip + 2)].pos;
-						const float p0x = __ldg(a), p0y = __ldg(a + 1), p0z = __ldg(a + 2);
-						const float e1x = __ldg(b) - p0x, e1y = __ldg(b + 1) - p0y, e1z = __ldg(b + 2) - p0z;
-						const float e2x = __ldg(c) - p0x, e2y = __ldg(c + 1) - p0y, e2z = __ldg(c + 2) - p0z;
-						const float sx = px - p0x, sy = py - p0y, sz = pz - p0z;
-						// Moeller-Trumbore exactly as include/vxb200.h states it (-fmad=false: no contraction)
-						const float pvx = dy * e2z - dz * e2y, pvy = dz * e2x - dx * e2z, pvz = dx * e2y - dy * e2x;
-						const float det = (e1x * pvx + e1y * pvy) + e1z * pvz;
-						const float inv = VXB_DIV(1.f, det);
-						const float u = ((sx * pvx + sy * pvy) + sz * pvz) * inv;
-						const float qvx = sy * e1z - sz * e1y, qvy = sz * e1x - sx * e1z, qvz = sx * e1y - sy * e1x;
-						const float v = ((dx * qvx + dy * qvy) + dz * qvz) * inv;
-						const float t = ((e2x * qvx + e2y * qvy) + e2z * qvz) * inv;
-						// positive comparisons only: a NaN fails
-						if (det != 0.f && u >= 0.f && u <= 1.f && v >= 0.f && u + v <= 1.f && t >= tMin && t <= tMax &&
-							vxb_ray_before(t, s, k, bt, bs, bk))
-						{
-							bt = t; bs = s; bk = k; bu = u; bv = v;
-						}
-					}
-				}
-				if (last) break;
-				if (tested)
-				{
-					float w = bt;
-					for (int o = 16; o > 0; o >>= 1) w = fminf(w, __shfl_xor_sync(0xFFFFFFFFu, w, o));
-					if (t1 > w + ldexpf(fabsf(t1), VXB_RAY_MARGIN_EXP)) break;
-				}
-				// ---- step across the nearest boundary (ties: x, then y, then z; the others follow with empty intervals) ----
-				if (nx == tn) { cx += dx > 0.f ? 1 : -1; nx = vxb_ray_next(cx, px, dx, nb); }
-				else if (ny == tn) { cy += dy > 0.f ? 1 : -1; ny = vxb_ray_next(cy, py, dy, nb); }
-				else { cz += dz > 0.f ? 1 : -1; nz = vxb_ray_next(cz, pz, dz, nb); }
-				t0 = t1;
 			}
-		}
+		});
 		// ---- the winner by the tie rule; its lane writes the hit ----
-		float wt = bt; unsigned ws = bs, wk = bk;
-		for (int o = 16; o > 0; o >>= 1)
-		{
-			const float t2 = __shfl_xor_sync(0xFFFFFFFFu, wt, o);
-			const unsigned s2 = __shfl_xor_sync(0xFFFFFFFFu, ws, o), k2 = __shfl_xor_sync(0xFFFFFFFFu, wk, o);
-			if (vxb_ray_before(t2, s2, k2, wt, ws, wk)) { wt = t2; ws = s2; wk = k2; }
-		}
-		const unsigned winner = __ffs(__ballot_sync(0xFFFFFFFFu, bs == ws && bk == wk)) - 1;
-		if (lane == winner)
+		if (lane == vxb_ray_winner(bt, bs, bk))
 		{
 			vxb_ray_hit h;
 			h.u = 0.f; h.v = 0.f; h.slot = VXB_RAY_MISS; h.block_id = 0; h.triangle = 0;
@@ -205,20 +262,9 @@ __global__ void __launch_bounds__(VXB_RAY_THREADS) vxb_raycast_kernel(const VxbR
 			h.normal[0] = h.normal[1] = h.normal[2] = 0.f;
 			if (bs != VXB_RAY_MISS)
 			{
-				const vxb_block_record* rec = m.dir + bs;
-				const unsigned vo = __ldg(&rec->vertex_offset);
-				const unsigned* ip = m.idx + __ldg(&rec->index_offset) + 3 * bk;
-				const float* n0 = m.verts[vo + __ldg(ip)].nrm;
-				const float* n1 = m.verts[vo + __ldg(ip + 1)].nrm;
-				const float* n2 = m.verts[vo + __ldg(ip + 2)].nrm;
-				h.t = bt; h.u = bu; h.v = bv; h.slot = bs; h.block_id = __ldg(&rec->id); h.triangle = bk;
+				h.t = bt; h.u = bu; h.v = bv; h.slot = bs; h.block_id = __ldg(&m.dir[bs].id); h.triangle = bk;
 				h.position[0] = px + bt * dx; h.position[1] = py + bt * dy; h.position[2] = pz + bt * dz;
-				const float w = (1.f - bu) - bv;
-				const float nxv = (w * __ldg(n0) + bu * __ldg(n1)) + bv * __ldg(n2);
-				const float nyv = (w * __ldg(n0 + 1) + bu * __ldg(n1 + 1)) + bv * __ldg(n2 + 1);
-				const float nzv = (w * __ldg(n0 + 2) + bu * __ldg(n1 + 2)) + bv * __ldg(n2 + 2);
-				const float len = VXB_SQRT((nxv * nxv + nyv * nyv) + nzv * nzv);
-				if (len > 0.f) { h.normal[0] = VXB_DIV(nxv, len); h.normal[1] = VXB_DIV(nyv, len); h.normal[2] = VXB_DIV(nzv, len); }
+				vxb_ray_blend_normal(m, bs, bk, bu, bv, h.normal);
 			}
 			hits[r] = h;
 		}
