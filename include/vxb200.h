@@ -414,6 +414,54 @@ int vxb_mesh_device_arenas(vxb_mesh* mesh, const vxb_block_record** records, con
 /* vxb_result_select_lod over the mesh's blocks; the lists are the mesh's own (the context's stay as they are) */
 int vxb_mesh_select_lod(vxb_mesh* mesh, const float camera[3], float base_distance, vxb_draw_lists* out);
 
+/* ---- bounds and the culled select: the cut drawn only where a view sees it ---------------------------------------------
+ * bounds        For every block the mesh keeps one axis-aligned box in OUTPUT (Y-up) coordinates: the component-wise min and
+ *               max of pos[0..2] and sec[0..2] (the primary and the secondary position; sec[3] is the flag word) over the
+ *               block's regular vertices and the transition vertices of all six faces.  It covers both positions because
+ *               the vertex shader may pick either (Rendering.md:44-52), and the transition vertices so that one box serves
+ *               the block's regular draw and its transition draws.  It is measured from the vertices, not taken from the
+ *               block lattice: it is usually much smaller than the block (a surface fills a part of it), and it does not
+ *               rest on the vertices staying inside the block at levels >= 1, where t is recomputed after the LOD descent
+ *               (TransVoxelImpl.cpp:1671-1699).  Min and max are exact: the box is a pure function of the block's vertices
+ *               (compare values: -0 and +0 are equal).
+ *               vxb_mesh_apply computes the boxes of the blocks it takes in; a surviving block keeps its box across edits,
+ *               compactions and growth; an erased block's box becomes min = +inf, max = -inf.  A renderer may read the boxes
+ *               for its own passes (occlusion tests, cascade fitting): vxb_mesh_bounds_get; the pointer stays valid until an
+ *               apply changes the grid size.  VXB_ERR_STATE before the first apply.
+ * culled select vxb_mesh_select_lod_views builds, in one pass over the directory, one pair of draw lists per view.  The CUT is
+ *               vxb_mesh_select_lod's for (lod_camera, base_distance) in every view - which blocks are drawn, block_adj,
+ *               which transition meshes - so that a shadow cascade and the colour pass draw the same geometry; only the
+ *               frustum differs.  A block of the cut is in view v's lists iff its box passes every plane k of the view, in
+ *               float32 without fused multiply-add, in exactly this order:
+ *                   c_i = n_i >= 0 ? max_i : min_i         (i = x, y, z; -0 >= 0)
+ *                   s   = ((nx*cx + ny*cy) + nz*cz) + d     pass iff s >= 0
+ *               Its transition draws follow it (same box).  block_adj is the cut's and does not depend on visibility: a
+ *               culled neighbour is still "drawn finer".  Per view the lists are a pure function of (mesh, lod_camera,
+ *               base_distance, view) as a set of (command, info) pairs; their order is unspecified; first_instance is the
+ *               draw's index into its own view's info array.  The lists are the mesh's own (vxb_mesh_select_lod's and the
+ *               context's stay as they are) and stay valid until the next vxb_mesh_select_lod_views or until an apply
+ *               changes `generation`.  The call blocks, like vxb_mesh_select_lod.
+ * Refusals (previous lists and `out` untouched): VXB_ERR_STATE before the first apply; VXB_ERR_ARGUMENT for a NULL pointer,
+ * for view_count = 0 or > VXB_VIEWS_MAX, and for a non-finite plane component (vxb_last_error names the view and the plane).
+ * There is no matrix input: the planes of a view-projection matrix are ten lines on the client and depend on its clip
+ * conventions. */
+typedef struct vxb_mesh_bounds
+{
+	const float* boxes;        /* DEVICE: 8 floats per (level, coord) slot: min xyz, 0, max xyz, 0; min > max for absent blocks */
+	uint32_t level_base[12];   /* slot of a block = level_base[level] + coord_id */
+	uint32_t slots;
+	uint32_t pad;
+} vxb_mesh_bounds;
+int vxb_mesh_bounds_get(vxb_mesh* mesh, vxb_mesh_bounds* out);
+/* tests / debugging: HOST, block_count x 6 floats {min xyz, max xyz} in directory order */
+int vxb_mesh_download_bounds(vxb_mesh* mesh, float* bounds);
+#define VXB_VIEWS_MAX 8
+/* Six planes, each {nx, ny, nz, d} in OUTPUT coordinates, pointing INTO the view volume: a point p is inside plane k
+ * iff ((nx*px + ny*py) + nz*pz) + d >= 0.  A plane {0,0,0,d>=0} passes everything (a view with fewer than six planes). */
+typedef struct vxb_view { float planes[6][4]; } vxb_view;
+int vxb_mesh_select_lod_views(vxb_mesh* mesh, const float lod_camera[3], float base_distance,
+                              const vxb_view* views, uint32_t view_count, vxb_draw_lists* out /* view_count entries */);
+
 /* ---- ray queries against the mesh: picking, line of sight, projectile hits, without leaving HBM ------------------------
  * Rays are cast against the LEVEL-0 regular triangles of the mesh (the full-detail surface, the one edits change); levels >= 1
  * and transition meshes are not part of the query.

@@ -202,6 +202,27 @@ class MeshInfo(C.Structure):
                 ("apply_ms", C.c_float), ("pad", C.c_uint32)]
 
 
+VXB_VIEWS_MAX = 8
+
+
+class View(C.Structure):
+    """vxb_view (include/vxb200.h "culled select"): six planes {nx, ny, nz, d} in OUTPUT coordinates, pointing into the view."""
+    _fields_ = [("planes", (C.c_float * 4) * 6)]
+
+
+class MeshBounds(C.Structure):
+    """vxb_mesh_bounds (include/vxb200.h "bounds")."""
+    _fields_ = [("boxes", C.c_void_p), ("level_base", C.c_uint32 * 12), ("slots", C.c_uint32), ("pad", C.c_uint32)]
+
+
+def make_views(planes):
+    """A View array from [views, 6, 4] plane coefficients."""
+    p = np.ascontiguousarray(planes, np.float32).reshape(-1, 6, 4)
+    views = (View * len(p))()
+    C.memmove(views, p.ctypes.data, p.nbytes)
+    return views
+
+
 class NcclId(C.Structure):
     _fields_ = [("internal", C.c_char * 128)]
 
@@ -303,6 +324,9 @@ def load_library():
         "vxb_mesh_download": (C.c_int, [vp, vp, vp, vp, vp, vp]),
         "vxb_mesh_device_arenas": (C.c_int, [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
         "vxb_mesh_select_lod": (C.c_int, [vp, vp, C.c_float, C.POINTER(DrawLists)]),
+        "vxb_mesh_bounds_get": (C.c_int, [vp, C.POINTER(MeshBounds)]),
+        "vxb_mesh_download_bounds": (C.c_int, [vp, vp]),
+        "vxb_mesh_select_lod_views": (C.c_int, [vp, vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_raycast": (C.c_int, [vp, vp, u32, vp]),
         "vxb_mesh_raycast_device": (C.c_int, [vp, vp, u32, vp]),
         "vxb_mesh_sphere_cast": (C.c_int, [vp, C.c_float, vp, u32, vp]),
@@ -329,7 +353,8 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_grid_upload_packed_streamed", "vxb_result_download_begin", "vxb_result_download_end",
                     "vxb_grid_fill_program", "vxb_grid_inject_program", "vxb_grid_program_stats",
                     "vxb_mesh_create", "vxb_mesh_destroy", "vxb_mesh_apply", "vxb_mesh_info_get", "vxb_mesh_download",
-                    "vxb_mesh_device_arenas", "vxb_mesh_select_lod", "vxb_mesh_raycast", "vxb_mesh_raycast_device",
+                    "vxb_mesh_device_arenas", "vxb_mesh_select_lod", "vxb_mesh_bounds_get", "vxb_mesh_download_bounds",
+                    "vxb_mesh_select_lod_views", "vxb_mesh_raycast", "vxb_mesh_raycast_device",
                     "vxb_mesh_sphere_cast", "vxb_mesh_sphere_cast_device", "vxb_mesh_closest_point", "vxb_mesh_closest_point_device"]
 
 
@@ -488,6 +513,31 @@ class Mesh:
                 _device_to_numpy(lists.regular_info, lists.regular_count, DRAW_INFO_DTYPE),
                 _device_to_numpy(lists.transition, lists.transition_count, DRAW_COMMAND_DTYPE),
                 _device_to_numpy(lists.transition_info, lists.transition_count, DRAW_INFO_DTYPE))
+
+    def bounds(self):
+        """The blocks' boxes as a (block_count, 6) float32 array {min xyz, max xyz} in directory order (vxb_mesh_download_bounds)."""
+        out = np.zeros((self.info().block_count, 6), np.float32)
+        self.ctx._check(self.L.vxb_mesh_download_bounds(self.h, _ptr(out)), "vxb_mesh_download_bounds")
+        return out
+
+    def bounds_device(self):
+        """vxb_mesh_bounds_get: a MeshBounds (device address of the boxes, the slot of every level, the slot count)."""
+        b = MeshBounds()
+        self.ctx._check(self.L.vxb_mesh_bounds_get(self.h, C.byref(b)), "vxb_mesh_bounds_get")
+        return b
+
+    def select_lod_views(self, lod_camera, base_distance, views, lists_out=None):
+        """vxb_mesh_select_lod_views: the cut of (lod_camera, base_distance) culled against each of `views` ([views, 6, 4]
+        plane coefficients or a View array).  Returns, per view, the four arrays select_lod returns; the device-resident
+        vxb_draw_lists go to `lists_out` (a DrawLists array of len(views)) when given."""
+        cam = np.ascontiguousarray(lod_camera, np.float32)
+        views = views if isinstance(views, C.Array) else make_views(views)
+        lists = (DrawLists * len(views))() if lists_out is None else lists_out
+        self.ctx._check(self.L.vxb_mesh_select_lod_views(self.h, _ptr(cam), base_distance, views, len(views), lists), "vxb_mesh_select_lod_views")
+        return [(_device_to_numpy(l.regular, l.regular_count, DRAW_COMMAND_DTYPE),
+                 _device_to_numpy(l.regular_info, l.regular_count, DRAW_INFO_DTYPE),
+                 _device_to_numpy(l.transition, l.transition_count, DRAW_COMMAND_DTYPE),
+                 _device_to_numpy(l.transition_info, l.transition_count, DRAW_INFO_DTYPE)) for l in lists]
 
     def raycast_rc(self, rays, hits=None):
         """vxb_mesh_raycast's return code for a RAY_DTYPE array; the hits go to `hits` (a RAY_HIT_DTYPE array, or None for a

@@ -39,6 +39,7 @@ static_assert(sizeof(VxbVertex) == 48, "PolygonVertex layout");
 static_assert(sizeof(vxb_block_record) == 128, "record layout");
 static_assert(sizeof(vxb_ray) == 32 && sizeof(vxb_ray_hit) == 48, "ray layouts");
 static_assert(sizeof(vxb_sphere_hit) == 64 && sizeof(vxb_closest_hit) == 48, "collision layouts");
+static_assert(sizeof(vxb_view) == 96 && sizeof(vxb_mesh_bounds) == 64 && VXB_MAX_LEVELS == 12, "view and bounds layouts");
 
 namespace
 {
@@ -2192,6 +2193,14 @@ struct vxb_mesh
 	DevBuf<vxb_draw_info> drawInfo, drawTInfo;
 	DevBuf<unsigned int> drawCounts;
 	vxb_draw_lists drawLists;
+	// bounds: two float4 {min, max} per (level, coord) slot, written by the apply; `bounds` describes them as of the last apply
+	DevBuf<float4> boxes;
+	vxb_mesh_bounds bounds;
+	DevBuf<float> boundsOut;                    // vxb_mesh_download_bounds' device staging
+	// vxb_mesh_select_lod_views: view v owns entries [v * stride, +stride) (transition: 6 x) and counts[2v], counts[2v + 1]
+	DevBuf<vxb_draw_command> viewCmd, viewTCmd;
+	DevBuf<vxb_draw_info> viewInfo, viewTInfo;
+	DevBuf<unsigned int> viewCounts;
 	cudaEvent_t ev[2] = { nullptr, nullptr };
 	bool content = false;                       // a run has been applied
 	uint64_t serial = 0;                        // vxb_context::runSerial of that run
@@ -2343,6 +2352,7 @@ int vxb_mesh_create(vxb_context* ctx, const uint64_t capacity[4], vxb_mesh** out
 	m->ctx = ctx;
 	memset(&m->info, 0, sizeof(m->info));
 	memset(&m->drawLists, 0, sizeof(m->drawLists));
+	memset(&m->bounds, 0, sizeof(m->bounds));
 	cudaError_t e = cudaEventCreate(&m->ev[0]);
 	if (e == cudaSuccess) e = cudaEventCreate(&m->ev[1]);
 	if (e == cudaSuccess && capacity)
@@ -2406,6 +2416,7 @@ int vxb_mesh_apply(vxb_mesh* m)
 		VXB_CUDA(ctx, m->drawCmd.ensure(slots)); VXB_CUDA(ctx, m->drawInfo.ensure(slots));
 		VXB_CUDA(ctx, m->drawTCmd.ensure(slots * 6)); VXB_CUDA(ctx, m->drawTInfo.ensure(slots * 6));
 		VXB_CUDA(ctx, m->drawCounts.ensure(2));
+		VXB_CUDA(ctx, m->boxes.ensure(slots * 2));
 		m->dirCap = slots;
 		++m->info.generation;
 	}
@@ -2472,6 +2483,9 @@ int vxb_mesh_apply(vxb_mesh* m)
 	bool anyUnmapped = false;
 	for (unsigned i = 0; i < 256; ++i) if (!ctx->lutValid[i] && ((ctx->info.used_materials[i >> 5] >> (i & 31)) & 1u)) anyUnmapped = true;
 
+	// the boxes of the blocks that leave: all of them, or the ones in the dirty range (the copy writes the new blocks')
+	if (!region) vxb_mesh_bounds_reset_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(m->boxes.p, (unsigned)slots);
+	else if (meshCount) vxb_mesh_bounds_erase_kernel<<<(meshCount + 255) / 256, 256, 0, st>>>(m->dir.p, meshCount, g, m->boxes.p);
 	if (all)
 	{
 		VXB_CUDA(ctx, cub::DeviceScan::ExclusiveScan(m->cubTemp.p, tempBytes, m->items.p, m->prefix.p, VxbMeshScanSum(), VxbMeshScan{ 0, 0, 0, 0, 0 }, (int)all, st));
@@ -2486,7 +2500,7 @@ int vxb_mesh_apply(vxb_mesh* m)
 	runSrc.v = ctx->verts.p; runSrc.i = ctx->idx.p; runSrc.tv = ctx->tverts.p; runSrc.ti = ctx->tidx.p;
 	if (jobs)
 		vxb_mesh_copy_kernel<<<jobs, 128, 0, st>>>(m->jobSrc.p, m->jobDst.p, m->dir.p, ctx->records.p, m->scratch.p, m->set[m->active].view(),
-			runSrc, m->set[target].view(), anyUnmapped ? 1 : 0);
+			runSrc, m->set[target].view(), anyUnmapped ? 1 : 0, m->keys.p, m->boxes.p);
 	VXB_CUDA(ctx, cudaGetLastError());
 	const unsigned merged = survivors + fresh;
 	if (merged) VXB_CUDA(ctx, cudaMemcpyAsync(m->dir.p, m->scratch.p, sizeof(vxb_block_record) * merged, cudaMemcpyDeviceToDevice, st));
@@ -2519,6 +2533,9 @@ int vxb_mesh_apply(vxb_mesh* m)
 	memcpy(i.stats, ctx->info.stats, sizeof(i.stats));
 	i.bytes_copied = copied;
 	VXB_CUDA(ctx, cudaEventElapsedTime(&i.apply_ms, m->ev[0], m->ev[1]));
+	m->bounds.boxes = reinterpret_cast<const float*>(m->boxes.p);
+	for (int l = 0; l < VXB_MAX_LEVELS; ++l) m->bounds.level_base[l] = g.levelBase[l];
+	m->bounds.slots = (uint32_t)slots;
 	m->content = true;
 	m->serial = ctx->runSerial;
 	m->n = n;
@@ -2575,6 +2592,86 @@ int vxb_mesh_select_lod(vxb_mesh* m, const float camera[3], float baseDistance, 
 		m->drawCounts, m->drawLists);
 	if (r != VXB_OK) return r;
 	if (out) *out = m->drawLists;
+	return VXB_OK;
+}
+
+int vxb_mesh_bounds_get(vxb_mesh* m, vxb_mesh_bounds* out)
+{
+	if (!m || !out) return VXB_ERR_ARGUMENT;
+	if (!m->content) return fail(m->ctx, VXB_ERR_STATE, "vxb_mesh_bounds_get: nothing applied yet");
+	*out = m->bounds;
+	return VXB_OK;
+}
+
+int vxb_mesh_download_bounds(vxb_mesh* m, float* bounds)
+{
+	if (!m || !bounds) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_download_bounds: nothing applied yet");
+	cudaSetDevice(ctx->device);
+	const unsigned blocks = m->info.block_count;
+	if (!blocks) return VXB_OK;
+	VXB_CUDA(ctx, m->boundsOut.ensure((size_t)blocks * 6));
+	vxb_mesh_bounds_gather_kernel<<<(blocks + 255) / 256, 256, 0, ctx->stream>>>(m->dir.p, blocks, m->bounds, m->boundsOut.p);
+	VXB_CUDA(ctx, cudaGetLastError());
+	VXB_CUDA(ctx, cudaMemcpyAsync(bounds, m->boundsOut.p, sizeof(float) * 6 * blocks, cudaMemcpyDeviceToHost, ctx->stream));
+	VXB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	return VXB_OK;
+}
+
+int vxb_mesh_select_lod_views(vxb_mesh* m, const float camera[3], float baseDistance, const vxb_view* views, uint32_t viewCount,
+	vxb_draw_lists* out)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!camera || !views || !out) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_select_lod_views: NULL lod_camera, views or out");
+	if (viewCount == 0 || viewCount > VXB_VIEWS_MAX) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_select_lod_views: view_count must be in [1, 8]");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_select_lod_views: nothing applied yet");
+	VxbViews vs;
+	memset(&vs, 0, sizeof(vs));
+	for (uint32_t v = 0; v < viewCount; ++v)
+	{
+		for (int k = 0; k < 6; ++k)
+			for (int c = 0; c < 4; ++c)
+				if (!std::isfinite(views[v].planes[k][c]))
+				{
+					char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_select_lod_views: view %u plane %d: non-finite component", v, k);
+					return fail(ctx, VXB_ERR_ARGUMENT, buf);
+				}
+		vs.view[v] = views[v];
+	}
+	cudaSetDevice(ctx->device);
+	cudaStream_t st = ctx->stream;
+	const uint32_t blocks = m->info.block_count;
+	const size_t stride = blocks ? blocks : 1;
+	VXB_CUDA(ctx, m->viewCmd.ensure(stride * viewCount)); VXB_CUDA(ctx, m->viewInfo.ensure(stride * viewCount));
+	VXB_CUDA(ctx, m->viewTCmd.ensure(stride * viewCount * 6)); VXB_CUDA(ctx, m->viewTInfo.ensure(stride * viewCount * 6));
+	VXB_CUDA(ctx, m->viewCounts.ensure(2 * VXB_VIEWS_MAX));
+	VXB_CUDA(ctx, cudaMemsetAsync(m->viewCounts.p, 0, sizeof(unsigned int) * 2 * VXB_VIEWS_MAX, st));
+	VxbDev d;
+	memset(&d, 0, sizeof(d));
+	d.n = (int)m->n; d.levels = (int)m->info.levels; d.lastLevel = d.levels - 1;
+	d.records = m->dir.p;
+	for (int l = 0; l < VXB_MAX_LEVELS; ++l) d.idBase[l] = m->bounds.level_base[l];
+	VxbLodArgs a;
+	for (int k = 0; k < 3; ++k) a.camera[k] = camera[k];
+	a.baseDistance = baseDistance;
+	a.counts = m->viewCounts.p;
+	a.regular = m->viewCmd.p; a.regularInfo = m->viewInfo.p; a.transition = m->viewTCmd.p; a.transitionInfo = m->viewTInfo.p;
+	a.capacity = (unsigned)(stride * 6);
+	if (blocks) vxb_lod_select_views_kernel<<<(blocks + 255) / 256, 256, 0, st>>>(d, a, blocks, vs, viewCount, m->boxes.p, (unsigned)stride);
+	unsigned n[2 * VXB_VIEWS_MAX];
+	VXB_CUDA(ctx, cudaMemcpyAsync(n, m->viewCounts.p, sizeof(n), cudaMemcpyDeviceToHost, st));
+	VXB_CUDA(ctx, cudaStreamSynchronize(st));
+	VXB_CUDA(ctx, cudaGetLastError());
+	for (uint32_t v = 0; v < viewCount; ++v)
+	{
+		vxb_draw_lists& l = out[v];
+		l.regular_count = n[2 * v]; l.transition_count = n[2 * v + 1];
+		l.counts = m->viewCounts.p + 2 * v;
+		l.regular = m->viewCmd.p + stride * v; l.regular_info = m->viewInfo.p + stride * v;
+		l.transition = m->viewTCmd.p + stride * v * 6; l.transition_info = m->viewTInfo.p + stride * v * 6;
+	}
 	return VXB_OK;
 }
 

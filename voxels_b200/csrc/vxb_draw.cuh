@@ -47,16 +47,10 @@ __device__ __forceinline__ bool vxb_lod_finer(const VxbDev& d, const VxbLodArgs&
 	return level > 0;
 }
 
-// one thread per emitted block (directory slot)
-__global__ void __launch_bounds__(256) vxb_lod_select_kernel(const VxbDev d, const VxbLodArgs a, const unsigned int blockCount)
+// which faces of the block border a region drawn finer (bit f in the output enum order = internal order z-, y-, x-, z+, y+, x+
+// of vxb_finish_kernel); level 0 has none
+__device__ __forceinline__ unsigned vxb_lod_block_adj(const VxbDev& d, const VxbLodArgs& a, int level, int nb, int bx, int by, int bz)
 {
-	const unsigned slot = blockIdx.x * blockDim.x + threadIdx.x;
-	if (slot >= blockCount) return;
-	const vxb_block_record r = d.records[slot];
-	const int level = (int)r.level, nb = (d.n >> 4) >> level;
-	const int bx = r.coord_id % nb, by = (r.coord_id / nb) % nb, bz = r.coord_id / (nb * nb);
-	if (!vxb_lod_selected(d, a, level, bx, by, bz)) return;
-	// faces in the output enum order = internal order z-, y-, x-, z+, y+, x+ (vxb_finish_kernel)
 	unsigned adj = 0;
 	if (level > 0)
 	{
@@ -68,6 +62,12 @@ __global__ void __launch_bounds__(256) vxb_lod_select_kernel(const VxbDev d, con
 			if (vxb_lod_finer(d, a, level, nx, ny, nz)) adj |= 1u << f;
 		}
 	}
+	return adj;
+}
+
+// the block's regular draw and the transition draws `adj` asks for, appended to a's lists
+__device__ __forceinline__ void vxb_lod_emit(const VxbLodArgs& a, const vxb_block_record& r, unsigned adj)
+{
 	const unsigned k = atomicAdd(&a.counts[0], 1u);
 	if (k < a.capacity)
 	{
@@ -89,5 +89,63 @@ __global__ void __launch_bounds__(256) vxb_lod_select_kernel(const VxbDev d, con
 		vxb_draw_info inf;
 		inf.block_id = r.id; inf.level = r.level; inf.block_adj = adj; inf.face = (unsigned)f;
 		a.transitionInfo[t] = inf;
+	}
+}
+
+// one thread per emitted block (directory slot)
+__global__ void __launch_bounds__(256) vxb_lod_select_kernel(const VxbDev d, const VxbLodArgs a, const unsigned int blockCount)
+{
+	const unsigned slot = blockIdx.x * blockDim.x + threadIdx.x;
+	if (slot >= blockCount) return;
+	const vxb_block_record r = d.records[slot];
+	const int level = (int)r.level, nb = (d.n >> 4) >> level;
+	const int bx = r.coord_id % nb, by = (r.coord_id / nb) % nb, bz = r.coord_id / (nb * nb);
+	if (!vxb_lod_selected(d, a, level, bx, by, bz)) return;
+	vxb_lod_emit(a, r, vxb_lod_block_adj(d, a, level, nb, bx, by, bz));
+}
+
+// The same cut, culled against view frusta (include/vxb200.h "culled select").  Only the frustum differs between the views: the
+// cut and block_adj are the LOD camera's in every one of them (a cut per view would draw different geometry in a shadow and
+// a colour pass).  boxes: the mesh's per-block bounds, slot d.idBase[level] + coord_id, {min xyz, 0}, {max xyz, 0}.
+struct VxbViews
+{
+	vxb_view view[VXB_VIEWS_MAX];
+};
+
+// does the box pass every plane of the view: the p-vertex test, float32 without fused multiply-add in the header's order
+__device__ __forceinline__ bool vxb_view_sees(const vxb_view& v, const float4& lo, const float4& hi)
+{
+	bool in = true;
+	for (int k = 0; k < 6; ++k)
+	{
+		const float nx = v.planes[k][0], ny = v.planes[k][1], nz = v.planes[k][2];
+		const float cx = nx >= 0.f ? hi.x : lo.x, cy = ny >= 0.f ? hi.y : lo.y, cz = nz >= 0.f ? hi.z : lo.z;
+		const float s = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(nx, cx), __fmul_rn(ny, cy)), __fmul_rn(nz, cz)), v.planes[k][3]);
+		in = in && s >= 0.f;
+	}
+	return in;
+}
+
+// one thread per directory slot; view v appends to counts[2v], counts[2v + 1] and to its `stride` (regular) / 6 * stride
+// (transition) entries of a's lists
+__global__ void __launch_bounds__(256) vxb_lod_select_views_kernel(const VxbDev d, const VxbLodArgs a, const unsigned int blockCount,
+	const __grid_constant__ VxbViews views, const unsigned int viewCount, const float4* __restrict__ boxes, const unsigned int stride)
+{
+	const unsigned slot = blockIdx.x * blockDim.x + threadIdx.x;
+	if (slot >= blockCount) return;
+	const vxb_block_record r = d.records[slot];
+	const int level = (int)r.level, nb = (d.n >> 4) >> level;
+	const int bx = r.coord_id % nb, by = (r.coord_id / nb) % nb, bz = r.coord_id / (nb * nb);
+	if (!vxb_lod_selected(d, a, level, bx, by, bz)) return;
+	const unsigned adj = vxb_lod_block_adj(d, a, level, nb, bx, by, bz);
+	const float4 lo = boxes[2 * (size_t)(d.idBase[level] + r.coord_id)], hi = boxes[2 * (size_t)(d.idBase[level] + r.coord_id) + 1];
+	for (unsigned v = 0; v < viewCount; ++v)
+	{
+		if (!vxb_view_sees(views.view[v], lo, hi)) continue;
+		VxbLodArgs av = a;
+		av.counts += 2 * v;
+		av.regular += (size_t)v * stride; av.regularInfo += (size_t)v * stride;
+		av.transition += (size_t)v * stride * 6; av.transitionInfo += (size_t)v * stride * 6;
+		vxb_lod_emit(av, r, adj);
 	}
 }

@@ -8,6 +8,8 @@
 // jobs) -> copy (one CTA per block).  The directory is rewritten densely; the arenas keep the survivors in place and
 // take the new blocks at their tail, or - when the tail would overflow or the garbage exceeds the live data - are
 // compacted into the second arena set.
+// Beside the directory the mesh keeps one box per (level, coord) slot - the sort key's slot space, so a survivor's box
+// never moves: the exact bounds of the block's vertices (include/vxb200.h "bounds"), reduced by the copy of a new block.
 #pragma once
 
 #include <cub/cub.cuh>
@@ -193,16 +195,33 @@ __global__ void __launch_bounds__(256) vxb_mesh_place_kernel(const vxb_block_rec
 }
 
 // vertices as 16-byte words (3 per 48-byte vertex); the third word of a vertex is {nrm.y, nrm.z, tex[0], tex[1]}: the
-// unmapped-material marker of vxb_finish_vertex (tex[0] low byte 0xFF) becomes the reference's all-zero textures
-__device__ __forceinline__ void vxb_mesh_copy_vertices(const VxbVertex* src, VxbVertex* dst, unsigned count, int fixMarkers)
+// unmapped-material marker of vxb_finish_vertex (tex[0] low byte 0xFF) becomes the reference's all-zero textures.
+// bound: the thread's running min / max of pos[0..2] and sec[0..2] take in the words that pass through it: the first
+// word of a vertex is {pos.x, pos.y, pos.z, sec.x}, the second starts with {sec.y, sec.z}
+__device__ __forceinline__ void vxb_mesh_copy_vertices(const VxbVertex* src, VxbVertex* dst, unsigned count, int fixMarkers, bool bound,
+	float (&lo)[3], float (&hi)[3])
 {
 	const uint4* s = reinterpret_cast<const uint4*>(src);
 	uint4* d = reinterpret_cast<uint4*>(dst);
 	for (unsigned k = threadIdx.x; k < 3 * count; k += blockDim.x)
 	{
 		uint4 w = __ldg(s + k);
-		if (fixMarkers && k % 3 == 2 && (w.z & 0xFFu) == 0xFFu) { w.z = 0; w.w = 0; }
+		const unsigned part = k % 3;
+		if (fixMarkers && part == 2 && (w.z & 0xFFu) == 0xFFu) { w.z = 0; w.w = 0; }
 		d[k] = w;
+		if (bound && part == 0)
+		{
+			const float x = __uint_as_float(w.x), y = __uint_as_float(w.y), z = __uint_as_float(w.z), sx = __uint_as_float(w.w);
+			lo[0] = fminf(lo[0], fminf(x, sx)); hi[0] = fmaxf(hi[0], fmaxf(x, sx));
+			lo[1] = fminf(lo[1], y); hi[1] = fmaxf(hi[1], y);
+			lo[2] = fminf(lo[2], z); hi[2] = fmaxf(hi[2], z);
+		}
+		else if (bound && part == 1)
+		{
+			const float sy = __uint_as_float(w.x), sz = __uint_as_float(w.y);
+			lo[1] = fminf(lo[1], sy); hi[1] = fmaxf(hi[1], sy);
+			lo[2] = fminf(lo[2], sz); hi[2] = fmaxf(hi[2], sz);
+		}
 	}
 }
 
@@ -234,12 +253,52 @@ __device__ __forceinline__ void vxb_mesh_copy_indices(const unsigned* src, unsig
 	}
 }
 
+// the box of a slot without a block: min > max
+__device__ __forceinline__ void vxb_mesh_box_clear(float4* __restrict__ boxes, unsigned slot)
+{
+	const float inf = __int_as_float(0x7F800000);
+	boxes[2 * (size_t)slot] = make_float4(inf, inf, inf, 0.f);
+	boxes[2 * (size_t)slot + 1] = make_float4(-inf, -inf, -inf, 0.f);
+}
+
+// a full apply: every slot starts without a block
+__global__ void __launch_bounds__(256) vxb_mesh_bounds_reset_kernel(float4* __restrict__ boxes, unsigned slots)
+{
+	const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t < slots) vxb_mesh_box_clear(boxes, t);
+}
+
+// a region apply: the slots of the erased blocks
+__global__ void __launch_bounds__(256) vxb_mesh_bounds_erase_kernel(const vxb_block_record* __restrict__ mesh, unsigned meshCount,
+	const VxbMeshRange g, float4* __restrict__ boxes)
+{
+	const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t >= meshCount) return;
+	const vxb_block_record r = mesh[t];
+	if (vxb_mesh_dirty(g, r)) vxb_mesh_box_clear(boxes, g.levelBase[r.level] + r.coord_id);
+}
+
+// the boxes in directory order, 6 floats per block (vxb_mesh_download_bounds)
+__global__ void __launch_bounds__(256) vxb_mesh_bounds_gather_kernel(const vxb_block_record* __restrict__ mesh, unsigned meshCount,
+	const __grid_constant__ vxb_mesh_bounds b, float* __restrict__ out)
+{
+	const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t >= meshCount) return;
+	const float* box = b.boxes + 8 * (size_t)(b.level_base[mesh[t].level] + mesh[t].coord_id);
+	float* o = out + 6 * (size_t)t;
+	o[0] = box[0]; o[1] = box[1]; o[2] = box[2]; o[3] = box[4]; o[4] = box[5]; o[5] = box[6];
+}
+
 // one CTA per job: the block's regular and transition vertices and indices from its source arenas (the mesh's other
-// set for survivors of a compaction, the context's result for new blocks) to the ranges `out` gives it
+// set for survivors of a compaction, the context's result for new blocks) to the ranges `out` gives it.  A new block's
+// box is reduced from the vertices on their way through the registers and stored at its (level, coord) slot: keys[run
+// slot], as the count kernel wrote it (the sort leaves its input as it was).  A survivor keeps the box it has.
 __global__ void __launch_bounds__(128) vxb_mesh_copy_kernel(const unsigned* __restrict__ jobSrc, const unsigned* __restrict__ jobDst,
 	const vxb_block_record* __restrict__ mesh, const vxb_block_record* __restrict__ run, const vxb_block_record* __restrict__ out,
-	const VxbMeshArenas meshSrc, const VxbMeshArenas runSrc, const VxbMeshArenas dst, int fixMarkers)
+	const VxbMeshArenas meshSrc, const VxbMeshArenas runSrc, const VxbMeshArenas dst, int fixMarkers,
+	const unsigned* __restrict__ keys, float4* __restrict__ boxes)
 {
+	__shared__ float sBox[4][6];
 	const unsigned src = jobSrc[blockIdx.x];
 	const bool fresh = (src & 0x80000000u) != 0;
 	const vxb_block_record& s = fresh ? run[src & 0x7FFFFFFFu] : mesh[src];
@@ -249,11 +308,36 @@ __global__ void __launch_bounds__(128) vxb_mesh_copy_kernel(const unsigned* __re
 	const unsigned* i = fresh ? runSrc.i : meshSrc.i;
 	const VxbVertex* tv = fresh ? runSrc.tv : meshSrc.tv;
 	const unsigned* ti = fresh ? runSrc.ti : meshSrc.ti;
-	vxb_mesh_copy_vertices(v + s.vertex_offset, dst.v + o.vertex_offset, s.vertex_count, fixMarkers);
+	const float inf = __int_as_float(0x7F800000);
+	float lo[3] = { inf, inf, inf }, hi[3] = { -inf, -inf, -inf };
+	vxb_mesh_copy_vertices(v + s.vertex_offset, dst.v + o.vertex_offset, s.vertex_count, fixMarkers, fresh, lo, hi);
 	vxb_mesh_copy_indices(i + s.index_offset, dst.i + o.index_offset, s.index_count);
 	for (int f = 0; f < 6; ++f)
 	{
-		vxb_mesh_copy_vertices(tv + s.trans_vertex_offset[f], dst.tv + o.trans_vertex_offset[f], s.trans_vertex_count[f], fixMarkers);
+		vxb_mesh_copy_vertices(tv + s.trans_vertex_offset[f], dst.tv + o.trans_vertex_offset[f], s.trans_vertex_count[f], fixMarkers, fresh, lo, hi);
 		vxb_mesh_copy_indices(ti + s.trans_index_offset[f], dst.ti + o.trans_index_offset[f], s.trans_index_count[f]);
+	}
+	if (!fresh) return; // the whole CTA
+	// min and max are exact: the box does not depend on the order of this reduction
+	for (int a = 0; a < 3; ++a)
+		for (int sh = 16; sh; sh >>= 1)
+		{
+			lo[a] = fminf(lo[a], __shfl_xor_sync(0xFFFFFFFFu, lo[a], sh));
+			hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xFFFFFFFFu, hi[a], sh));
+		}
+	if ((threadIdx.x & 31) == 0)
+		for (int a = 0; a < 3; ++a) { sBox[threadIdx.x >> 5][a] = lo[a]; sBox[threadIdx.x >> 5][3 + a] = hi[a]; }
+	__syncthreads();
+	if (threadIdx.x < 2)
+	{
+		// thread 0: min, thread 1: max, over the four warps
+		const int b = 3 * threadIdx.x;
+		float c[3];
+		for (int a = 0; a < 3; ++a)
+		{
+			c[a] = sBox[0][b + a];
+			for (int w = 1; w < 4; ++w) c[a] = threadIdx.x ? fmaxf(c[a], sBox[w][b + a]) : fminf(c[a], sBox[w][b + a]);
+		}
+		boxes[2 * (size_t)keys[src & 0x7FFFFFFFu] + threadIdx.x] = make_float4(c[0], c[1], c[2], 0.f);
 	}
 }
