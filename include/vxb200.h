@@ -462,6 +462,55 @@ typedef struct vxb_view { float planes[6][4]; } vxb_view;
 int vxb_mesh_select_lod_views(vxb_mesh* mesh, const float lod_camera[3], float base_distance,
                               const vxb_view* views, uint32_t view_count, vxb_draw_lists* out /* view_count entries */);
 
+/* ---- the LOD cut: a descending, balanced cut of the mesh's octree, culled against up to eight views ----------------------
+ * vxb_mesh_select_cut draws the mesh at every level of detail: fine blocks near lod_camera, coarser ones farther away,
+ * never two touching blocks more than one level apart, so the transition meshes close every seam (Rendering.md:23,35-38).
+ * The rule.  A node (level l, grid block coordinates b) has the lattice box, in OUTPUT (Y-up) axes:
+ *     s = 16 * 2^l,   lo = (bx, bz, by) * s,   hi = lo + s
+ * and, in float32 without fused multiply-add, in exactly this order (c = lod_camera):
+ *     e_i    = max(max(lo_i - c_i, c_i - hi_i), 0)          i = x, y, z
+ *     dist2  = ((ex*ex + ey*ey) + ez*ez)
+ *     lim    = lod_factor * s
+ *     refine(l, b) = l > 0 && dist2 < lim*lim
+ *     on the cut   = !refine(l, b) && (l == top || refine(l + 1, b >> 1))
+ *     block_adj bit f (TransitionFaceId order, as above) = the same-level neighbour across face f is inside the grid and
+ *                  refine(l, neighbour)
+ * In words: a node is refined while the camera is closer than lod_factor times its edge length to its box (0 inside it).
+ * Monotone, also in float32.  A child's box lies inside its parent's box, so every lo_i - c_i and c_i - hi_i of the child is
+ * at most the parent's; rounding is monotone, so every e_i, each product and each sum can only grow from the parent to the
+ * child.  The child's lim is exactly half the parent's (s is a power of two), so its lim*lim is at most the parent's.  Hence
+ * refine(child) implies refine(parent), and by induction every ancestor's.  That is why "on the cut" is the O(1) test
+ * above: a node whose parent refines has every ancestor refining, with no loop over the ancestors; and the cut tiles the
+ * grid, every level-0 block lying under exactly one node of the cut.
+ * Balanced for lod_factor >= sqrt(3).  Let N (level l, edge s_l) be on the cut and touch (share a face, an edge or a
+ * corner with) a cut node of level <= l - 2.  That node's ancestor P of level l - 1 refines (a node of the cut has every
+ * ancestor refining) and touches N (it contains the touching node, and it is not inside N, whose descendants do not refine).  The distance from the camera
+ * to a box grows by at most the diameter of the boxes it is measured across, so with k = lod_factor
+ *     dist(N) <= dist(P) + diam(P) < k*s_l/2 + sqrt(3)*s_l/2 = (k + sqrt(3))*s_l/2 <= k*s_l    for k >= sqrt(3),
+ * which contradicts N not refining.  So every pair of touching cut nodes differs by at
+ * most one level, and the finer neighbours a drawn block's block_adj names are exactly one level finer - the case the
+ * transition meshes are made for.  The call refuses lod_factor < VXB_LOD_FACTOR_MIN (a margin over sqrt(3) against the
+ * rounding of the float formula), NaN and infinity.
+ * Choosing lod_factor.  A cell of a level-l block spans 2^l voxels and the block's edge is 16 cells, so where the block stops
+ * refining (distance lod_factor * s) a cell covers about H / (32 * tan(theta / 2) * lod_factor) pixels of a viewport H
+ * pixels high with a vertical field of view theta.  For at most p pixels per cell: lod_factor = H / (32 * tan(theta / 2) * p);
+ * e.g. 1080 px, 60 degrees, 4 px per cell: 14.6.
+ * Views.  The culling is vxb_mesh_select_lod_views', unchanged: a block of the cut is in view v's lists iff its box passes
+ * every plane of the view (the p-vertex test above); its transition draws follow it; block_adj is the cut's and does not
+ * depend on visibility; the order within a list is unspecified; first_instance is the draw's index into its own view's
+ * info array.  For an unculled cut pass one view of pass-everything planes.
+ * Buffers.  The lists are the call's own device buffers (per view block_count regular and 6 x block_count transition
+ * entries); they stay valid until the next vxb_mesh_select_cut or until an apply changes `generation`, and the call leaves
+ * the lists of vxb_mesh_select_lod and vxb_mesh_select_lod_views as they are.  The call blocks (one read of the counts).
+ * Refusals (previous lists and `out` untouched): VXB_ERR_STATE before the first apply, and when the mesh does not hold
+ * every level with its transition meshes - some run applied since the last full apply had max_levels below the grid's
+ * levels or VXB_FLAG_NO_TRANSITIONS (the next complete full run and apply lift it); VXB_ERR_ARGUMENT for a NULL pointer,
+ * view_count = 0 or > VXB_VIEWS_MAX, a non-finite plane component (vxb_last_error names the view and the plane), a
+ * non-finite lod_camera component, and a bad lod_factor. */
+#define VXB_LOD_FACTOR_MIN 2.0f
+int vxb_mesh_select_cut(vxb_mesh* mesh, const float lod_camera[3], float lod_factor,
+                        const vxb_view* views, uint32_t view_count, vxb_draw_lists* out /* view_count entries */);
+
 /* ---- ray queries against the mesh: picking, line of sight, projectile hits, without leaving HBM ------------------------
  * Rays are cast against the LEVEL-0 regular triangles of the mesh (the full-detail surface, the one edits change); levels >= 1
  * and transition meshes are not part of the query.

@@ -203,6 +203,7 @@ class MeshInfo(C.Structure):
 
 
 VXB_VIEWS_MAX = 8
+VXB_LOD_FACTOR_MIN = 2.0
 
 
 class View(C.Structure):
@@ -327,6 +328,7 @@ def load_library():
         "vxb_mesh_bounds_get": (C.c_int, [vp, C.POINTER(MeshBounds)]),
         "vxb_mesh_download_bounds": (C.c_int, [vp, vp]),
         "vxb_mesh_select_lod_views": (C.c_int, [vp, vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_select_cut": (C.c_int, [vp, vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_raycast": (C.c_int, [vp, vp, u32, vp]),
         "vxb_mesh_raycast_device": (C.c_int, [vp, vp, u32, vp]),
         "vxb_mesh_sphere_cast": (C.c_int, [vp, C.c_float, vp, u32, vp]),
@@ -354,7 +356,7 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_grid_fill_program", "vxb_grid_inject_program", "vxb_grid_program_stats",
                     "vxb_mesh_create", "vxb_mesh_destroy", "vxb_mesh_apply", "vxb_mesh_info_get", "vxb_mesh_download",
                     "vxb_mesh_device_arenas", "vxb_mesh_select_lod", "vxb_mesh_bounds_get", "vxb_mesh_download_bounds",
-                    "vxb_mesh_select_lod_views", "vxb_mesh_raycast", "vxb_mesh_raycast_device",
+                    "vxb_mesh_select_lod_views", "vxb_mesh_select_cut", "vxb_mesh_raycast", "vxb_mesh_raycast_device",
                     "vxb_mesh_sphere_cast", "vxb_mesh_sphere_cast_device", "vxb_mesh_closest_point", "vxb_mesh_closest_point_device"]
 
 
@@ -538,6 +540,27 @@ class Mesh:
                  _device_to_numpy(l.regular_info, l.regular_count, DRAW_INFO_DTYPE),
                  _device_to_numpy(l.transition, l.transition_count, DRAW_COMMAND_DTYPE),
                  _device_to_numpy(l.transition_info, l.transition_count, DRAW_INFO_DTYPE)) for l in lists]
+
+    def select_cut_rc(self, lod_camera, lod_factor, views, lists_out=None, count=None):
+        """vxb_mesh_select_cut's return code: `lod_camera` and `views` ([views, 6, 4] plane coefficients or a View array) may be
+        None for NULL pointers, `lists_out` (a DrawLists array) None for a NULL out; `count` defaults to len(views)."""
+        cam = np.ascontiguousarray(lod_camera, np.float32) if lod_camera is not None else None
+        if views is not None and not isinstance(views, C.Array):
+            views = make_views(views)
+        n = (0 if views is None else len(views)) if count is None else count
+        return self.L.vxb_mesh_select_cut(self.h, _ptr(cam), lod_factor, views, n, lists_out)
+
+    def select_cut(self, lod_camera, lod_factor, views, lists_out=None):
+        """vxb_mesh_select_cut: the balanced LOD cut of (lod_camera, lod_factor) culled against each of `views` ([views, 6, 4]
+        plane coefficients or a View array).  Returns, per view, the four arrays select_lod returns; the device-resident
+        vxb_draw_lists go to `lists_out` (a DrawLists array of len(views)) when given."""
+        views = views if isinstance(views, C.Array) else make_views(views)
+        lists = (DrawLists * len(views))() if lists_out is None else lists_out
+        self.ctx._check(self.select_cut_rc(lod_camera, lod_factor, views, lists), "vxb_mesh_select_cut")
+        return [(_device_to_numpy(l.regular, l.regular_count, DRAW_COMMAND_DTYPE),
+                 _device_to_numpy(l.regular_info, l.regular_count, DRAW_INFO_DTYPE),
+                 _device_to_numpy(l.transition, l.transition_count, DRAW_COMMAND_DTYPE),
+                 _device_to_numpy(l.transition_info, l.transition_count, DRAW_INFO_DTYPE)) for l in lists[:len(views)]]
 
     def raycast_rc(self, rays, hits=None):
         """vxb_mesh_raycast's return code for a RAY_DTYPE array; the hits go to `hits` (a RAY_HIT_DTYPE array, or None for a

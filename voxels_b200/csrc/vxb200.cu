@@ -206,6 +206,7 @@ struct vxb_context
 	bool haveResult = false;
 	uint64_t runSerial = 0;                 // counts the runs (vxb_polygonize*), so that a mesh can tell whether it missed one
 	bool resultSharded = false, resultRegion = false;
+	bool resultComplete = false;            // the last run made every level and the transition meshes (vxb_mesh_select_cut)
 	std::vector<vxb_mesh*> meshes;          // released by vxb_destroy
 	vxb_result_info info;
 	std::vector<vxb_block_record> sortedRecords;
@@ -1644,6 +1645,7 @@ struct Run
 		memcpy(ctx->runEmit, hc.emitCount, sizeof(ctx->runEmit));
 		ctx->haveResult = true;
 		ctx->resultSharded = sharded; ctx->resultRegion = region != nullptr;
+		ctx->resultComplete = computed == ctx->levels && dev.transitions;
 		if (!region && !sharded) { ctx->haveFullRun = (computed == ctx->levels); ctx->nextId = (uint32_t)L.totalBlocks; }
 		else if (sharded) ctx->haveFullRun = false;
 	}
@@ -2091,7 +2093,7 @@ int selectLod(vxb_context* ctx, const VxbDev& d, uint32_t blocks, size_t cap, co
 	VXB_CUDA(ctx, cudaMemsetAsync(counts.p, 0, 8, ctx->stream));
 	VxbLodArgs a;
 	for (int k = 0; k < 3; ++k) a.camera[k] = camera[k];
-	a.baseDistance = baseDistance;
+	a.lod = baseDistance;
 	a.counts = counts.p;
 	a.regular = cmd.p; a.regularInfo = info.p; a.transition = tcmd.p; a.transitionInfo = tinfo.p;
 	a.capacity = (unsigned)(cap * 6);
@@ -2197,12 +2199,17 @@ struct vxb_mesh
 	DevBuf<float4> boxes;
 	vxb_mesh_bounds bounds;
 	DevBuf<float> boundsOut;                    // vxb_mesh_download_bounds' device staging
-	// vxb_mesh_select_lod_views: view v owns entries [v * stride, +stride) (transition: 6 x) and counts[2v], counts[2v + 1]
-	DevBuf<vxb_draw_command> viewCmd, viewTCmd;
-	DevBuf<vxb_draw_info> viewInfo, viewTInfo;
-	DevBuf<unsigned int> viewCounts;
+	// the per-view lists of vxb_mesh_select_lod_views and of vxb_mesh_select_cut, each call its own: view v owns entries
+	// [v * stride, +stride) (transition: 6 x) and counts[2v], counts[2v + 1]
+	struct ViewLists
+	{
+		DevBuf<vxb_draw_command> cmd, tcmd;
+		DevBuf<vxb_draw_info> info, tinfo;
+		DevBuf<unsigned int> counts;
+	} viewLists, cutLists;
 	cudaEvent_t ev[2] = { nullptr, nullptr };
 	bool content = false;                       // a run has been applied
+	bool complete = false;                      // every run applied since the last full apply made all levels and transitions
 	uint64_t serial = 0;                        // vxb_context::runSerial of that run
 	uint32_t n = 0;
 	vxb_mesh_info info;
@@ -2337,6 +2344,62 @@ long long invalidRay(const vxb_ray* rays, uint32_t count, const char** why)
 		if (x.t_min > x.t_max) { *why = "t_min > t_max"; return r; }
 	}
 	return -1;
+}
+
+// The culled selects' shared body, after the caller's NULL, view-count and state checks: the plane check (a refusal names the
+// view and the plane and leaves `lists` and `out` untouched), one pass of vxb_lod_select_views_kernel<Cut> into `lists`, one
+// read of the counts.  lod: the Cut's parameter (VxbLodArgs::lod).
+template <class Cut>
+int selectViews(vxb_mesh* m, const char* what, const float camera[3], float lod, const vxb_view* views, uint32_t viewCount,
+	vxb_mesh::ViewLists& lists, vxb_draw_lists* out)
+{
+	vxb_context* ctx = m->ctx;
+	VxbViews vs;
+	memset(&vs, 0, sizeof(vs));
+	for (uint32_t v = 0; v < viewCount; ++v)
+	{
+		for (int k = 0; k < 6; ++k)
+			for (int c = 0; c < 4; ++c)
+				if (!std::isfinite(views[v].planes[k][c]))
+				{
+					char buf[160]; snprintf(buf, sizeof(buf), "%s: view %u plane %d: non-finite component", what, v, k);
+					return fail(ctx, VXB_ERR_ARGUMENT, buf);
+				}
+		vs.view[v] = views[v];
+	}
+	cudaSetDevice(ctx->device);
+	cudaStream_t st = ctx->stream;
+	const uint32_t blocks = m->info.block_count;
+	const size_t stride = blocks ? blocks : 1;
+	VXB_CUDA(ctx, lists.cmd.ensure(stride * viewCount)); VXB_CUDA(ctx, lists.info.ensure(stride * viewCount));
+	VXB_CUDA(ctx, lists.tcmd.ensure(stride * viewCount * 6)); VXB_CUDA(ctx, lists.tinfo.ensure(stride * viewCount * 6));
+	VXB_CUDA(ctx, lists.counts.ensure(2 * VXB_VIEWS_MAX));
+	VXB_CUDA(ctx, cudaMemsetAsync(lists.counts.p, 0, sizeof(unsigned int) * 2 * VXB_VIEWS_MAX, st));
+	VxbDev d;
+	memset(&d, 0, sizeof(d));
+	d.n = (int)m->n; d.levels = (int)m->info.levels; d.lastLevel = d.levels - 1;
+	d.records = m->dir.p;
+	for (int l = 0; l < VXB_MAX_LEVELS; ++l) d.idBase[l] = m->bounds.level_base[l];
+	VxbLodArgs a;
+	for (int k = 0; k < 3; ++k) a.camera[k] = camera[k];
+	a.lod = lod;
+	a.counts = lists.counts.p;
+	a.regular = lists.cmd.p; a.regularInfo = lists.info.p; a.transition = lists.tcmd.p; a.transitionInfo = lists.tinfo.p;
+	a.capacity = (unsigned)(stride * 6);
+	if (blocks) vxb_lod_select_views_kernel<Cut><<<(blocks + 255) / 256, 256, 0, st>>>(d, a, blocks, vs, viewCount, m->boxes.p, (unsigned)stride);
+	unsigned n[2 * VXB_VIEWS_MAX];
+	VXB_CUDA(ctx, cudaMemcpyAsync(n, lists.counts.p, sizeof(n), cudaMemcpyDeviceToHost, st));
+	VXB_CUDA(ctx, cudaStreamSynchronize(st));
+	VXB_CUDA(ctx, cudaGetLastError());
+	for (uint32_t v = 0; v < viewCount; ++v)
+	{
+		vxb_draw_lists& l = out[v];
+		l.regular_count = n[2 * v]; l.transition_count = n[2 * v + 1];
+		l.counts = lists.counts.p + 2 * v;
+		l.regular = lists.cmd.p + stride * v; l.regular_info = lists.info.p + stride * v;
+		l.transition = lists.tcmd.p + stride * v * 6; l.transition_info = lists.tinfo.p + stride * v * 6;
+	}
+	return VXB_OK;
 }
 }
 
@@ -2536,6 +2599,7 @@ int vxb_mesh_apply(vxb_mesh* m)
 	m->bounds.boxes = reinterpret_cast<const float*>(m->boxes.p);
 	for (int l = 0; l < VXB_MAX_LEVELS; ++l) m->bounds.level_base[l] = g.levelBase[l];
 	m->bounds.slots = (uint32_t)slots;
+	m->complete = ctx->resultComplete && (!region || m->complete);
 	m->content = true;
 	m->serial = ctx->runSerial;
 	m->n = n;
@@ -2627,52 +2691,24 @@ int vxb_mesh_select_lod_views(vxb_mesh* m, const float camera[3], float baseDist
 	if (!camera || !views || !out) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_select_lod_views: NULL lod_camera, views or out");
 	if (viewCount == 0 || viewCount > VXB_VIEWS_MAX) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_select_lod_views: view_count must be in [1, 8]");
 	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_select_lod_views: nothing applied yet");
-	VxbViews vs;
-	memset(&vs, 0, sizeof(vs));
-	for (uint32_t v = 0; v < viewCount; ++v)
-	{
-		for (int k = 0; k < 6; ++k)
-			for (int c = 0; c < 4; ++c)
-				if (!std::isfinite(views[v].planes[k][c]))
-				{
-					char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_select_lod_views: view %u plane %d: non-finite component", v, k);
-					return fail(ctx, VXB_ERR_ARGUMENT, buf);
-				}
-		vs.view[v] = views[v];
-	}
-	cudaSetDevice(ctx->device);
-	cudaStream_t st = ctx->stream;
-	const uint32_t blocks = m->info.block_count;
-	const size_t stride = blocks ? blocks : 1;
-	VXB_CUDA(ctx, m->viewCmd.ensure(stride * viewCount)); VXB_CUDA(ctx, m->viewInfo.ensure(stride * viewCount));
-	VXB_CUDA(ctx, m->viewTCmd.ensure(stride * viewCount * 6)); VXB_CUDA(ctx, m->viewTInfo.ensure(stride * viewCount * 6));
-	VXB_CUDA(ctx, m->viewCounts.ensure(2 * VXB_VIEWS_MAX));
-	VXB_CUDA(ctx, cudaMemsetAsync(m->viewCounts.p, 0, sizeof(unsigned int) * 2 * VXB_VIEWS_MAX, st));
-	VxbDev d;
-	memset(&d, 0, sizeof(d));
-	d.n = (int)m->n; d.levels = (int)m->info.levels; d.lastLevel = d.levels - 1;
-	d.records = m->dir.p;
-	for (int l = 0; l < VXB_MAX_LEVELS; ++l) d.idBase[l] = m->bounds.level_base[l];
-	VxbLodArgs a;
-	for (int k = 0; k < 3; ++k) a.camera[k] = camera[k];
-	a.baseDistance = baseDistance;
-	a.counts = m->viewCounts.p;
-	a.regular = m->viewCmd.p; a.regularInfo = m->viewInfo.p; a.transition = m->viewTCmd.p; a.transitionInfo = m->viewTInfo.p;
-	a.capacity = (unsigned)(stride * 6);
-	if (blocks) vxb_lod_select_views_kernel<<<(blocks + 255) / 256, 256, 0, st>>>(d, a, blocks, vs, viewCount, m->boxes.p, (unsigned)stride);
-	unsigned n[2 * VXB_VIEWS_MAX];
-	VXB_CUDA(ctx, cudaMemcpyAsync(n, m->viewCounts.p, sizeof(n), cudaMemcpyDeviceToHost, st));
-	VXB_CUDA(ctx, cudaStreamSynchronize(st));
-	VXB_CUDA(ctx, cudaGetLastError());
-	for (uint32_t v = 0; v < viewCount; ++v)
-	{
-		vxb_draw_lists& l = out[v];
-		l.regular_count = n[2 * v]; l.transition_count = n[2 * v + 1];
-		l.counts = m->viewCounts.p + 2 * v;
-		l.regular = m->viewCmd.p + stride * v; l.regular_info = m->viewInfo.p + stride * v;
-		l.transition = m->viewTCmd.p + stride * v * 6; l.transition_info = m->viewTInfo.p + stride * v * 6;
-	}
-	return VXB_OK;
+	return selectViews<VxbCentreCut>(m, "vxb_mesh_select_lod_views", camera, baseDistance, views, viewCount, m->viewLists, out);
+}
+
+int vxb_mesh_select_cut(vxb_mesh* m, const float camera[3], float lodFactor, const vxb_view* views, uint32_t viewCount, vxb_draw_lists* out)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!camera || !views || !out) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_select_cut: NULL lod_camera, views or out");
+	if (viewCount == 0 || viewCount > VXB_VIEWS_MAX) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_select_cut: view_count must be in [1, 8]");
+	if (!std::isfinite(lodFactor) || !(lodFactor >= VXB_LOD_FACTOR_MIN))
+		return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_select_cut: lod_factor must be finite and >= 2");
+	if (!std::isfinite(camera[0]) || !std::isfinite(camera[1]) || !std::isfinite(camera[2]))
+		return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_select_cut: non-finite lod_camera component");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_select_cut: nothing applied yet");
+	if (!m->complete)
+		return fail(ctx, VXB_ERR_STATE, "vxb_mesh_select_cut: the mesh lacks levels or transition meshes (a run since the last full "
+			"apply had max_levels below the grid's levels or VXB_FLAG_NO_TRANSITIONS)");
+	return selectViews<VxbBoxCut>(m, "vxb_mesh_select_cut", camera, lodFactor, views, viewCount, m->cutLists, out);
 }
 
 int vxb_mesh_raycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits)

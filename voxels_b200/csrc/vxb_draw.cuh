@@ -10,7 +10,7 @@
 struct VxbLodArgs
 {
 	float camera[3];      // output (Y-up) coordinates, like the vertices
-	float baseDistance;   // a node of level l is fine enough when the camera is farther than baseDistance * 2^l from its centre
+	float lod;            // the cut's parameter: base_distance (VxbCentreCut) or lod_factor (VxbBoxCut)
 	unsigned int* counts; // [0] regular draws, [1] transition draws
 	vxb_draw_command* regular; vxb_draw_info* regularInfo;
 	vxb_draw_command* transition; vxb_draw_info* transitionInfo;
@@ -26,7 +26,7 @@ __device__ __forceinline__ bool vxb_lod_stops(const VxbDev& d, const VxbLodArgs&
 	const float cx = ((float)bx + 0.5f) * m, cy = ((float)bz + 0.5f) * m, cz = ((float)by + 0.5f) * m;
 	const float dx = cx - a.camera[0], dy = cy - a.camera[1], dz = cz - a.camera[2];
 	const float dist2 = (dx * dx + dy * dy) + dz * dz;
-	const float lim = a.baseDistance * (float)(1 << level);
+	const float lim = a.lod * (float)(1 << level);
 	return dist2 >= lim * lim;
 }
 
@@ -126,8 +126,63 @@ __device__ __forceinline__ bool vxb_view_sees(const vxb_view& v, const float4& l
 	return in;
 }
 
-// one thread per directory slot; view v appends to counts[2v], counts[2v + 1] and to its `stride` (regular) / 6 * stride
-// (transition) entries of a's lists
+// The two cut rules the views kernel is instantiated with: whether a block is on the cut, and its block_adj.
+// VxbCentreCut: vxb_mesh_select_lod's (centre distance against a.lod = base_distance * 2^l, the top level always stops).
+struct VxbCentreCut
+{
+	static __device__ __forceinline__ bool on_cut(const VxbDev& d, const VxbLodArgs& a, int level, int, int bx, int by, int bz)
+	{
+		return vxb_lod_selected(d, a, level, bx, by, bz);
+	}
+	static __device__ __forceinline__ unsigned block_adj(const VxbDev& d, const VxbLodArgs& a, int level, int nb, int bx, int by, int bz)
+	{
+		return vxb_lod_block_adj(d, a, level, nb, bx, by, bz);
+	}
+};
+
+// VxbBoxCut: vxb_mesh_select_cut's (include/vxb200.h "the LOD cut"): a node is refined while the camera is closer than
+// a.lod = lod_factor times its edge to its lattice box.  Refinement is monotone up the octree and the cut is balanced (the
+// header's two arguments), so the cut test and block_adj are O(1): no walk over the ancestors.
+struct VxbBoxCut
+{
+	// refine(l, b): float32 without fused multiply-add, in the header's order
+	static __device__ __forceinline__ bool refines(const VxbLodArgs& a, int level, int bx, int by, int bz)
+	{
+		if (level == 0) return false;
+		const float s = (float)(16 << level);
+		// the lattice box in output axes (x, z, y); lo and hi are exact (integers below 2^24)
+		const float lo[3] = { (float)bx * s, (float)bz * s, (float)by * s };
+		float e[3];
+		for (int i = 0; i < 3; ++i) e[i] = fmaxf(fmaxf(__fsub_rn(lo[i], a.camera[i]), __fsub_rn(a.camera[i], __fadd_rn(lo[i], s))), 0.f);
+		const float dist2 = __fadd_rn(__fadd_rn(__fmul_rn(e[0], e[0]), __fmul_rn(e[1], e[1])), __fmul_rn(e[2], e[2]));
+		const float lim = __fmul_rn(a.lod, s);
+		return dist2 < __fmul_rn(lim, lim);
+	}
+	static __device__ __forceinline__ bool on_cut(const VxbDev& d, const VxbLodArgs& a, int level, int, int bx, int by, int bz)
+	{
+		return !refines(a, level, bx, by, bz) && (level == d.lastLevel || refines(a, level + 1, bx >> 1, by >> 1, bz >> 1));
+	}
+	// bit f (vxb_lod_block_adj's face order): the same-level neighbour across face f is inside the grid and refines
+	static __device__ __forceinline__ unsigned block_adj(const VxbDev&, const VxbLodArgs& a, int level, int nb, int bx, int by, int bz)
+	{
+		unsigned adj = 0;
+		if (level > 0)
+		{
+			const int dxyz[6][3] = { { 0, 0, -1 }, { 0, -1, 0 }, { -1, 0, 0 }, { 0, 0, 1 }, { 0, 1, 0 }, { 1, 0, 0 } };
+			for (int f = 0; f < 6; ++f)
+			{
+				const int nx = bx + dxyz[f][0], ny = by + dxyz[f][1], nz = bz + dxyz[f][2];
+				if (nx < 0 || ny < 0 || nz < 0 || nx >= nb || ny >= nb || nz >= nb) continue;
+				if (refines(a, level, nx, ny, nz)) adj |= 1u << f;
+			}
+		}
+		return adj;
+	}
+};
+
+// one thread per directory slot; the Cut rule decides the cut and block_adj, view v appends to counts[2v], counts[2v + 1]
+// and to its `stride` (regular) / 6 * stride (transition) entries of a's lists
+template <class Cut>
 __global__ void __launch_bounds__(256) vxb_lod_select_views_kernel(const VxbDev d, const VxbLodArgs a, const unsigned int blockCount,
 	const __grid_constant__ VxbViews views, const unsigned int viewCount, const float4* __restrict__ boxes, const unsigned int stride)
 {
@@ -136,8 +191,8 @@ __global__ void __launch_bounds__(256) vxb_lod_select_views_kernel(const VxbDev 
 	const vxb_block_record r = d.records[slot];
 	const int level = (int)r.level, nb = (d.n >> 4) >> level;
 	const int bx = r.coord_id % nb, by = (r.coord_id / nb) % nb, bz = r.coord_id / (nb * nb);
-	if (!vxb_lod_selected(d, a, level, bx, by, bz)) return;
-	const unsigned adj = vxb_lod_block_adj(d, a, level, nb, bx, by, bz);
+	if (!Cut::on_cut(d, a, level, nb, bx, by, bz)) return;
+	const unsigned adj = Cut::block_adj(d, a, level, nb, bx, by, bz);
 	const float4 lo = boxes[2 * (size_t)(d.idBase[level] + r.coord_id)], hi = boxes[2 * (size_t)(d.idBase[level] + r.coord_id) + 1];
 	for (unsigned v = 0; v < viewCount; ++v)
 	{
