@@ -655,6 +655,96 @@ int vxb_mesh_closest_point(vxb_mesh* mesh, float max_distance, const float* poin
 int vxb_mesh_sphere_cast_device(vxb_mesh* mesh, float radius, const vxb_ray* rays, uint32_t count, vxb_sphere_hit* hits);
 int vxb_mesh_closest_point_device(vxb_mesh* mesh, float max_distance, const float* points, uint32_t count, vxb_closest_hit* hits);
 
+/* ---- capsule queries against the mesh: capsule sweeps and closest points to segments, for capsule character controllers ---
+ * A capsule is the segment [c - h, c + h] (c = centre, h = half axis: any direction, zero allowed) with a radius r.  Like the
+ * collision queries above: LEVEL-0 regular triangles only, both faces, OUTPUT (Y-up) coordinates, a pure function of the mesh
+ * and the query, float32 with no fused multiply-add in exactly the order written here, the same dot and cross products, and
+ * the same tie rule (least t or dd, then the lower slot, then the lower triangle).
+ *   Closest pair of the segment (c, h) and triangle (a, b, c_) - one routine for both queries and the sweep's start test.
+ *     p0_i = c_i - h_i; p1_i = c_i + h_i; D_i = h_i + h_i.  Candidates, in this order, each a triangle point `point` with
+ *     barycentrics (u, v), a segment parameter w in [0, 1] and a dd:
+ *       1  p0: the closest point of the triangle to p0 (the collision queries' routine), dd = |p0 - point|^2, w = 0
+ *       2  p1: the same for p1, w = 1
+ *       3  the edges ab, bc, ca in turn (Ericson's ClosestPtSegmentSegment, exact zero tests for his epsilons), for the edge
+ *          q0 -> q1: E = q1 - q0; R = p0 - q0; A = D.D; e = E.E; f = E.R.  A == 0: no candidate (1 gives the distance).
+ *          Otherwise c = D.R and, if e == 0: t = 0, w = clamp(-c / A); else b = D.E; den = A*e - b*b;
+ *          w = den != 0 ? clamp((b*f - c*e) / den) : 0; t = (b*w + f) / e; t < 0: t = 0, w = clamp(-c / A);
+ *          else t > 1: t = 1, w = clamp((b - c) / A).  clamp(x) = x < 0 ? 0 : (x > 1 ? 1 : x).
+ *          X_i = p0_i + w*D_i; point_i = q0_i + t*E_i; dd = |X - point|^2; (u, v) = (t, 0) on ab, (1 - t, t) on bc, (0, 1 - t)
+ *          on ca.
+ *       4  the segment crossing the triangle: Moeller-Trumbore of the ray queries from p0 along D (s = p0 - a, e1 = b - a,
+ *          e2 = c_ - a), giving det, u, v and w, accepted iff det != 0 && u >= 0 && u <= 1 && v >= 0 && u + v <= 1 && w >= 0
+ *          && w <= 1; dd = 0, point_i = (a_i + e1_i*u) + e2_i*v.
+ *     The result is the candidate with the least dd, the first in this order on a tie; s = (w + w) - 1 and
+ *     axis_point_i = c_i + s*h_i.  With h = 0 only candidates 1 and 2 exist and agree, so the result is the collision
+ *     queries' closest point bit for bit (s = -1).
+ *
+ *   vxb_mesh_closest_to_segment: every triangle whose dd is at most max_distance*max_distance (in float) is a candidate; the
+ *     result is the least dd by the tie rule, distance = sqrt(dd).  The penetration depth of a capsule is r - distance.
+ *
+ *   vxb_mesh_capsule_cast: the capsule's centre moves along the path (a vxb_ray, the same rules), its half axis and radius fixed.
+ *     It touches triangle T when the sphere of radius r at the centre touches P = T + [-h, h] (Minkowski sum).  With
+ *     c0_i = o_i + t_min*d_i:
+ *       started in contact   the closest pair at c0 has dd <= r*r: t = t_min, flags = VXB_SPHERE_STARTED_IN_CONTACT.
+ *       otherwise            the least t of these tests, each the sphere sweep's formula (and +inf when it fails):
+ *         faces     the caps (a - h, b - h, c_ - h) and (a + h, b + h, c_ + h), then the parallelograms of ab, bc, ca:
+ *                   for the edge q0 -> q1 the sphere's face test on the vertices (q0 - h, q1 - h, q0 + h), with u <= 1 and
+ *                   v <= 1 in place of u + v <= 1 (the parallelogram q0 - h, q1 - h, q1 + h, q0 + h).
+ *         edges     the cap edges ab, bc, ca of the cap -h, the same of the cap +h, then the lateral edges a - h -> a + h,
+ *                   b - h -> b + h, c_ - h -> c_ + h.
+ *         vertices  a - h, b - h, c_ - h, a + h, b + h, c_ + h.
+ *       (shifted points per component: q_i - h_i, q_i + h_i).  Every feature lies in P, so no test fires before the first
+ *       contact; the faces cover P, so the first contact is on one of them or on their edges and vertices.  With h = 0 the
+ *       t is the sphere sweep's bit for bit: the parallelograms and lateral edges fail through det = 0 and A = 0.
+ *     The hit: t, center_i = o_i + t*d_i, and point, axis_point, u, v and s of the closest pair at that centre; normal as for
+ *     the closest point.  Ties of several triangles as for the sphere sweep.
+ * A miss: slot = VXB_RAY_MISS, t (distance) = +inf, every other field zero.
+ * Reach: a sweep is valid when r > 0 and max_i |h_i| + r <= VXB_SPHERE_RADIUS_MAX, a segment when max_i |h_i| +
+ * max_distance <= VXB_SPHERE_RADIUS_MAX (both sums in float); a contact puts the centre within |h_i| + r of its triangle
+ * along axis i, so every block within reach stays one of the 27 neighbours of the centre's block.  The sweep walk grows the
+ * block boxes by max_i |h_i| + r + 1/16.
+ * Refusals: VXB_ERR_STATE before the first vxb_mesh_apply; VXB_ERR_ARGUMENT for a NULL pointer with count > 0 (count = 0
+ * does nothing) and, on both variants, for a max_distance outside 0 <= m <= 15.  The HOST variants refuse a query with an
+ * invalid path (the ray rules), a non-finite half axis or radius, a shape out of reach, or a non-finite centre, naming its
+ * index in vxb_last_error and writing nothing to `hits`; the DEVICE variants return a miss for it. */
+typedef struct vxb_capsule_sweep
+{
+	vxb_ray path;           /* the centre's path */
+	float half_axis[3];     /* h: the segment is centre -+ h */
+	float radius;           /* r > 0 */
+} vxb_capsule_sweep;                                                                                         /* 48 bytes */
+typedef struct vxb_segment { float center[3]; float half_axis[3]; } vxb_segment;                           /* 24 bytes */
+typedef struct vxb_capsule_hit
+{
+	float t;                /* centre = origin + t * direction at the first contact */
+	uint32_t slot;          /* as vxb_ray_hit; VXB_RAY_MISS */
+	uint32_t block_id;
+	uint32_t triangle;
+	float center[3];        /* path.origin + t * path.direction */
+	float point[3];         /* the contact point on the triangle */
+	float axis_point[3];    /* the point of the capsule's segment paired with it: center + s * half_axis */
+	float normal[3];        /* the vertex normals blended at (u, v), the ray hit's formula */
+	float u, v, s;          /* barycentrics of `point`; s in [-1, 1] */
+	uint32_t flags;         /* VXB_SPHERE_STARTED_IN_CONTACT */
+} vxb_capsule_hit;                                                                                           /* 80 bytes */
+typedef struct vxb_segment_hit
+{
+	float distance;         /* sqrt(dd) of the closest pair; +inf on a miss */
+	uint32_t slot;          /* as vxb_ray_hit; VXB_RAY_MISS */
+	uint32_t block_id;
+	uint32_t triangle;
+	float point[3];         /* the closest point of the level-0 surface within max_distance of the segment */
+	float axis_point[3];    /* the segment's point paired with it: center + s * half_axis */
+	float normal[3];        /* the vertex normals blended at (u, v), the ray hit's formula */
+	float u, v, s;          /* barycentrics of `point`; s in [-1, 1] */
+} vxb_segment_hit;                                                                                           /* 64 bytes */
+/* HOST memory; block until the hits are written. */
+int vxb_mesh_capsule_cast(vxb_mesh* mesh, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits);
+int vxb_mesh_closest_to_segment(vxb_mesh* mesh, float max_distance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits);
+/* DEVICE memory; enqueued on vxb_stream(ctx) like vxb_mesh_raycast_device: they see the mesh as of their place in the queue. */
+int vxb_mesh_capsule_cast_device(vxb_mesh* mesh, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits);
+int vxb_mesh_closest_to_segment_device(vxb_mesh* mesh, float max_distance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits);
+
 /* GetMaterial(id) == nullptr handling (TransVoxelImpl.cpp:1364-1368: textures stay zero, one LS_Error log per
  * vertex): after vxb_result_download the material ids of those vertices, in the reference's logging order
  * (level, block, regular vertices, then transition faces), can be read here.  Returns the count; copies at

@@ -191,6 +191,36 @@ CLOSEST_HIT_DTYPE = np.dtype([("distance", "<f4"), ("slot", "<u4"), ("block_id",
                               ("normal", "<f4", 3), ("u", "<f4"), ("v", "<f4")])
 assert SPHERE_HIT_DTYPE.itemsize == 64 and CLOSEST_HIT_DTYPE.itemsize == 48
 
+# vxb_capsule_sweep / vxb_segment / vxb_capsule_hit / vxb_segment_hit (include/vxb200.h "capsule queries")
+CAPSULE_SWEEP_DTYPE = np.dtype([("path", RAY_DTYPE), ("half_axis", "<f4", 3), ("radius", "<f4")])
+SEGMENT_DTYPE = np.dtype([("center", "<f4", 3), ("half_axis", "<f4", 3)])
+CAPSULE_HIT_DTYPE = np.dtype([("t", "<f4"), ("slot", "<u4"), ("block_id", "<u4"), ("triangle", "<u4"), ("center", "<f4", 3),
+                              ("point", "<f4", 3), ("axis_point", "<f4", 3), ("normal", "<f4", 3), ("u", "<f4"), ("v", "<f4"),
+                              ("s", "<f4"), ("flags", "<u4")])
+SEGMENT_HIT_DTYPE = np.dtype([("distance", "<f4"), ("slot", "<u4"), ("block_id", "<u4"), ("triangle", "<u4"), ("point", "<f4", 3),
+                              ("axis_point", "<f4", 3), ("normal", "<f4", 3), ("u", "<f4"), ("v", "<f4"), ("s", "<f4")])
+assert CAPSULE_SWEEP_DTYPE.itemsize == 48 and SEGMENT_DTYPE.itemsize == 24
+assert CAPSULE_HIT_DTYPE.itemsize == 80 and SEGMENT_HIT_DTYPE.itemsize == 64
+
+
+def make_capsule_sweeps(origins, directions, half_axes, radius, t_min=0.0, t_max=np.inf):
+    """A CAPSULE_SWEEP_DTYPE array: the centre paths as make_rays, `half_axes` [count, 3] or [3], `radius` a scalar or [count]."""
+    rays = make_rays(origins, directions, t_min, t_max)
+    sweeps = np.zeros(len(rays), CAPSULE_SWEEP_DTYPE)
+    sweeps["path"] = rays
+    sweeps["half_axis"] = np.broadcast_to(np.asarray(half_axes, np.float32), (len(rays), 3))
+    sweeps["radius"] = np.float32(radius) if np.isscalar(radius) else np.asarray(radius, np.float32)
+    return sweeps
+
+
+def make_segments(centers, half_axes):
+    """A SEGMENT_DTYPE array from [count, 3] centres and [count, 3] (or [3]) half axes."""
+    c = np.asarray(centers, np.float32).reshape(-1, 3)
+    segs = np.zeros(len(c), SEGMENT_DTYPE)
+    segs["center"] = c
+    segs["half_axis"] = np.broadcast_to(np.asarray(half_axes, np.float32), (len(c), 3))
+    return segs
+
 
 class MeshInfo(C.Structure):
     """vxb_mesh_info (include/vxb200.h)."""
@@ -335,6 +365,10 @@ def load_library():
         "vxb_mesh_sphere_cast_device": (C.c_int, [vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_closest_point": (C.c_int, [vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_closest_point_device": (C.c_int, [vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_capsule_cast": (C.c_int, [vp, vp, u32, vp]),
+        "vxb_mesh_capsule_cast_device": (C.c_int, [vp, vp, u32, vp]),
+        "vxb_mesh_closest_to_segment": (C.c_int, [vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_closest_to_segment_device": (C.c_int, [vp, C.c_float, vp, u32, vp]),
         "vxb_host_alloc": (vp, [C.c_size_t]),
         "vxb_host_free": (None, [vp]),
     }
@@ -357,7 +391,9 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_mesh_create", "vxb_mesh_destroy", "vxb_mesh_apply", "vxb_mesh_info_get", "vxb_mesh_download",
                     "vxb_mesh_device_arenas", "vxb_mesh_select_lod", "vxb_mesh_bounds_get", "vxb_mesh_download_bounds",
                     "vxb_mesh_select_lod_views", "vxb_mesh_select_cut", "vxb_mesh_raycast", "vxb_mesh_raycast_device",
-                    "vxb_mesh_sphere_cast", "vxb_mesh_sphere_cast_device", "vxb_mesh_closest_point", "vxb_mesh_closest_point_device"]
+                    "vxb_mesh_sphere_cast", "vxb_mesh_sphere_cast_device", "vxb_mesh_closest_point", "vxb_mesh_closest_point_device",
+                    "vxb_mesh_capsule_cast", "vxb_mesh_capsule_cast_device", "vxb_mesh_closest_to_segment",
+                    "vxb_mesh_closest_to_segment_device"]
 
 
 def nccl_unique_id():
@@ -625,6 +661,51 @@ class Mesh:
         self.ctx._check(self.L.vxb_mesh_closest_point_device(self.h, max_distance, None if points_ptr is None else C.c_void_p(points_ptr),
                                                              count, None if hits_ptr is None else C.c_void_p(hits_ptr)),
                         "vxb_mesh_closest_point_device")
+
+    def capsule_cast_rc(self, sweeps, hits=None, count=None):
+        """vxb_mesh_capsule_cast's return code for a CAPSULE_SWEEP_DTYPE array (or None for a NULL pointer); the hits go to
+        `hits` (a CAPSULE_HIT_DTYPE array, or None for a NULL pointer); `count` defaults to len(sweeps)."""
+        sweeps = np.ascontiguousarray(sweeps, CAPSULE_SWEEP_DTYPE) if sweeps is not None else None
+        n = (0 if sweeps is None else len(sweeps)) if count is None else count
+        return self.L.vxb_mesh_capsule_cast(self.h, _ptr(sweeps), n, _ptr(hits))
+
+    def capsule_cast(self, sweeps):
+        """Sweeps capsules against the mesh's level-0 triangles (vxb_mesh_capsule_cast): `sweeps` is a CAPSULE_SWEEP_DTYPE
+        array (make_capsule_sweeps), OUTPUT (Y-up) coordinates.  Returns a CAPSULE_HIT_DTYPE array."""
+        sweeps = np.ascontiguousarray(sweeps, CAPSULE_SWEEP_DTYPE)
+        hits = np.zeros(len(sweeps), CAPSULE_HIT_DTYPE)
+        self.ctx._check(self.L.vxb_mesh_capsule_cast(self.h, _ptr(sweeps), len(sweeps), _ptr(hits)), "vxb_mesh_capsule_cast")
+        return hits
+
+    def capsule_cast_device(self, sweeps_ptr, count, hits_ptr):
+        """vxb_mesh_capsule_cast_device: `count` vxb_capsule_sweep at the device address `sweeps_ptr`, hits to `hits_ptr`;
+        enqueued on the context's stream, returns without waiting."""
+        self.ctx._check(self.L.vxb_mesh_capsule_cast_device(self.h, None if sweeps_ptr is None else C.c_void_p(sweeps_ptr), count,
+                                                            None if hits_ptr is None else C.c_void_p(hits_ptr)), "vxb_mesh_capsule_cast_device")
+
+    def closest_to_segment_rc(self, max_distance, segments, hits=None, count=None):
+        """vxb_mesh_closest_to_segment's return code for a SEGMENT_DTYPE array (or None for a NULL pointer); the hits go to
+        `hits` (a SEGMENT_HIT_DTYPE array, or None for a NULL pointer); `count` defaults to len(segments)."""
+        segments = np.ascontiguousarray(segments, SEGMENT_DTYPE) if segments is not None else None
+        n = (0 if segments is None else len(segments)) if count is None else count
+        return self.L.vxb_mesh_closest_to_segment(self.h, max_distance, _ptr(segments), n, _ptr(hits))
+
+    def closest_to_segment(self, segments, max_distance):
+        """The nearest level-0 surface point within `max_distance` voxels of each segment (a SEGMENT_DTYPE array, make_segments;
+        OUTPUT, Y-up coordinates), vxb_mesh_closest_to_segment.  Returns a SEGMENT_HIT_DTYPE array."""
+        segments = np.ascontiguousarray(segments, SEGMENT_DTYPE)
+        hits = np.zeros(len(segments), SEGMENT_HIT_DTYPE)
+        self.ctx._check(self.L.vxb_mesh_closest_to_segment(self.h, max_distance, _ptr(segments), len(segments), _ptr(hits)),
+                        "vxb_mesh_closest_to_segment")
+        return hits
+
+    def closest_to_segment_device(self, max_distance, segments_ptr, count, hits_ptr):
+        """vxb_mesh_closest_to_segment_device: `count` vxb_segment at the device address `segments_ptr`, hits to `hits_ptr`;
+        enqueued on the context's stream, returns without waiting."""
+        self.ctx._check(self.L.vxb_mesh_closest_to_segment_device(self.h, max_distance,
+                                                                  None if segments_ptr is None else C.c_void_p(segments_ptr), count,
+                                                                  None if hits_ptr is None else C.c_void_p(hits_ptr)),
+                        "vxb_mesh_closest_to_segment_device")
 
 
 class Context:

@@ -39,6 +39,8 @@ static_assert(sizeof(VxbVertex) == 48, "PolygonVertex layout");
 static_assert(sizeof(vxb_block_record) == 128, "record layout");
 static_assert(sizeof(vxb_ray) == 32 && sizeof(vxb_ray_hit) == 48, "ray layouts");
 static_assert(sizeof(vxb_sphere_hit) == 64 && sizeof(vxb_closest_hit) == 48, "collision layouts");
+static_assert(sizeof(vxb_capsule_sweep) == 48 && sizeof(vxb_segment) == 24 && sizeof(vxb_capsule_hit) == 80 && sizeof(vxb_segment_hit) == 64,
+	"capsule layouts");
 static_assert(sizeof(vxb_view) == 96 && sizeof(vxb_mesh_bounds) == 64 && VXB_MAX_LEVELS == 12, "view and bounds layouts");
 
 namespace
@@ -2223,6 +2225,10 @@ struct vxb_mesh
 	DevBuf<vxb_sphere_hit> sphereOut;
 	DevBuf<float> pointIn;                      // 3 floats per closest-point query
 	DevBuf<vxb_closest_hit> closestOut;
+	DevBuf<vxb_capsule_sweep> capsuleIn;
+	DevBuf<vxb_capsule_hit> capsuleOut;
+	DevBuf<vxb_segment> segmentIn;
+	DevBuf<vxb_segment_hit> segmentOut;
 };
 
 namespace
@@ -2295,6 +2301,36 @@ int enqueueClosestPoint(vxb_mesh* m, float maxDistance, const float* points, uin
 	vxb_closest_point_kernel<<<queryCtas(m->ctx, count, VXB_COLLIDE_THREADS), VXB_COLLIDE_THREADS, 0, m->ctx->stream>>>(rm, maxDistance, points, count, hits);
 	VXB_CUDA(m->ctx, cudaGetLastError());
 	return VXB_OK;
+}
+
+int enqueueCapsuleCast(vxb_mesh* m, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits)
+{
+	VxbRayMesh rm;
+	const int e = ensureMap(m, rm);
+	if (e != VXB_OK) return e;
+	vxb_capsule_cast_kernel<<<queryCtas(m->ctx, count, VXB_COLLIDE_THREADS), VXB_COLLIDE_THREADS, 0, m->ctx->stream>>>(rm, sweeps, count, hits);
+	VXB_CUDA(m->ctx, cudaGetLastError());
+	return VXB_OK;
+}
+
+int enqueueClosestSegment(vxb_mesh* m, float maxDistance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits)
+{
+	VxbRayMesh rm;
+	const int e = ensureMap(m, rm);
+	if (e != VXB_OK) return e;
+	vxb_closest_segment_kernel<<<queryCtas(m->ctx, count, VXB_COLLIDE_THREADS), VXB_COLLIDE_THREADS, 0, m->ctx->stream>>>(rm, maxDistance, segments, count, hits);
+	VXB_CUDA(m->ctx, cudaGetLastError());
+	return VXB_OK;
+}
+
+// the reach rule of the capsule queries (include/vxb200.h), in float as the kernels evaluate it: a finite half axis and
+// max_i |h_i| + extra <= 15
+bool capsuleReach(const float h[3], float extra)
+{
+	if (!std::isfinite(h[0]) || !std::isfinite(h[1]) || !std::isfinite(h[2])) return false;
+	const float hm = std::max(std::max(std::fabs(h[0]), std::fabs(h[1])), std::fabs(h[2]));
+	const float reach = hm + extra;
+	return reach <= VXB_SPHERE_RADIUS_MAX;
 }
 
 // the batch arguments of the collision queries (include/vxb200.h): 0 < radius <= 15, 0 <= max_distance <= 15; NaN fails
@@ -2799,6 +2835,77 @@ int vxb_mesh_closest_point_device(vxb_mesh* m, float maxDistance, const float* p
 	if (!count) return VXB_OK;
 	cudaSetDevice(ctx->device);
 	return enqueueClosestPoint(m, maxDistance, points, count, hits);
+}
+
+int vxb_mesh_capsule_cast(vxb_mesh* m, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (count && (!sweeps || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_capsule_cast: NULL sweeps or hits");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_capsule_cast: nothing applied yet");
+	if (!count) return VXB_OK;
+	for (uint32_t q = 0; q < count; ++q)
+	{
+		const char* why = nullptr;
+		const float r = sweeps[q].radius;
+		invalidRay(&sweeps[q].path, 1, &why);
+		if (!why && !(r > 0.f)) why = "radius must be > 0";
+		if (!why && !capsuleReach(sweeps[q].half_axis, r)) why = "non-finite half axis or radius, or max |half_axis| + radius above 15";
+		if (why)
+		{
+			char buf[192]; snprintf(buf, sizeof(buf), "vxb_mesh_capsule_cast: sweep %u: %s", q, why);
+			return fail(ctx, VXB_ERR_ARGUMENT, buf);
+		}
+	}
+	return hostQuery(m, m->capsuleIn, 1, m->capsuleOut, sweeps, count, hits,
+		[&](const vxb_capsule_sweep* in, vxb_capsule_hit* out) { return enqueueCapsuleCast(m, in, count, out); });
+}
+
+int vxb_mesh_capsule_cast_device(vxb_mesh* m, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (count && (!sweeps || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_capsule_cast_device: NULL sweeps or hits");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_capsule_cast_device: nothing applied yet");
+	if (!count) return VXB_OK;
+	cudaSetDevice(ctx->device);
+	return enqueueCapsuleCast(m, sweeps, count, hits);
+}
+
+int vxb_mesh_closest_to_segment(vxb_mesh* m, float maxDistance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!validMaxDistance(maxDistance)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_to_segment: max_distance must be in [0, 15]");
+	if (count && (!segments || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_to_segment: NULL segments or hits");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_closest_to_segment: nothing applied yet");
+	if (!count) return VXB_OK;
+	for (uint32_t q = 0; q < count; ++q)
+	{
+		const char* why = nullptr;
+		const float* c = segments[q].center;
+		if (!std::isfinite(c[0]) || !std::isfinite(c[1]) || !std::isfinite(c[2])) why = "non-finite centre";
+		else if (!capsuleReach(segments[q].half_axis, maxDistance)) why = "non-finite half axis, or max |half_axis| + max_distance above 15";
+		if (why)
+		{
+			char buf[192]; snprintf(buf, sizeof(buf), "vxb_mesh_closest_to_segment: segment %u: %s", q, why);
+			return fail(ctx, VXB_ERR_ARGUMENT, buf);
+		}
+	}
+	return hostQuery(m, m->segmentIn, 1, m->segmentOut, segments, count, hits,
+		[&](const vxb_segment* in, vxb_segment_hit* out) { return enqueueClosestSegment(m, maxDistance, in, count, out); });
+}
+
+int vxb_mesh_closest_to_segment_device(vxb_mesh* m, float maxDistance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (!validMaxDistance(maxDistance)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_to_segment_device: max_distance must be in [0, 15]");
+	if (count && (!segments || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_to_segment_device: NULL segments or hits");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_closest_to_segment_device: nothing applied yet");
+	if (!count) return VXB_OK;
+	cudaSetDevice(ctx->device);
+	return enqueueClosestSegment(m, maxDistance, segments, count, hits);
 }
 
 } // extern "C"

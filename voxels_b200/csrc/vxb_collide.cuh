@@ -12,6 +12,8 @@
 //                   lies outside (below 0 or above n), only the first or last block of the axis is that close, and that is
 //                   the clamped index.  So the 27 neighbours of the clamped block hold every block that can contribute, for
 //                   queries inside and outside the grid box alike.
+//   capsules        the same two routes with the reach |h_i| + r (sweeps: the walk grown by max_i |h_i| + r + eps) or
+//                   |h_i| + max_distance (segments: the per-axis box gap instead of the distance); see "capsules" below.
 #pragma once
 
 #define VXB_COLLIDE_THREADS VXB_RAY_THREADS
@@ -94,18 +96,12 @@ VXB_FN float vxb_sweep_vertex(const float3 o, const float3 d, const float3 q, fl
 	return dd > 0.f && disc >= 0.f && t >= tMin && t <= tMax ? t : CUDART_INF_F;
 }
 
-// The first contact of the sphere (radius r, centre o + t d, t in [t_min, t_max]) with triangle (a, b, c), include/vxb200.h
-// "sphere sweep": +inf when there is none; `started` when the sphere touches the triangle at t_min already.  c0 = o + t_min d.
-VXB_FN float vxb_sweep_triangle(const float3 o, const float3 d, const float3 c0, float r, float rr, float dd, float tMin, float tMax,
-	const float3 a, const float3 b, const float3 c, bool& started)
+// The sweep's face test: the plane of (a, b, c) offset by r toward the side of c0, as a Moeller-Trumbore cast of the ray
+// moved by -r along that side (+inf when it fails).  Quad: the parallelogram a, b, b + c - a (v <= 1 in place of u + v <= 1).
+template <bool Quad>
+VXB_FN float vxb_sweep_face(const float3 o, const float3 d, const float3 c0, float r, float tMin, float tMax, const float3 a,
+	const float3 b, const float3 c)
 {
-	started = false;
-	{
-		float3 q; float u, v;
-		vxb_closest_on_triangle(c0, a, b, c, q, u, v);
-		if (vxb_dist2(c0, q) <= rr) { started = true; return tMin; }
-	}
-	// the face: the plane offset by r toward the side of c0, as a Moeller-Trumbore cast of the ray moved by -r along that side
 	const float e1x = b.x - a.x, e1y = b.y - a.y, e1z = b.z - a.z;
 	const float e2x = c.x - a.x, e2y = c.y - a.y, e2z = c.z - a.z;
 	const float nx = e1y * e2z - e1z * e2y, ny = e1z * e2x - e1x * e2z, nz = e1x * e2y - e1y * e2x;
@@ -120,8 +116,22 @@ VXB_FN float vxb_sweep_triangle(const float3 o, const float3 d, const float3 c0,
 	const float qvx = sy * e1z - sz * e1y, qvy = sz * e1x - sx * e1z, qvz = sx * e1y - sy * e1x;
 	const float fv = ((d.x * qvx + d.y * qvy) + d.z * qvz) * inv;
 	const float ft = ((e2x * qvx + e2y * qvy) + e2z * qvz) * inv;
-	float t = (side >= 0.f ? det > 0.f : det < 0.f) && fu >= 0.f && fu <= 1.f && fv >= 0.f && fu + fv <= 1.f && ft >= tMin &&
-		ft <= tMax ? ft : CUDART_INF_F;
+	return (side >= 0.f ? det > 0.f : det < 0.f) && fu >= 0.f && fu <= 1.f && fv >= 0.f && (Quad ? fv <= 1.f : fu + fv <= 1.f) &&
+		ft >= tMin && ft <= tMax ? ft : CUDART_INF_F;
+}
+
+// The first contact of the sphere (radius r, centre o + t d, t in [t_min, t_max]) with triangle (a, b, c), include/vxb200.h
+// "sphere sweep": +inf when there is none; `started` when the sphere touches the triangle at t_min already.  c0 = o + t_min d.
+VXB_FN float vxb_sweep_triangle(const float3 o, const float3 d, const float3 c0, float r, float rr, float dd, float tMin, float tMax,
+	const float3 a, const float3 b, const float3 c, bool& started)
+{
+	started = false;
+	{
+		float3 q; float u, v;
+		vxb_closest_on_triangle(c0, a, b, c, q, u, v);
+		if (vxb_dist2(c0, q) <= rr) { started = true; return tMin; }
+	}
+	float t = vxb_sweep_face<false>(o, d, c0, r, tMin, tMax, a, b, c);
 	// the edges ab, bc, ca, then the vertices a, b, c
 	t = fminf(t, vxb_sweep_edge(o, d, a, b, rr, tMin, tMax));
 	t = fminf(t, vxb_sweep_edge(o, d, b, c, rr, tMin, tMax));
@@ -259,6 +269,317 @@ __global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_closest_point_kernel(
 				vxb_ray_blend_normal(m, bs, bk, bu, bv, h.normal);
 			}
 			hits[q] = h;
+		}
+	}
+}
+
+// ---- capsules (include/vxb200.h "capsule queries") ---------------------------------------------------------------------
+//
+// A capsule (segment c -+ h, radius r) touches triangle T exactly when the sphere of radius r at c touches the convex set
+// P = T + [-h, h].  The sweep runs the sphere's tests on P's features:
+//   no early contact   every face, edge and vertex tested lies in P, and each accepted test puts the centre within r (up to
+//                      rounding) of a point of its feature, so no test fires before the first contact with P.
+//   the faces cover P  take z = y + x h in P (y in T, |x| <= 1) and the parameters {s : z + s h in T} = [s0, s1], which hold
+//                      -x.  If -1 or 1 is in it, z lies in the cap T + h or T - h; otherwise [s0, s1] lies inside (-1, 1),
+//                      z + s0 h is on an edge of T and z lies in that edge's parallelogram.  This holds for any h, also
+//                      one in T's plane, where P is flat.
+//   first contact      at the first contact t*, the point z of P nearest the centre lies on a face F of that cover.  If the
+//                      centre - z is normal to F, it is r from F's plane on the side the centre is on; that signed distance
+//                      is affine in t and has not yet risen to r at t* from above, so c0 is on the same side: F's offset-
+//                      plane test (side from c0) accepts t*.  Otherwise z is on F's boundary, an edge of T +- h or a lateral
+//                      edge, and the cylinder test of that edge (or, at an end of it, the sphere test of the vertex) accepts
+//                      t*.  A path parallel to F at distance r first touches F's boundary, so it is the same case.
+// With h = 0 the caps are T, the parallelograms and the lateral edges have zero extent and fail (det = 0, A = 0), and the cap
+// edges and shifted vertices are the sphere's: the contact t is the sphere sweep's.
+//
+// The per-triangle reject.  A contact puts the centre within |h_i| + r of its triangle along axis i (the capsule point paired
+// with the contact is within r, and it is within |h_i| of the centre), so inside the triangle's box grown by g_i = |h_i| + r +
+// VXB_RAY_EPS.  The reject runs the walk's slab test on that box: a triangle whose grown box the path misses has no contact,
+// by the walk's argument at the top of vxb_ray.cuh (rounded planes and slab parameters stay far inside the eps slack).  The
+// closest-to-segment query rejects a triangle (and skips a block) whose box is farther than |h_i| + max_distance + eps from
+// the centre along some axis, for the same reason.  The reject never changes a result; it only avoids the full tests.
+
+VXB_FN float vxb_clamp01(float x) { return x < 0.f ? 0.f : (x > 1.f ? 1.f : x); }
+
+// Candidate 3 of the closest pair for the edge q0 -> q1 (Ericson's ClosestPtSegmentSegment, exact zero tests): dd (+inf when
+// the segment has zero length), the edge point y at parameter t, and the segment parameter w.  p0, D: the segment p0 + w D;
+// A = D.D.
+VXB_FN float vxb_segment_edge(const float3 p0, const float3 D, float A, const float3 q0, const float3 q1, float3& y, float& t, float& w)
+{
+	t = 0.f; w = 0.f; y = q0;
+	if (A == 0.f) return CUDART_INF_F;
+	const float ex = q1.x - q0.x, ey = q1.y - q0.y, ez = q1.z - q0.z;
+	const float rx = p0.x - q0.x, ry = p0.y - q0.y, rz = p0.z - q0.z;
+	const float e = (ex * ex + ey * ey) + ez * ez;
+	const float f = (ex * rx + ey * ry) + ez * rz;
+	const float c = (D.x * rx + D.y * ry) + D.z * rz;
+	if (e == 0.f) w = vxb_clamp01(VXB_DIV(-c, A));
+	else
+	{
+		const float b = (D.x * ex + D.y * ey) + D.z * ez;
+		const float den = A * e - b * b;
+		w = den != 0.f ? vxb_clamp01(VXB_DIV(b * f - c * e, den)) : 0.f;
+		t = VXB_DIV(b * w + f, e);
+		if (t < 0.f) { t = 0.f; w = vxb_clamp01(VXB_DIV(-c, A)); }
+		else if (t > 1.f) { t = 1.f; w = vxb_clamp01(VXB_DIV(b - c, A)); }
+	}
+	y = make_float3(q0.x + t * ex, q0.y + t * ey, q0.z + t * ez);
+	return vxb_dist2(make_float3(p0.x + w * D.x, p0.y + w * D.y, p0.z + w * D.z), y);
+}
+
+// The closest pair of the segment ctr -+ h and triangle (a, b, c) in the order include/vxb200.h states: dd, the triangle point
+// q with barycentrics (u, v), and the segment parameter w in [0, 1] (s = 2w - 1).
+VXB_FN float vxb_segment_triangle(const float3 ctr, const float3 h, const float3 a, const float3 b, const float3 c, float3& q, float& u,
+	float& v, float& w)
+{
+	const float3 p0 = make_float3(ctr.x - h.x, ctr.y - h.y, ctr.z - h.z);
+	const float3 D = make_float3(h.x + h.x, h.y + h.y, h.z + h.z);
+	vxb_closest_on_triangle(p0, a, b, c, q, u, v);
+	float best = vxb_dist2(p0, q);
+	w = 0.f;
+	{
+		const float3 p1 = make_float3(ctr.x + h.x, ctr.y + h.y, ctr.z + h.z);
+		float3 q1; float u1, v1;
+		vxb_closest_on_triangle(p1, a, b, c, q1, u1, v1);
+		const float d1 = vxb_dist2(p1, q1);
+		if (d1 < best) { best = d1; q = q1; u = u1; v = v1; w = 1.f; }
+	}
+	const float A = (D.x * D.x + D.y * D.y) + D.z * D.z;
+	float3 y; float t, we;
+	float de = vxb_segment_edge(p0, D, A, a, b, y, t, we);
+	if (de < best) { best = de; q = y; u = t; v = 0.f; w = we; }
+	de = vxb_segment_edge(p0, D, A, b, c, y, t, we);
+	if (de < best) { best = de; q = y; u = 1.f - t; v = t; w = we; }
+	de = vxb_segment_edge(p0, D, A, c, a, y, t, we);
+	if (de < best) { best = de; q = y; u = 0.f; v = 1.f - t; w = we; }
+	// the segment crossing the triangle: Moeller-Trumbore from p0 along D
+	const float e1x = b.x - a.x, e1y = b.y - a.y, e1z = b.z - a.z;
+	const float e2x = c.x - a.x, e2y = c.y - a.y, e2z = c.z - a.z;
+	const float sx = p0.x - a.x, sy = p0.y - a.y, sz = p0.z - a.z;
+	const float pvx = D.y * e2z - D.z * e2y, pvy = D.z * e2x - D.x * e2z, pvz = D.x * e2y - D.y * e2x;
+	const float det = (e1x * pvx + e1y * pvy) + e1z * pvz;
+	const float inv = VXB_DIV(1.f, det);
+	const float fu = ((sx * pvx + sy * pvy) + sz * pvz) * inv;
+	const float qvx = sy * e1z - sz * e1y, qvy = sz * e1x - sx * e1z, qvz = sx * e1y - sy * e1x;
+	const float fv = ((D.x * qvx + D.y * qvy) + D.z * qvz) * inv;
+	const float fw = ((e2x * qvx + e2y * qvy) + e2z * qvz) * inv;
+	if (det != 0.f && fu >= 0.f && fu <= 1.f && fv >= 0.f && fu + fv <= 1.f && fw >= 0.f && fw <= 1.f && 0.f < best)
+	{
+		best = 0.f; u = fu; v = fv; w = fw;
+		q = make_float3((a.x + e1x * fu) + e2x * fv, (a.y + e1y * fu) + e2y * fv, (a.z + e1z * fu) + e2z * fv);
+	}
+	return best;
+}
+
+// The first contact of the capsule (half axis h, radius r, centre o + t d, t in [t_min, t_max]) with triangle (a, b, c),
+// include/vxb200.h "capsule sweep": +inf when there is none; `started` when it touches the triangle at t_min already.
+VXB_FN float vxb_capsule_triangle(const float3 o, const float3 d, const float3 c0, const float3 h, float r, float rr, float dd, float tMin,
+	float tMax, const float3 a, const float3 b, const float3 c, bool& started)
+{
+	started = false;
+	{
+		float3 q; float u, v, w;
+		if (vxb_segment_triangle(c0, h, a, b, c, q, u, v, w) <= rr) { started = true; return tMin; }
+	}
+	const float3 am = make_float3(a.x - h.x, a.y - h.y, a.z - h.z), ap = make_float3(a.x + h.x, a.y + h.y, a.z + h.z);
+	const float3 bm = make_float3(b.x - h.x, b.y - h.y, b.z - h.z), bp = make_float3(b.x + h.x, b.y + h.y, b.z + h.z);
+	const float3 cm = make_float3(c.x - h.x, c.y - h.y, c.z - h.z), cp = make_float3(c.x + h.x, c.y + h.y, c.z + h.z);
+	// the faces: the caps, then the parallelograms of ab, bc, ca
+	float t = vxb_sweep_face<false>(o, d, c0, r, tMin, tMax, am, bm, cm);
+	t = fminf(t, vxb_sweep_face<false>(o, d, c0, r, tMin, tMax, ap, bp, cp));
+	t = fminf(t, vxb_sweep_face<true>(o, d, c0, r, tMin, tMax, am, bm, ap));
+	t = fminf(t, vxb_sweep_face<true>(o, d, c0, r, tMin, tMax, bm, cm, bp));
+	t = fminf(t, vxb_sweep_face<true>(o, d, c0, r, tMin, tMax, cm, am, cp));
+	// the edges of the cap -h, of the cap +h, then the lateral edges
+	t = fminf(t, vxb_sweep_edge(o, d, am, bm, rr, tMin, tMax));
+	t = fminf(t, vxb_sweep_edge(o, d, bm, cm, rr, tMin, tMax));
+	t = fminf(t, vxb_sweep_edge(o, d, cm, am, rr, tMin, tMax));
+	t = fminf(t, vxb_sweep_edge(o, d, ap, bp, rr, tMin, tMax));
+	t = fminf(t, vxb_sweep_edge(o, d, bp, cp, rr, tMin, tMax));
+	t = fminf(t, vxb_sweep_edge(o, d, cp, ap, rr, tMin, tMax));
+	t = fminf(t, vxb_sweep_edge(o, d, am, ap, rr, tMin, tMax));
+	t = fminf(t, vxb_sweep_edge(o, d, bm, bp, rr, tMin, tMax));
+	t = fminf(t, vxb_sweep_edge(o, d, cm, cp, rr, tMin, tMax));
+	// the shifted vertices
+	t = fminf(t, vxb_sweep_vertex(o, d, am, rr, dd, tMin, tMax));
+	t = fminf(t, vxb_sweep_vertex(o, d, bm, rr, dd, tMin, tMax));
+	t = fminf(t, vxb_sweep_vertex(o, d, cm, rr, dd, tMin, tMax));
+	t = fminf(t, vxb_sweep_vertex(o, d, ap, rr, dd, tMin, tMax));
+	t = fminf(t, vxb_sweep_vertex(o, d, bp, rr, dd, tMin, tMax));
+	t = fminf(t, vxb_sweep_vertex(o, d, cp, rr, dd, tMin, tMax));
+	return t;
+}
+
+// the reach of a capsule shape (include/vxb200.h): a finite half axis and max_i |h_i| + extra <= VXB_SPHERE_RADIUS_MAX
+VXB_FN bool vxb_capsule_reach(const float3 h, float extra)
+{
+	const float hm = fmaxf(fmaxf(fabsf(h.x), fabsf(h.y)), fabsf(h.z));
+	return isfinite(h.x) && isfinite(h.y) && isfinite(h.z) && hm + extra <= VXB_SPHERE_RADIUS_MAX;
+}
+
+// The per-triangle reject of the sweep: whether the path meets the box of (a, b, c) grown by g along each axis.
+VXB_FN bool vxb_path_meets_box(const vxb_ray& ray, const float3 g, const float3 a, const float3 b, const float3 c)
+{
+	float te = ray.t_min, tx = ray.t_max;
+	vxb_ray_slab(ray.origin[0], ray.direction[0], fminf(fminf(a.x, b.x), c.x) - g.x, fmaxf(fmaxf(a.x, b.x), c.x) + g.x, te, tx);
+	vxb_ray_slab(ray.origin[1], ray.direction[1], fminf(fminf(a.y, b.y), c.y) - g.y, fmaxf(fmaxf(a.y, b.y), c.y) + g.y, te, tx);
+	vxb_ray_slab(ray.origin[2], ray.direction[2], fminf(fminf(a.z, b.z), c.z) - g.z, fmaxf(fmaxf(a.z, b.z), c.z) + g.z, te, tx);
+	return te <= tx;
+}
+
+// the hit fields of the closest pair at `ctr`: point q, axis point x = ctr + s h, u, v and s = 2w - 1
+VXB_FN void vxb_pair_fields(const float3 ctr, const float3 h, const float3 a, const float3 b, const float3 c, float3& q, float3& x,
+	float& u, float& v, float& s)
+{
+	float w;
+	vxb_segment_triangle(ctr, h, a, b, c, q, u, v, w);
+	s = (w + w) - 1.f;
+	x = make_float3(ctr.x + s * h.x, ctr.y + s * h.y, ctr.z + s * h.z);
+}
+
+// One warp per capsule sweep, persistent over the batch: the block walk of the ray casts with boxes grown by max_i |h_i| + r +
+// eps (the proof at the top of vxb_ray.cuh), and the per-triangle reject above.  Sweeps and hits in OUTPUT (Y-up) coordinates.
+__global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_capsule_cast_kernel(const VxbRayMesh m, const vxb_capsule_sweep* __restrict__ sweeps,
+	unsigned count, vxb_capsule_hit* __restrict__ hits)
+{
+	const unsigned lane = threadIdx.x & 31;
+	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
+	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
+	{
+		const vxb_capsule_sweep cs = sweeps[q];
+		const vxb_ray& ray = cs.path;
+		const float3 o = make_float3(ray.origin[0], ray.origin[1], ray.origin[2]);
+		const float3 d = make_float3(ray.direction[0], ray.direction[1], ray.direction[2]);
+		const float3 h = make_float3(cs.half_axis[0], cs.half_axis[1], cs.half_axis[2]);
+		const float r = cs.radius, rr = r * r;
+		const float tMin = ray.t_min, tMax = ray.t_max;
+		const float3 c0 = make_float3(o.x + tMin * d.x, o.y + tMin * d.y, o.z + tMin * d.z);
+		const float dd = (d.x * d.x + d.y * d.y) + d.z * d.z;
+		const float3 g = make_float3(fabsf(h.x) + r + VXB_RAY_EPS, fabsf(h.y) + r + VXB_RAY_EPS, fabsf(h.z) + r + VXB_RAY_EPS);
+		float bt = CUDART_INF_F;   // this lane's first contact
+		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
+		bool bStarted = false;
+		if (r > 0.f && vxb_capsule_reach(h, r))   // the same for the whole warp
+			vxb_ray_walk(m, ray, fmaxf(fmaxf(g.x, g.y), g.z), bt, [&](const unsigned s) {
+				const vxb_block_record* rec = m.dir + s;
+				const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
+				for (unsigned k = lane; k < tris; k += 32)
+				{
+					float3 a, b, c;
+					vxb_ray_triangle(m, vo, io, k, a, b, c);
+					if (!vxb_path_meets_box(ray, g, a, b, c)) continue;
+					bool started;
+					const float t = vxb_capsule_triangle(o, d, c0, h, r, rr, dd, tMin, tMax, a, b, c, started);
+					if (t < CUDART_INF_F && vxb_ray_before(t, s, k, bt, bs, bk)) { bt = t; bs = s; bk = k; bStarted = started; }
+				}
+			});
+		if (lane == vxb_ray_winner(bt, bs, bk))
+		{
+			vxb_capsule_hit x;
+			x.t = CUDART_INF_F; x.slot = VXB_RAY_MISS; x.block_id = 0; x.triangle = 0;
+			x.center[0] = x.center[1] = x.center[2] = 0.f;
+			x.point[0] = x.point[1] = x.point[2] = 0.f;
+			x.axis_point[0] = x.axis_point[1] = x.axis_point[2] = 0.f;
+			x.normal[0] = x.normal[1] = x.normal[2] = 0.f;
+			x.u = 0.f; x.v = 0.f; x.s = 0.f; x.flags = 0;
+			if (bs != VXB_RAY_MISS)
+			{
+				const vxb_block_record* rec = m.dir + bs;
+				float3 a, b, c;
+				vxb_ray_triangle(m, __ldg(&rec->vertex_offset), __ldg(&rec->index_offset), bk, a, b, c);
+				const float3 ct = make_float3(o.x + bt * d.x, o.y + bt * d.y, o.z + bt * d.z);
+				float3 pq, px;
+				vxb_pair_fields(ct, h, a, b, c, pq, px, x.u, x.v, x.s);
+				x.point[0] = pq.x; x.point[1] = pq.y; x.point[2] = pq.z;
+				x.axis_point[0] = px.x; x.axis_point[1] = px.y; x.axis_point[2] = px.z;
+				x.t = bt; x.slot = bs; x.block_id = __ldg(&rec->id); x.triangle = bk;
+				x.center[0] = ct.x; x.center[1] = ct.y; x.center[2] = ct.z;
+				vxb_ray_blend_normal(m, bs, bk, x.u, x.v, x.normal);
+				x.flags = bStarted ? VXB_SPHERE_STARTED_IN_CONTACT : 0u;
+			}
+			hits[q] = x;
+		}
+	}
+}
+
+// One warp per segment, persistent over the batch: lane k < 27 takes neighbour k of the centre's block (clamped into the
+// grid) and skips it when its box is farther than |h_i| + max_distance + eps along some axis; the warp then tests the
+// candidate blocks' triangles strided over the lanes, with the same per-axis reject per triangle.  OUTPUT (Y-up) coordinates.
+// (A minimum of one CTA per SM in the launch bounds: without it ptxas holds this kernel to 64 registers and spills.)
+__global__ void __launch_bounds__(VXB_COLLIDE_THREADS, 1) vxb_closest_segment_kernel(const VxbRayMesh m, const float maxDistance,
+	const vxb_segment* __restrict__ segments, unsigned count, vxb_segment_hit* __restrict__ hits)
+{
+	const unsigned lane = threadIdx.x & 31;
+	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
+	const int nb = m.nb;
+	const float md2 = maxDistance * maxDistance;
+	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
+	{
+		const vxb_segment sg = segments[q];
+		const float3 p = make_float3(sg.center[0], sg.center[1], sg.center[2]);
+		const float3 h = make_float3(sg.half_axis[0], sg.half_axis[1], sg.half_axis[2]);
+		const float3 g = make_float3(fabsf(h.x) + maxDistance + VXB_RAY_EPS, fabsf(h.y) + maxDistance + VXB_RAY_EPS,
+			fabsf(h.z) + maxDistance + VXB_RAY_EPS);
+		float bd = CUDART_INF_F;   // this lane's nearest triangle
+		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
+		bool cand = false;
+		unsigned slot = VXB_RAY_MISS;
+		if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && vxb_capsule_reach(h, maxDistance) && lane < 27)
+		{
+			const float top = (float)(nb - 1);
+			const int bx = (int)fminf(fmaxf(floorf(p.x * 0.0625f), 0.f), top) + (int)(lane % 3) - 1;
+			const int by = (int)fminf(fmaxf(floorf(p.y * 0.0625f), 0.f), top) + (int)((lane / 3) % 3) - 1;
+			const int bz = (int)fminf(fmaxf(floorf(p.z * 0.0625f), 0.f), top) + (int)(lane / 9) - 1;
+			if (bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb &&
+				!((float)(16 * bx) - p.x > g.x || p.x - (float)(16 * bx + 16) > g.x) &&
+				!((float)(16 * by) - p.y > g.y || p.y - (float)(16 * by + 16) > g.y) &&
+				!((float)(16 * bz) - p.z > g.z || p.z - (float)(16 * bz + 16) > g.z))
+			{
+				slot = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
+				cand = slot != VXB_RAY_MISS;
+			}
+		}
+		unsigned todo = __ballot_sync(0xFFFFFFFFu, cand);
+		while (todo)
+		{
+			const unsigned src = __ffs(todo) - 1;
+			todo &= todo - 1;
+			const unsigned s = __shfl_sync(0xFFFFFFFFu, slot, src);
+			const vxb_block_record* rec = m.dir + s;
+			const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
+			for (unsigned k = lane; k < tris; k += 32)
+			{
+				float3 a, b, c, x;
+				float u, v, w;
+				vxb_ray_triangle(m, vo, io, k, a, b, c);
+				if (fminf(fminf(a.x, b.x), c.x) - p.x > g.x || p.x - fmaxf(fmaxf(a.x, b.x), c.x) > g.x ||
+					fminf(fminf(a.y, b.y), c.y) - p.y > g.y || p.y - fmaxf(fmaxf(a.y, b.y), c.y) > g.y ||
+					fminf(fminf(a.z, b.z), c.z) - p.z > g.z || p.z - fmaxf(fmaxf(a.z, b.z), c.z) > g.z) continue;
+				const float d2 = vxb_segment_triangle(p, h, a, b, c, x, u, v, w);
+				if (d2 <= md2 && vxb_ray_before(d2, s, k, bd, bs, bk)) { bd = d2; bs = s; bk = k; }
+			}
+		}
+		if (lane == vxb_ray_winner(bd, bs, bk))
+		{
+			vxb_segment_hit x;
+			x.distance = CUDART_INF_F; x.slot = VXB_RAY_MISS; x.block_id = 0; x.triangle = 0;
+			x.point[0] = x.point[1] = x.point[2] = 0.f;
+			x.axis_point[0] = x.axis_point[1] = x.axis_point[2] = 0.f;
+			x.normal[0] = x.normal[1] = x.normal[2] = 0.f;
+			x.u = 0.f; x.v = 0.f; x.s = 0.f;
+			if (bs != VXB_RAY_MISS)
+			{
+				const vxb_block_record* rec = m.dir + bs;
+				float3 a, b, c;
+				vxb_ray_triangle(m, __ldg(&rec->vertex_offset), __ldg(&rec->index_offset), bk, a, b, c);
+				float3 pq, px;
+				vxb_pair_fields(p, h, a, b, c, pq, px, x.u, x.v, x.s);
+				x.point[0] = pq.x; x.point[1] = pq.y; x.point[2] = pq.z;
+				x.axis_point[0] = px.x; x.axis_point[1] = px.y; x.axis_point[2] = px.z;
+				x.distance = VXB_SQRT(bd); x.slot = bs; x.block_id = __ldg(&rec->id); x.triangle = bk;
+				vxb_ray_blend_normal(m, bs, bk, x.u, x.v, x.normal);
+			}
+			hits[q] = x;
 		}
 	}
 }

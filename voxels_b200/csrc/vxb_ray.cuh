@@ -31,6 +31,13 @@
 //                cell's 27 neighbours.  A larger radius would need a wider neighbourhood, which is why the radius is capped.
 //   stop         unchanged: te is still two correctly rounded operations from the (rounded) plane, and a contact inside the
 //                grown box has t >= the true te.
+//
+// Capsule sweeps (half axis h, radius r; vxb_collide.cuh) run it with g = max_i |h_i| + r + VXB_RAY_EPS:
+//   tested set   a contact pairs a point c + x h of the capsule's segment (|x| <= 1) with a triangle point within r of it, so
+//                the centre c is within |x h_i| + r <= |h_i| + r <= g - eps (+ rounding) of the triangle along every axis
+//                i, hence inside its block's box grown by g.  A sweep that starts in contact has c(t_min) there too.
+//   anchoring    as for spheres with g in place of r + eps: the reach rule max_i |h_i| + r <= 15 keeps g + rounding < 16.
+//   stop         unchanged.
 #pragma once
 
 #include <math_constants.h>
