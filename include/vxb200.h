@@ -561,6 +561,54 @@ int vxb_mesh_raycast(vxb_mesh* mesh, const vxb_ray* rays, uint32_t count, vxb_ra
  * The mesh's state at the call is what the cast sees: a later apply is queued after it. */
 int vxb_mesh_raycast_device(vxb_mesh* mesh, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits);
 
+/* ---- ray queries against the drawn LOD cut: picking what the renderer shows --------------------------------------------
+ * vxb_mesh_raycast answers about the level-0 surface; where the renderer draws coarser blocks (vxb_mesh_select_cut) the
+ * drawn surface differs from it by up to a cell of the drawn level (2^l voxels).  vxb_mesh_raycast_cut casts against the
+ * triangles the renderer draws for the cut of (lod_camera, lod_factor), so that a cursor or a marker lands on what is seen.
+ *   The drawn set   The cut is exactly vxb_mesh_select_cut's for (lod_camera, lod_factor): the same refine, the same "on the
+ *                   cut" test and the same block_adj; view culling plays no part.  For every block of the cut, the drawn
+ *                   set is its regular triangles and, for every face f with bit f of block_adj set, the triangles of its
+ *                   transition mesh f.  Every vertex (regular or transition) takes the position the vertex shader selects
+ *                   (Rendering.md:48-54): with mask = the bits of sec[3], sec[0..2] when mask != 0 and (mask & block_adj) ==
+ *                   mask, otherwise pos.
+ *   The hit         The test, position, normal and miss value are vxb_mesh_raycast's, on the selected positions (the normal
+ *                   blends the vertices' nrm, which both positions share).  Least t wins; ties go to the lower slot, then to
+ *                   the lower part (the regular mesh before transition face 0, ..., face 5), then to the lower triangle.  A
+ *                   pure function of the mesh (content and order), of (lod_camera, lod_factor) and of the ray: not of the
+ *                   launch, the variant or the rest of the batch.  A miss: slot = VXB_RAY_MISS, t = +inf, every other field
+ *                   (level and face too) zero.
+ *   At lod_factor = 1e30, lim*lim overflows to +inf, so every node above level 0 refines: the cut is all of level 0 with
+ *                   block_adj = 0 and no transition draws.  There the first 48 bytes of every hit equal vxb_mesh_raycast's,
+ *                   with level = 0 and face = 0xFFFFFFFF on a hit.
+ *   The walk        At levels >= 1 a drawn vertex is not proven to stay inside its block's lattice box (t is recomputed after
+ *                   the LOD descent), so the cast rests on the mesh's bounds (the measured boxes above) and on the excursion
+ *                   e: the largest distance by which any block's measured box leaves its lattice box.  The first cut cast
+ *                   after an apply (or after the mesh changed grid size) rebuilds a map from every (level, coord) slot of the
+ *                   bounds to the directory (bounds.slots x 4 bytes: 1.2 MB at 1024^3) and measures e, and WAITS for the
+ *                   stream once to read e back.  Later casts until the next apply do not wait (the device variant).
+ * Refusals (`hits` untouched): VXB_ERR_STATE before the first apply, when the mesh does not hold every level with its
+ * transition meshes (as vxb_mesh_select_cut), and when e + 1/16 exceeds 15 voxels, the reach of the walk (vxb_last_error
+ * names e); VXB_ERR_ARGUMENT for a NULL pointer with count > 0, a lod_factor below VXB_LOD_FACTOR_MIN or not finite, and a
+ * non-finite lod_camera component.  count = 0 does nothing.  The HOST variant also refuses an invalid ray as
+ * vxb_mesh_raycast does, naming its index; on the DEVICE variant such a ray is a miss. */
+typedef struct vxb_cut_hit
+{
+	float t, u, v;          /* as vxb_ray_hit */
+	uint32_t slot;          /* mesh directory slot of the drawn block; VXB_RAY_MISS */
+	uint32_t block_id;      /* vxb_block_record.id of that block */
+	uint32_t triangle;      /* k: indices [part offset + 3k, +3) of the part `face` names (index_offset or trans_index_offset[face]) */
+	float position[3];      /* origin + t * direction */
+	float normal[3];        /* as vxb_ray_hit */
+	uint32_t level;         /* the hit block's level */
+	uint32_t face;          /* 0xFFFFFFFF: the regular mesh; f: the transition mesh of face f (TransitionFaceId order) */
+} vxb_cut_hit;                                                                      /* 56 bytes; the first 48 are vxb_ray_hit's */
+/* HOST memory; blocks until the hits are written. */
+int vxb_mesh_raycast_cut(vxb_mesh* mesh, const float lod_camera[3], float lod_factor,
+                         const vxb_ray* rays, uint32_t count, vxb_cut_hit* hits);
+/* DEVICE memory; enqueued on vxb_stream(ctx) like vxb_mesh_raycast_device (the first cast after an apply waits, see above). */
+int vxb_mesh_raycast_cut_device(vxb_mesh* mesh, const float lod_camera[3], float lod_factor,
+                                const vxb_ray* rays, uint32_t count, vxb_cut_hit* hits);
+
 /* ---- collision queries against the mesh: sphere sweeps and closest points, for character controllers and cameras -------
  * Like the ray queries: the LEVEL-0 regular triangles only, both faces, OUTPUT (Y-up) coordinates, a pure function of the
  * mesh (content and order) and of the query (not of the launch, the variant or the rest of the batch), float32 with no fused

@@ -169,6 +169,10 @@ RAY_DTYPE = np.dtype([("origin", "<f4", 3), ("t_min", "<f4"), ("direction", "<f4
 RAY_HIT_DTYPE = np.dtype([("t", "<f4"), ("u", "<f4"), ("v", "<f4"), ("slot", "<u4"), ("block_id", "<u4"), ("triangle", "<u4"),
                           ("position", "<f4", 3), ("normal", "<f4", 3)])
 assert RAY_DTYPE.itemsize == 32 and RAY_HIT_DTYPE.itemsize == 48
+# vxb_cut_hit (include/vxb200.h "ray queries against the drawn LOD cut"): vxb_ray_hit's 48 bytes, then level and face
+CUT_HIT_DTYPE = np.dtype(RAY_HIT_DTYPE.descr + [("level", "<u4"), ("face", "<u4")])
+CUT_FACE_REGULAR = 0xFFFFFFFF
+assert CUT_HIT_DTYPE.itemsize == 56
 
 
 def make_rays(origins, directions, t_min=0.0, t_max=np.inf):
@@ -361,6 +365,8 @@ def load_library():
         "vxb_mesh_select_cut": (C.c_int, [vp, vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_raycast": (C.c_int, [vp, vp, u32, vp]),
         "vxb_mesh_raycast_device": (C.c_int, [vp, vp, u32, vp]),
+        "vxb_mesh_raycast_cut": (C.c_int, [vp, vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_raycast_cut_device": (C.c_int, [vp, vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_sphere_cast": (C.c_int, [vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_sphere_cast_device": (C.c_int, [vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_closest_point": (C.c_int, [vp, C.c_float, vp, u32, vp]),
@@ -391,6 +397,7 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_mesh_create", "vxb_mesh_destroy", "vxb_mesh_apply", "vxb_mesh_info_get", "vxb_mesh_download",
                     "vxb_mesh_device_arenas", "vxb_mesh_select_lod", "vxb_mesh_bounds_get", "vxb_mesh_download_bounds",
                     "vxb_mesh_select_lod_views", "vxb_mesh_select_cut", "vxb_mesh_raycast", "vxb_mesh_raycast_device",
+                    "vxb_mesh_raycast_cut", "vxb_mesh_raycast_cut_device",
                     "vxb_mesh_sphere_cast", "vxb_mesh_sphere_cast_device", "vxb_mesh_closest_point", "vxb_mesh_closest_point_device",
                     "vxb_mesh_capsule_cast", "vxb_mesh_capsule_cast_device", "vxb_mesh_closest_to_segment",
                     "vxb_mesh_closest_to_segment_device"]
@@ -617,6 +624,30 @@ class Mesh:
         data_ptr()); enqueued on the context's stream, returns without waiting."""
         self.ctx._check(self.L.vxb_mesh_raycast_device(self.h, None if rays_ptr is None else C.c_void_p(rays_ptr), count,
                                                        None if hits_ptr is None else C.c_void_p(hits_ptr)), "vxb_mesh_raycast_device")
+
+    def raycast_cut_rc(self, lod_camera, lod_factor, rays, hits=None, count=None):
+        """vxb_mesh_raycast_cut's return code: `lod_camera` and `rays` (a RAY_DTYPE array) may be None for NULL pointers, `hits`
+        (a CUT_HIT_DTYPE array) None for a NULL pointer; `count` defaults to len(rays)."""
+        cam = np.ascontiguousarray(lod_camera, np.float32) if lod_camera is not None else None
+        rays = np.ascontiguousarray(rays, RAY_DTYPE) if rays is not None else None
+        n = (0 if rays is None else len(rays)) if count is None else count
+        return self.L.vxb_mesh_raycast_cut(self.h, _ptr(cam), lod_factor, _ptr(rays), n, _ptr(hits))
+
+    def raycast_cut(self, lod_camera, lod_factor, origins, directions=None, t_min=0.0, t_max=np.inf):
+        """Casts rays against the triangles vxb_mesh_select_cut's cut of (lod_camera, lod_factor) draws (vxb_mesh_raycast_cut):
+        `origins` / `directions` as for raycast.  Returns a CUT_HIT_DTYPE array."""
+        rays = np.ascontiguousarray(origins if directions is None else make_rays(origins, directions, t_min, t_max), RAY_DTYPE)
+        hits = np.zeros(len(rays), CUT_HIT_DTYPE)
+        self.ctx._check(self.raycast_cut_rc(lod_camera, lod_factor, rays, hits), "vxb_mesh_raycast_cut")
+        return hits
+
+    def raycast_cut_device(self, lod_camera, lod_factor, rays_ptr, count, hits_ptr):
+        """vxb_mesh_raycast_cut_device: `count` vxb_ray at the device address `rays_ptr`, hits to `hits_ptr`; enqueued on the
+        context's stream (the first cast after an apply waits for it once)."""
+        cam = np.ascontiguousarray(lod_camera, np.float32) if lod_camera is not None else None
+        self.ctx._check(self.L.vxb_mesh_raycast_cut_device(self.h, _ptr(cam), lod_factor, None if rays_ptr is None else C.c_void_p(rays_ptr),
+                                                           count, None if hits_ptr is None else C.c_void_p(hits_ptr)),
+                        "vxb_mesh_raycast_cut_device")
 
     def sphere_cast_rc(self, radius, rays, hits=None, count=None):
         """vxb_mesh_sphere_cast's return code for a RAY_DTYPE array (or None for a NULL pointer); the hits go to `hits` (a

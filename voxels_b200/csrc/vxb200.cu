@@ -34,6 +34,7 @@
 #include "vxb_mesh.cuh"
 #include "vxb_ray.cuh"
 #include "vxb_collide.cuh"
+#include "vxb_cutray.cuh"
 
 static_assert(sizeof(VxbVertex) == 48, "PolygonVertex layout");
 static_assert(sizeof(vxb_block_record) == 128, "record layout");
@@ -42,6 +43,7 @@ static_assert(sizeof(vxb_sphere_hit) == 64 && sizeof(vxb_closest_hit) == 48, "co
 static_assert(sizeof(vxb_capsule_sweep) == 48 && sizeof(vxb_segment) == 24 && sizeof(vxb_capsule_hit) == 80 && sizeof(vxb_segment_hit) == 64,
 	"capsule layouts");
 static_assert(sizeof(vxb_view) == 96 && sizeof(vxb_mesh_bounds) == 64 && VXB_MAX_LEVELS == 12, "view and bounds layouts");
+static_assert(sizeof(vxb_cut_hit) == 56 && offsetof(vxb_cut_hit, level) == 48, "vxb_cut_hit layout");
 
 namespace
 {
@@ -2229,6 +2231,14 @@ struct vxb_mesh
 	DevBuf<vxb_capsule_hit> capsuleOut;
 	DevBuf<vxb_segment> segmentIn;
 	DevBuf<vxb_segment_hit> segmentOut;
+	// cut ray casts (vxb_cutray.cuh): the all-level map (bounds slot -> directory slot) and the excursion, measured for the
+	// applied run `cutSerial` on a grid of `cutN`; separate from rayMap, so the level-0 queries never see them
+	DevBuf<unsigned int> cutMap, cutExcursion;
+	bool cutBuilt = false;
+	uint64_t cutSerial = 0;
+	uint32_t cutN = 0;
+	float excursion = 0.f;
+	DevBuf<vxb_cut_hit> cutOut;
 };
 
 namespace
@@ -2266,6 +2276,53 @@ int ensureMap(vxb_mesh* m, VxbRayMesh& rm)
 	return VXB_OK;
 }
 
+// The all-level map and the excursion for the applied run (rebuilt after every apply), queued on ctx->stream; the excursion
+// is read back, so a rebuild waits for the stream once.  Then the refusal of an excursion beyond the walk's reach, and the
+// kernel's view of the mesh.
+int ensureCutMap(vxb_mesh* m, const char* what, VxbCutRayMesh& c)
+{
+	vxb_context* ctx = m->ctx;
+	cudaStream_t st = ctx->stream;
+	const uint32_t nb = m->n / 16;
+	VxbCutMapArgs a;
+	for (int l = 0; l < VXB_MAX_LEVELS; ++l) a.levelBase[l] = m->bounds.level_base[l];
+	a.nb = (int)nb;
+	if (!m->cutBuilt || m->cutSerial != m->serial || m->cutN != m->n)
+	{
+		const size_t slots = m->bounds.slots;
+		if (slots > m->cutMap.count)
+		{
+			VXB_CUDA(ctx, cudaStreamSynchronize(st)); // a query still queued may read the old map
+			VXB_CUDA(ctx, m->cutMap.ensure(slots));
+		}
+		VXB_CUDA(ctx, m->cutExcursion.ensure(1));
+		VXB_CUDA(ctx, cudaMemsetAsync(m->cutMap.p, 0xFF, slots * sizeof(unsigned int), st));
+		VXB_CUDA(ctx, cudaMemsetAsync(m->cutExcursion.p, 0, sizeof(unsigned int), st));
+		const unsigned blocks = m->info.block_count;
+		if (blocks) vxb_cutray_map_kernel<<<(blocks + 255) / 256, 256, 0, st>>>(m->dir.p, blocks, a, m->boxes.p, m->cutMap.p, m->cutExcursion.p);
+		VXB_CUDA(ctx, cudaGetLastError());
+		unsigned bits = 0;
+		VXB_CUDA(ctx, cudaMemcpyAsync(&bits, m->cutExcursion.p, sizeof(bits), cudaMemcpyDeviceToHost, st));
+		VXB_CUDA(ctx, cudaStreamSynchronize(st));
+		memcpy(&m->excursion, &bits, sizeof(bits));
+		m->cutBuilt = true; m->cutSerial = m->serial; m->cutN = m->n;
+	}
+	if (!(m->excursion + VXB_RAY_EPS <= 15.f))
+	{
+		char buf[192];
+		snprintf(buf, sizeof(buf), "%s: a block's vertices leave its lattice box by %g voxels; the walk reaches 15 - 1/16", what, (double)m->excursion);
+		return fail(ctx, VXB_ERR_STATE, buf);
+	}
+	c.m.dir = m->dir.p; c.m.map = m->cutMap.p; c.m.verts = m->set[m->active].v.p; c.m.idx = m->set[m->active].i.p; c.m.nb = (int)nb;
+	c.tverts = m->set[m->active].tv.p; c.tidx = m->set[m->active].ti.p;
+	c.boxes = m->boxes.p;
+	c.slots = a;
+	c.top = (int)m->info.levels - 1;
+	c.grow = std::nextafter(m->excursion + VXB_RAY_EPS, INFINITY);
+	memset(&c.cut, 0, sizeof(c.cut));
+	return VXB_OK;
+}
+
 // CTAs of a persistent one-warp-per-query launch
 unsigned queryCtas(const vxb_context* ctx, uint32_t count, unsigned threads)
 {
@@ -2279,6 +2336,18 @@ int enqueueRaycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit
 	const int e = ensureMap(m, rm);
 	if (e != VXB_OK) return e;
 	vxb_raycast_kernel<<<queryCtas(m->ctx, count, VXB_RAY_THREADS), VXB_RAY_THREADS, 0, m->ctx->stream>>>(rm, rays, count, hits);
+	VXB_CUDA(m->ctx, cudaGetLastError());
+	return VXB_OK;
+}
+
+int enqueueRaycastCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, const vxb_ray* rays, uint32_t count, vxb_cut_hit* hits)
+{
+	VxbCutRayMesh c;
+	const int e = ensureCutMap(m, what, c);
+	if (e != VXB_OK) return e;
+	for (int k = 0; k < 3; ++k) c.cut.camera[k] = camera[k];
+	c.cut.lod = lodFactor;
+	vxb_raycast_cut_kernel<<<queryCtas(m->ctx, count, VXB_RAY_THREADS), VXB_RAY_THREADS, 0, m->ctx->stream>>>(c, rays, count, hits);
 	VXB_CUDA(m->ctx, cudaGetLastError());
 	return VXB_OK;
 }
@@ -2774,6 +2843,66 @@ int vxb_mesh_raycast_device(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vx
 	if (!count) return VXB_OK;
 	cudaSetDevice(ctx->device);
 	return enqueueRaycast(m, rays, count, hits);
+}
+
+} // extern "C"
+
+namespace
+{
+// the checks of the cut casts (include/vxb200.h "ray queries against the drawn LOD cut"): vxb_mesh_raycast's NULL rule,
+// vxb_mesh_select_cut's lod_factor, lod_camera and state rules
+int cutCastChecks(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, const vxb_ray* rays, uint32_t count, const vxb_cut_hit* hits)
+{
+	vxb_context* ctx = m->ctx;
+	char buf[192];
+	if (count && (!camera || !rays || !hits)) { snprintf(buf, sizeof(buf), "%s: NULL lod_camera, rays or hits", what); return fail(ctx, VXB_ERR_ARGUMENT, buf); }
+	if (!std::isfinite(lodFactor) || !(lodFactor >= VXB_LOD_FACTOR_MIN))
+	{
+		snprintf(buf, sizeof(buf), "%s: lod_factor must be finite and >= 2", what);
+		return fail(ctx, VXB_ERR_ARGUMENT, buf);
+	}
+	if (camera && (!std::isfinite(camera[0]) || !std::isfinite(camera[1]) || !std::isfinite(camera[2])))
+	{
+		snprintf(buf, sizeof(buf), "%s: non-finite lod_camera component", what);
+		return fail(ctx, VXB_ERR_ARGUMENT, buf);
+	}
+	if (!m->content) { snprintf(buf, sizeof(buf), "%s: nothing applied yet", what); return fail(ctx, VXB_ERR_STATE, buf); }
+	if (!m->complete)
+	{
+		snprintf(buf, sizeof(buf), "%s: the mesh lacks levels or transition meshes (a run since the last full apply had max_levels "
+			"below the grid's levels or VXB_FLAG_NO_TRANSITIONS)", what);
+		return fail(ctx, VXB_ERR_STATE, buf);
+	}
+	return VXB_OK;
+}
+}
+
+extern "C"
+{
+
+int vxb_mesh_raycast_cut(vxb_mesh* m, const float camera[3], float lodFactor, const vxb_ray* rays, uint32_t count, vxb_cut_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	const int e = cutCastChecks(m, "vxb_mesh_raycast_cut", camera, lodFactor, rays, count, hits);
+	if (e != VXB_OK || !count) return e;
+	const char* why = "";
+	const long long bad = invalidRay(rays, count, &why);
+	if (bad >= 0)
+	{
+		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_raycast_cut: ray %lld: %s", bad, why);
+		return fail(m->ctx, VXB_ERR_ARGUMENT, buf);
+	}
+	return hostQuery(m, m->rayIn, 1, m->cutOut, rays, count, hits,
+		[&](const vxb_ray* in, vxb_cut_hit* out) { return enqueueRaycastCut(m, "vxb_mesh_raycast_cut", camera, lodFactor, in, count, out); });
+}
+
+int vxb_mesh_raycast_cut_device(vxb_mesh* m, const float camera[3], float lodFactor, const vxb_ray* rays, uint32_t count, vxb_cut_hit* hits)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	const int e = cutCastChecks(m, "vxb_mesh_raycast_cut_device", camera, lodFactor, rays, count, hits);
+	if (e != VXB_OK || !count) return e;
+	cudaSetDevice(m->ctx->device);
+	return enqueueRaycastCut(m, "vxb_mesh_raycast_cut_device", camera, lodFactor, rays, count, hits);
 }
 
 int vxb_mesh_sphere_cast(vxb_mesh* m, float radius, const vxb_ray* rays, uint32_t count, vxb_sphere_hit* hits)

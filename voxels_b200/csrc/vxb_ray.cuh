@@ -114,16 +114,33 @@ VXB_FN void vxb_ray_triangle(const VxbRayMesh& m, unsigned vo, unsigned io, unsi
 	c = make_float3(__ldg(pc), __ldg(pc + 1), __ldg(pc + 2));
 }
 
-// The vertex normals of triangle k of slot s blended at (u, v) and normalised, the hit normal of include/vxb200.h:
-// w = (1 - u) - v; n_i = (w*n0_i + u*n1_i) + v*n2_i; n_i / sqrt((nx*nx + ny*ny) + nz*nz), or (0, 0, 0) when that is 0.
-VXB_FN void vxb_ray_blend_normal(const VxbRayMesh& m, unsigned s, unsigned k, float u, float v, float* out)
+// Moeller-Trumbore exactly as include/vxb200.h states it (-fmad=false: no contraction): does the segment (p, d, [tMin, tMax])
+// hit the triangle (p0, p1, p2), with its (t, u, v)
+VXB_FN bool vxb_ray_mt(float px, float py, float pz, float dx, float dy, float dz, float tMin, float tMax, const float3& p0,
+	const float3& p1, const float3& p2, float& t, float& u, float& v)
 {
-	const vxb_block_record* rec = m.dir + s;
-	const unsigned vo = __ldg(&rec->vertex_offset);
-	const unsigned* ip = m.idx + __ldg(&rec->index_offset) + 3 * k;
-	const float* n0 = m.verts[vo + __ldg(ip)].nrm;
-	const float* n1 = m.verts[vo + __ldg(ip + 1)].nrm;
-	const float* n2 = m.verts[vo + __ldg(ip + 2)].nrm;
+	const float e1x = p1.x - p0.x, e1y = p1.y - p0.y, e1z = p1.z - p0.z;
+	const float e2x = p2.x - p0.x, e2y = p2.y - p0.y, e2z = p2.z - p0.z;
+	const float sx = px - p0.x, sy = py - p0.y, sz = pz - p0.z;
+	const float pvx = dy * e2z - dz * e2y, pvy = dz * e2x - dx * e2z, pvz = dx * e2y - dy * e2x;
+	const float det = (e1x * pvx + e1y * pvy) + e1z * pvz;
+	const float inv = VXB_DIV(1.f, det);
+	u = ((sx * pvx + sy * pvy) + sz * pvz) * inv;
+	const float qvx = sy * e1z - sz * e1y, qvy = sz * e1x - sx * e1z, qvz = sx * e1y - sy * e1x;
+	v = ((dx * qvx + dy * qvy) + dz * qvz) * inv;
+	t = ((e2x * qvx + e2y * qvy) + e2z * qvz) * inv;
+	// positive comparisons only: a NaN fails
+	return det != 0.f && u >= 0.f && u <= 1.f && v >= 0.f && u + v <= 1.f && t >= tMin && t <= tMax;
+}
+
+// The vertex normals of the triangle at indices ip (+ vertex offset vo into verts) blended at (u, v) and normalised, the hit
+// normal of include/vxb200.h: w = (1 - u) - v; n_i = (w*n0_i + u*n1_i) + v*n2_i; n_i / sqrt((nx*nx + ny*ny) + nz*nz), or
+// (0, 0, 0) when that is 0.
+VXB_FN void vxb_blend_normal(const VxbVertex* verts, unsigned vo, const unsigned* ip, float u, float v, float* out)
+{
+	const float* n0 = verts[vo + __ldg(ip)].nrm;
+	const float* n1 = verts[vo + __ldg(ip + 1)].nrm;
+	const float* n2 = verts[vo + __ldg(ip + 2)].nrm;
 	const float w = (1.f - u) - v;
 	const float nxv = (w * __ldg(n0) + u * __ldg(n1)) + v * __ldg(n2);
 	const float nyv = (w * __ldg(n0 + 1) + u * __ldg(n1 + 1)) + v * __ldg(n2 + 1);
@@ -131,6 +148,13 @@ VXB_FN void vxb_ray_blend_normal(const VxbRayMesh& m, unsigned s, unsigned k, fl
 	const float len = VXB_SQRT((nxv * nxv + nyv * nyv) + nzv * nzv);
 	out[0] = out[1] = out[2] = 0.f;
 	if (len > 0.f) { out[0] = VXB_DIV(nxv, len); out[1] = VXB_DIV(nyv, len); out[2] = VXB_DIV(nzv, len); }
+}
+
+// the blended normal of regular triangle k of slot s
+VXB_FN void vxb_ray_blend_normal(const VxbRayMesh& m, unsigned s, unsigned k, float u, float v, float* out)
+{
+	const vxb_block_record* rec = m.dir + s;
+	vxb_blend_normal(m.verts, __ldg(&rec->vertex_offset), m.idx + __ldg(&rec->index_offset) + 3 * k, u, v, out);
 }
 
 // The lane holding the warp's least (t, slot, triangle) by the tie rule (every lane takes part; each candidate is held by
@@ -147,16 +171,18 @@ VXB_FN unsigned vxb_ray_winner(float t, unsigned s, unsigned k)
 	return __ffs(__ballot_sync(0xFFFFFFFFu, s == ws && k == wk)) - 1;
 }
 
-// The conservative block walk of the proof at the top, for one segment per warp (every lane calls it with the same ray):
-// the boxes are grown by `grow` (VXB_RAY_EPS for rays, r + VXB_RAY_EPS for sweeps).  `block(s)` is called by the whole warp
-// once for every block of the tested set that has a map entry, in walk order; it tests the block's triangles (strided over
-// the lanes) and lowers this lane's best parameter `best`, which the stop rule reads.  Rays and blocks in OUTPUT (Y-up)
-// coordinates; block coordinates of the map are grid (Z-up): output (x, y, z) = grid (x, z, y).
-template <class Block>
-VXB_FN void vxb_ray_walk(const VxbRayMesh& m, const vxb_ray& ray, const float grow, const float& best, Block&& block)
+// The conservative block walk of the proof at the top, for one segment per warp (every lane calls it with the same ray),
+// with the candidate step as a parameter: lane k < 27 calls `cand(bx, by, bz, T0, T1, t0, t1, last, slot)` for neighbour k
+// of the cell [t0, t1) when that block lies in the grid; it returns whether there is a directory slot to test there, and
+// writes it to `slot`.
+// The grid box is clipped grown by `grow`.  With Dedup, lanes that return the same slot hand it on once (the lowest lane).
+// `block(s)` is called by the whole warp once per slot handed on, in walk order; it tests the slot's triangles (strided
+// over the lanes) and lowers this lane's best parameter `best`, which the stop rule reads.  Rays and blocks in OUTPUT
+// (Y-up) coordinates; block coordinates of the map are grid (Z-up): output (x, y, z) = grid (x, z, y).
+template <bool Dedup, class Cand, class Block>
+VXB_FN void vxb_ray_walk_by(const int nb, const vxb_ray& ray, const float grow, const float& best, Cand&& cand, Block&& block)
 {
 	const unsigned lane = threadIdx.x & 31;
-	const int nb = m.nb;
 	const float n = (float)(16 * nb);
 	// this lane's neighbour offset (lanes 27..31 have none)
 	const int ox = (int)(lane % 3) - 1, oy = (int)((lane / 3) % 3) - 1, oz = (int)(lane / 9) - 1;
@@ -182,21 +208,15 @@ VXB_FN void vxb_ray_walk(const VxbRayMesh& m, const vxb_ray& ray, const float gr
 		const float t1 = last ? T1 : fmaxf(tn, t0);
 		// ---- the neighbours anchored in [t0, t1) ----
 		const int bx = cx + ox, by = cy + oy, bz = cz + oz;
-		bool cand = false;
+		bool take = false;
 		unsigned slot = VXB_RAY_MISS;
-		if (lane < 27 && bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb)
+		if (lane < 27 && bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb) take = cand(bx, by, bz, T0, T1, t0, t1, last, slot);
+		if constexpr (Dedup)
 		{
-			float te = T0, tx = T1;
-			vxb_ray_slab(px, dx, vxb_ray_lo(bx, grow), vxb_ray_hi(bx, grow), te, tx);
-			vxb_ray_slab(py, dy, vxb_ray_lo(by, grow), vxb_ray_hi(by, grow), te, tx);
-			vxb_ray_slab(pz, dz, vxb_ray_lo(bz, grow), vxb_ray_hi(bz, grow), te, tx);
-			if (te <= tx && te >= t0 && (te < t1 || last))
-			{
-				slot = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
-				cand = slot != VXB_RAY_MISS;
-			}
+			const unsigned peers = __match_any_sync(0xFFFFFFFFu, slot);   // every lane takes part (lanes without a slot hold VXB_RAY_MISS)
+			take = take && (peers & ((1u << lane) - 1u)) == 0;
 		}
-		unsigned todo = __ballot_sync(0xFFFFFFFFu, cand);
+		unsigned todo = __ballot_sync(0xFFFFFFFFu, take);
 		const bool tested = todo != 0;
 		while (todo)
 		{
@@ -217,6 +237,30 @@ VXB_FN void vxb_ray_walk(const VxbRayMesh& m, const vxb_ray& ray, const float gr
 		else { cz += dz > 0.f ? 1 : -1; nz = vxb_ray_next(cz, pz, dz, nb); }
 		t0 = t1;
 	}
+}
+
+// The level-0 walk: the tested set is every level-0 block whose lattice box grown by `grow` (VXB_RAY_EPS for rays,
+// r + VXB_RAY_EPS for sweeps) meets the clipped segment and has a map entry; each one is anchored once, so no merging.
+template <class Block>
+VXB_FN void vxb_ray_walk(const VxbRayMesh& m, const vxb_ray& ray, const float grow, const float& best, Block&& block)
+{
+	const float px = ray.origin[0], py = ray.origin[1], pz = ray.origin[2];
+	const float dx = ray.direction[0], dy = ray.direction[1], dz = ray.direction[2];
+	const int nb = m.nb;
+	vxb_ray_walk_by<false>(nb, ray, grow, best,
+		[&](int bx, int by, int bz, float T0, float T1, float t0, float t1, bool last, unsigned& slot) {
+			float te = T0, tx = T1;
+			vxb_ray_slab(px, dx, vxb_ray_lo(bx, grow), vxb_ray_hi(bx, grow), te, tx);
+			vxb_ray_slab(py, dy, vxb_ray_lo(by, grow), vxb_ray_hi(by, grow), te, tx);
+			vxb_ray_slab(pz, dz, vxb_ray_lo(bz, grow), vxb_ray_hi(bz, grow), te, tx);
+			if (te <= tx && te >= t0 && (te < t1 || last))
+			{
+				slot = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
+				return slot != VXB_RAY_MISS;
+			}
+			return false;
+		},
+		block);
 }
 
 // One warp per ray, persistent over the batch.  Rays and hits in OUTPUT (Y-up) coordinates.
@@ -240,20 +284,8 @@ __global__ void __launch_bounds__(VXB_RAY_THREADS) vxb_raycast_kernel(const VxbR
 			{
 				float3 p0, p1, p2;
 				vxb_ray_triangle(m, vo, io, k, p0, p1, p2);
-				const float e1x = p1.x - p0.x, e1y = p1.y - p0.y, e1z = p1.z - p0.z;
-				const float e2x = p2.x - p0.x, e2y = p2.y - p0.y, e2z = p2.z - p0.z;
-				const float sx = px - p0.x, sy = py - p0.y, sz = pz - p0.z;
-				// Moeller-Trumbore exactly as include/vxb200.h states it (-fmad=false: no contraction)
-				const float pvx = dy * e2z - dz * e2y, pvy = dz * e2x - dx * e2z, pvz = dx * e2y - dy * e2x;
-				const float det = (e1x * pvx + e1y * pvy) + e1z * pvz;
-				const float inv = VXB_DIV(1.f, det);
-				const float u = ((sx * pvx + sy * pvy) + sz * pvz) * inv;
-				const float qvx = sy * e1z - sz * e1y, qvy = sz * e1x - sx * e1z, qvz = sx * e1y - sy * e1x;
-				const float v = ((dx * qvx + dy * qvy) + dz * qvz) * inv;
-				const float t = ((e2x * qvx + e2y * qvy) + e2z * qvz) * inv;
-				// positive comparisons only: a NaN fails
-				if (det != 0.f && u >= 0.f && u <= 1.f && v >= 0.f && u + v <= 1.f && t >= tMin && t <= tMax &&
-					vxb_ray_before(t, s, k, bt, bs, bk))
+				float t, u, v;
+				if (vxb_ray_mt(px, py, pz, dx, dy, dz, tMin, tMax, p0, p1, p2, t, u, v) && vxb_ray_before(t, s, k, bt, bs, bk))
 				{
 					bt = t; bs = s; bk = k; bu = u; bv = v;
 				}
