@@ -793,6 +793,61 @@ int vxb_mesh_closest_to_segment(vxb_mesh* mesh, float max_distance, const vxb_se
 int vxb_mesh_capsule_cast_device(vxb_mesh* mesh, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits);
 int vxb_mesh_closest_to_segment_device(vxb_mesh* mesh, float max_distance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits);
 
+/* ---- box overlap gathers: the level-0 triangles in axis-aligned boxes, for a client's physics mid-phase and navmesh tiles --
+ * Every other query returns one answer per query; vxb_mesh_overlap_box returns, per box, every triangle that overlaps it, so
+ * that a physics engine runs its own narrowphase for its own shapes (processAllTriangles-style callbacks), a navmesh builder
+ * rebuilds the tiles around an edit, and a decal clips what it covers.
+ *   Scope       The LEVEL-0 regular triangles only, both faces, OUTPUT (Y-up) coordinates.  The query box is closed.
+ *   The test    A separating-axis test in float32 with no fused multiply-add, in exactly this order, with p0, p1, p2 the pos
+ *               of vertices index[3k], index[3k+1], index[3k+2] (+ vertex_offset):
+ *     1  box axes, exact (no arithmetic): for each i, min(p0_i, p1_i, p2_i) <= max_i && max(p0_i, p1_i, p2_i) >= min_i,
+ *        else no overlap.
+ *     2  box frame: c_i = (min_i + max_i) * 0.5; h_i = max_i*0.5 - min_i*0.5 (finite for every finite box, unlike
+ *        (max_i - min_i) * 0.5); v_k = p_k - c per component; e0 = v1 - v0, e1 = v2 - v1, e2 = v0 - v2.
+ *     3  the axes, in this order: the normal n = e0 x e1 (the collision queries' cross product), then u_i x e_j for i = x, y, z
+ *        (outer) and j = 0, 1, 2 (inner), written with their literal zero:
+ *            u_x x e = (0, -e_z, e_y);   u_y x e = (e_z, 0, -e_x);   u_z x e = (-e_y, e_x, 0).
+ *        For an axis a: s_k = (a_x*v_k.x + a_y*v_k.y) + a_z*v_k.z for k = 0, 1, 2 (all three vertices on every axis: in float
+ *        the two vertices of an edge do not project equally, so Akenine-Moller's two-vertex shortcut is not taken);
+ *        r = (h_x*|a_x| + h_y*|a_y|) + h_z*|a_z|; the axis separates iff (s0 > r && s1 > r && s2 > r) || (s0 < -r && s1 < -r
+ *        && s2 < -r), i.e. min(s) > r || max(s) < -r with positive comparisons (a NaN s never separates).
+ *     4  the triangle overlaps iff no axis separates.  A zero axis (a degenerate edge, a collinear triangle) never separates.
+ *   A kernel may drop the products with a literal zero component: h and v are finite, so such a product is +-0, and
+ *   x + (+-0) == x.  At most the sign of a zero s or r changes, which no comparison above sees.
+ *   The result  offsets has count + 1 entries: the exclusive prefix sum of the boxes' triangle counts, offsets[count] = the
+ *               total; tris[offsets[q] .. offsets[q+1]) are the triangles of box q, in ascending coord_id of their block (grid
+ *               order), then ascending triangle index.  A pure function of the mesh (content and order) and the box: not of the
+ *               launch, the variant or the other boxes of the batch.
+ *   Capacity    tris == NULL (with capacity == 0) counts only and returns VXB_OK.  The HOST variant returns VXB_ERR_CAPACITY
+ *               when offsets[count] > capacity; it still writes `offsets` (size tris from offsets[count] and repeat) and
+ *               leaves `tris` untouched.  The DEVICE variant always writes `offsets` and writes `tris` only when offsets[count]
+ *               <= capacity, decided on the device, with no host synchronisation: compare the two when reading them.
+ *   The walk    An accepted triangle's vertices lie in its block's closed lattice box and in its measured box (the bounds
+ *               above), and they meet the query box (test 1).  So the candidates are the blocks whose closed lattice box
+ *               meets the query box, clipped to the grid, and a candidate whose measured box misses the query box is skipped.
+ *               Both tests are exact: the gather needs no epsilon.  There is no limit on box size; a box partly or wholly
+ *               outside the grid is legal.  One box is walked by one warp, so a single very large box takes as long as its
+ *               blocks and triangles take one warp.  The level-0 map is the ray queries'.
+ * Refusals (`offsets` and `tris` untouched): VXB_ERR_STATE before the first vxb_mesh_apply; VXB_ERR_ARGUMENT for a NULL boxes
+ * or offsets, or a NULL tris with capacity > 0, when count > 0; count = 0 does nothing.  The HOST variant refuses a box with
+ * a non-finite component or min_i > max_i (NaN included), naming its index in vxb_last_error; on the DEVICE variant such a
+ * box has 0 triangles. */
+typedef struct vxb_box { float min[3]; float max[3]; } vxb_box;                          /* 24 bytes, OUTPUT (Y-up) coordinates */
+typedef struct vxb_overlap_triangle
+{
+	float p[3][3];          /* pos of the triangle's three vertices, index order */
+	uint32_t slot;          /* mesh directory slot, as vxb_ray_hit */
+	uint32_t block_id;      /* vxb_block_record.id */
+	uint32_t triangle;      /* k: indices [index_offset + 3k, +3) of the block */
+} vxb_overlap_triangle;                                                                  /* 48 bytes */
+/* HOST memory; blocks.  offsets: count + 1 entries. */
+int vxb_mesh_overlap_box(vxb_mesh* mesh, const vxb_box* boxes, uint32_t count,
+                         uint64_t* offsets, vxb_overlap_triangle* tris, uint64_t capacity);
+/* DEVICE memory; enqueued on vxb_stream(ctx) like the other _device queries (it sees the mesh as of its place in the queue),
+ * returns without waiting. */
+int vxb_mesh_overlap_box_device(vxb_mesh* mesh, const vxb_box* boxes, uint32_t count,
+                                uint64_t* offsets, vxb_overlap_triangle* tris, uint64_t capacity);
+
 /* GetMaterial(id) == nullptr handling (TransVoxelImpl.cpp:1364-1368: textures stay zero, one LS_Error log per
  * vertex): after vxb_result_download the material ids of those vertices, in the reference's logging order
  * (level, block, regular vertices, then transition faces), can be read here.  Returns the count; copies at

@@ -206,6 +206,19 @@ SEGMENT_HIT_DTYPE = np.dtype([("distance", "<f4"), ("slot", "<u4"), ("block_id",
 assert CAPSULE_SWEEP_DTYPE.itemsize == 48 and SEGMENT_DTYPE.itemsize == 24
 assert CAPSULE_HIT_DTYPE.itemsize == 80 and SEGMENT_HIT_DTYPE.itemsize == 64
 
+# vxb_box / vxb_overlap_triangle (include/vxb200.h "box overlap gathers")
+BOX_DTYPE = np.dtype([("min", "<f4", 3), ("max", "<f4", 3)])
+OVERLAP_TRIANGLE_DTYPE = np.dtype([("p", "<f4", (3, 3)), ("slot", "<u4"), ("block_id", "<u4"), ("triangle", "<u4")])
+assert BOX_DTYPE.itemsize == 24 and OVERLAP_TRIANGLE_DTYPE.itemsize == 48
+
+
+def make_boxes(mins, maxs):
+    """A BOX_DTYPE array from [count, 3] minima and maxima (OUTPUT, Y-up coordinates)."""
+    lo = np.asarray(mins, np.float32).reshape(-1, 3)
+    boxes = np.zeros(len(lo), BOX_DTYPE)
+    boxes["min"], boxes["max"] = lo, np.asarray(maxs, np.float32).reshape(-1, 3)
+    return boxes
+
 
 def make_capsule_sweeps(origins, directions, half_axes, radius, t_min=0.0, t_max=np.inf):
     """A CAPSULE_SWEEP_DTYPE array: the centre paths as make_rays, `half_axes` [count, 3] or [3], `radius` a scalar or [count]."""
@@ -375,6 +388,8 @@ def load_library():
         "vxb_mesh_capsule_cast_device": (C.c_int, [vp, vp, u32, vp]),
         "vxb_mesh_closest_to_segment": (C.c_int, [vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_closest_to_segment_device": (C.c_int, [vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_overlap_box": (C.c_int, [vp, vp, u32, vp, vp, u64]),
+        "vxb_mesh_overlap_box_device": (C.c_int, [vp, vp, u32, vp, vp, u64]),
         "vxb_host_alloc": (vp, [C.c_size_t]),
         "vxb_host_free": (None, [vp]),
     }
@@ -400,7 +415,7 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_mesh_raycast_cut", "vxb_mesh_raycast_cut_device",
                     "vxb_mesh_sphere_cast", "vxb_mesh_sphere_cast_device", "vxb_mesh_closest_point", "vxb_mesh_closest_point_device",
                     "vxb_mesh_capsule_cast", "vxb_mesh_capsule_cast_device", "vxb_mesh_closest_to_segment",
-                    "vxb_mesh_closest_to_segment_device"]
+                    "vxb_mesh_closest_to_segment_device", "vxb_mesh_overlap_box", "vxb_mesh_overlap_box_device"]
 
 
 def nccl_unique_id():
@@ -737,6 +752,35 @@ class Mesh:
                                                                   None if segments_ptr is None else C.c_void_p(segments_ptr), count,
                                                                   None if hits_ptr is None else C.c_void_p(hits_ptr)),
                         "vxb_mesh_closest_to_segment_device")
+
+    def overlap_boxes_rc(self, boxes, offsets, tris=None, capacity=None, count=None):
+        """vxb_mesh_overlap_box's return code for a BOX_DTYPE array (or None for a NULL pointer): offsets to `offsets` (a uint64
+        array of count + 1, or None), triangles to `tris` (an OVERLAP_TRIANGLE_DTYPE array, or None for a NULL pointer);
+        `capacity` defaults to len(tris) (0 without), `count` to len(boxes)."""
+        boxes = np.ascontiguousarray(boxes, BOX_DTYPE) if boxes is not None else None
+        n = (0 if boxes is None else len(boxes)) if count is None else count
+        cap = (0 if tris is None else len(tris)) if capacity is None else capacity
+        return self.L.vxb_mesh_overlap_box(self.h, _ptr(boxes), n, _ptr(offsets), _ptr(tris), cap)
+
+    def overlap_boxes(self, boxes):
+        """The level-0 triangles overlapping each box of a BOX_DTYPE array (make_boxes; OUTPUT, Y-up coordinates),
+        vxb_mesh_overlap_box: a count-only call, then the fill.  Returns (offsets [count + 1] uint64, OVERLAP_TRIANGLE_DTYPE
+        array): box q's triangles are tris[offsets[q]:offsets[q + 1]]."""
+        boxes = np.ascontiguousarray(boxes, BOX_DTYPE)
+        offsets = np.zeros(len(boxes) + 1, np.uint64)
+        self.ctx._check(self.overlap_boxes_rc(boxes, offsets), "vxb_mesh_overlap_box")
+        tris = np.zeros(int(offsets[-1]), OVERLAP_TRIANGLE_DTYPE)
+        self.ctx._check(self.overlap_boxes_rc(boxes, offsets, tris), "vxb_mesh_overlap_box")
+        return offsets, tris
+
+    def overlap_boxes_device(self, boxes_ptr, count, offsets_ptr, tris_ptr, capacity):
+        """vxb_mesh_overlap_box_device: `count` vxb_box at the device address `boxes_ptr`, count + 1 uint64 offsets to
+        `offsets_ptr`, at most `capacity` triangles to `tris_ptr` (None: count only); enqueued on the context's stream, returns
+        without waiting."""
+        self.ctx._check(self.L.vxb_mesh_overlap_box_device(self.h, None if boxes_ptr is None else C.c_void_p(boxes_ptr), count,
+                                                           None if offsets_ptr is None else C.c_void_p(offsets_ptr),
+                                                           None if tris_ptr is None else C.c_void_p(tris_ptr), capacity),
+                        "vxb_mesh_overlap_box_device")
 
 
 class Context:

@@ -35,6 +35,7 @@
 #include "vxb_ray.cuh"
 #include "vxb_collide.cuh"
 #include "vxb_cutray.cuh"
+#include "vxb_overlap.cuh"
 
 static_assert(sizeof(VxbVertex) == 48, "PolygonVertex layout");
 static_assert(sizeof(vxb_block_record) == 128, "record layout");
@@ -44,6 +45,7 @@ static_assert(sizeof(vxb_capsule_sweep) == 48 && sizeof(vxb_segment) == 24 && si
 	"capsule layouts");
 static_assert(sizeof(vxb_view) == 96 && sizeof(vxb_mesh_bounds) == 64 && VXB_MAX_LEVELS == 12, "view and bounds layouts");
 static_assert(sizeof(vxb_cut_hit) == 56 && offsetof(vxb_cut_hit, level) == 48, "vxb_cut_hit layout");
+static_assert(sizeof(vxb_box) == 24 && sizeof(vxb_overlap_triangle) == 48, "overlap layouts");
 
 namespace
 {
@@ -2239,6 +2241,11 @@ struct vxb_mesh
 	uint32_t cutN = 0;
 	float excursion = 0.f;
 	DevBuf<vxb_cut_hit> cutOut;
+	// box overlap gathers (vxb_overlap.cuh): the per-box counts and the scan's storage, the host variant's staging
+	DevBuf<uint64_t> overlapCounts, overlapOffsets;
+	DevBuf<unsigned char> overlapTemp;
+	DevBuf<vxb_box> boxIn;
+	DevBuf<vxb_overlap_triangle> overlapOut;
 };
 
 namespace
@@ -2390,6 +2397,54 @@ int enqueueClosestSegment(vxb_mesh* m, float maxDistance, const vxb_segment* seg
 	vxb_closest_segment_kernel<<<queryCtas(m->ctx, count, VXB_COLLIDE_THREADS), VXB_COLLIDE_THREADS, 0, m->ctx->stream>>>(rm, maxDistance, segments, count, hits);
 	VXB_CUDA(m->ctx, cudaGetLastError());
 	return VXB_OK;
+}
+
+// the gather kernels' view of the mesh: the level-0 map (ensureMap) and the level-0 bounds
+int overlapView(vxb_mesh* m, VxbOverlapMesh& om)
+{
+	const int e = ensureMap(m, om.m);
+	om.boxes = m->boxes.p;
+	om.base0 = m->bounds.level_base[0];
+	return e;
+}
+
+// The gather's pipeline on ctx->stream: the count kernel, the exclusive scan of the counts into `offsets` (count + 1
+// entries), and, when tris is given, the write kernel (which compares offsets[count] with capacity on the device).  Scratch
+// that grows waits for the stream first: a gather still queued may use it.
+int enqueueOverlap(vxb_mesh* m, const vxb_box* boxes, uint32_t count, uint64_t* offsets, vxb_overlap_triangle* tris, uint64_t capacity)
+{
+	vxb_context* ctx = m->ctx;
+	cudaStream_t st = ctx->stream;
+	VxbOverlapMesh om;
+	const int e = overlapView(m, om);
+	if (e != VXB_OK) return e;
+	const uint64_t entries = (uint64_t)count + 1;
+	size_t tempBytes = 0;
+	VXB_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, tempBytes, m->overlapCounts.p, offsets, entries, st));
+	if (entries > m->overlapCounts.count || tempBytes > m->overlapTemp.count)
+	{
+		VXB_CUDA(ctx, cudaStreamSynchronize(st));
+		VXB_CUDA(ctx, m->overlapCounts.ensure(entries)); VXB_CUDA(ctx, m->overlapTemp.ensure(std::max<size_t>(tempBytes, 1)));
+	}
+	const unsigned ctas = queryCtas(ctx, count, VXB_OVERLAP_THREADS);
+	vxb_overlap_kernel<false><<<ctas, VXB_OVERLAP_THREADS, 0, st>>>(om, boxes, count, m->overlapCounts.p, nullptr, 0);
+	VXB_CUDA(ctx, cudaGetLastError());
+	VXB_CUDA(ctx, cub::DeviceScan::ExclusiveSum(m->overlapTemp.p, tempBytes, m->overlapCounts.p, offsets, entries, st));
+	if (tris)
+	{
+		vxb_overlap_kernel<true><<<ctas, VXB_OVERLAP_THREADS, 0, st>>>(om, boxes, count, offsets, tris, capacity);
+		VXB_CUDA(ctx, cudaGetLastError());
+	}
+	return VXB_OK;
+}
+
+// the host variant's box rule (include/vxb200.h "box overlap gathers"): the index of the first invalid box, or -1
+long long invalidBox(const vxb_box* boxes, uint32_t count)
+{
+	for (uint32_t q = 0; q < count; ++q)
+		for (int i = 0; i < 3; ++i)
+			if (!std::isfinite(boxes[q].min[i]) || !std::isfinite(boxes[q].max[i]) || !(boxes[q].min[i] <= boxes[q].max[i])) return q;
+	return -1;
 }
 
 // the reach rule of the capsule queries (include/vxb200.h), in float as the kernels evaluate it: a finite half axis and
@@ -3035,6 +3090,69 @@ int vxb_mesh_closest_to_segment_device(vxb_mesh* m, float maxDistance, const vxb
 	if (!count) return VXB_OK;
 	cudaSetDevice(ctx->device);
 	return enqueueClosestSegment(m, maxDistance, segments, count, hits);
+}
+
+int vxb_mesh_overlap_box(vxb_mesh* m, const vxb_box* boxes, uint32_t count, uint64_t* offsets, vxb_overlap_triangle* tris, uint64_t capacity)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (count && (!boxes || !offsets || (!tris && capacity))) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_overlap_box: NULL boxes, offsets or tris");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_overlap_box: nothing applied yet");
+	if (!count) return VXB_OK;
+	const long long bad = invalidBox(boxes, count);
+	if (bad >= 0)
+	{
+		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_overlap_box: box %lld: non-finite component or min > max", bad);
+		return fail(ctx, VXB_ERR_ARGUMENT, buf);
+	}
+	cudaSetDevice(ctx->device);
+	cudaStream_t st = ctx->stream;
+	const uint64_t entries = (uint64_t)count + 1;
+	if (count > m->boxIn.count || entries > m->overlapOffsets.count)
+	{
+		VXB_CUDA(ctx, cudaStreamSynchronize(st)); // nothing queued may still use the staging being replaced
+		VXB_CUDA(ctx, m->boxIn.ensure(count)); VXB_CUDA(ctx, m->overlapOffsets.ensure(entries));
+	}
+	VXB_CUDA(ctx, cudaMemcpyAsync(m->boxIn.p, boxes, sizeof(vxb_box) * count, cudaMemcpyHostToDevice, st));
+	// count and scan, then the total decides the fill: the triangles are only written when they fit
+	int r = enqueueOverlap(m, m->boxIn.p, count, m->overlapOffsets.p, nullptr, 0);
+	if (r != VXB_OK) return r;
+	uint64_t total = 0;
+	VXB_CUDA(ctx, cudaMemcpyAsync(&total, m->overlapOffsets.p + count, sizeof(total), cudaMemcpyDeviceToHost, st));
+	VXB_CUDA(ctx, cudaStreamSynchronize(st));
+	if (tris && total <= capacity && total)
+	{
+		if (total > m->overlapOut.count) VXB_CUDA(ctx, m->overlapOut.ensure(total)); // the stream is idle here
+		VxbOverlapMesh om;
+		r = overlapView(m, om);   // the map is built: this queues nothing
+		if (r != VXB_OK) return r;
+		vxb_overlap_kernel<true><<<queryCtas(ctx, count, VXB_OVERLAP_THREADS), VXB_OVERLAP_THREADS, 0, st>>>(om, m->boxIn.p, count,
+			m->overlapOffsets.p, m->overlapOut.p, total);
+		VXB_CUDA(ctx, cudaGetLastError());
+		VXB_CUDA(ctx, cudaMemcpyAsync(tris, m->overlapOut.p, sizeof(vxb_overlap_triangle) * total, cudaMemcpyDeviceToHost, st));
+	}
+	VXB_CUDA(ctx, cudaMemcpyAsync(offsets, m->overlapOffsets.p, sizeof(uint64_t) * entries, cudaMemcpyDeviceToHost, st));
+	VXB_CUDA(ctx, cudaStreamSynchronize(st));
+	if (tris && total > capacity)
+	{
+		char buf[192];
+		snprintf(buf, sizeof(buf), "vxb_mesh_overlap_box: %llu triangles exceed the capacity of %llu; offsets are written",
+			(unsigned long long)total, (unsigned long long)capacity);
+		return fail(ctx, VXB_ERR_CAPACITY, buf);
+	}
+	return VXB_OK;
+}
+
+int vxb_mesh_overlap_box_device(vxb_mesh* m, const vxb_box* boxes, uint32_t count, uint64_t* offsets, vxb_overlap_triangle* tris, uint64_t capacity)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	if (count && (!boxes || !offsets || (!tris && capacity)))
+		return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_overlap_box_device: NULL boxes, offsets or tris");
+	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_overlap_box_device: nothing applied yet");
+	if (!count) return VXB_OK;
+	cudaSetDevice(ctx->device);
+	return enqueueOverlap(m, boxes, count, offsets, tris, capacity);
 }
 
 } // extern "C"
