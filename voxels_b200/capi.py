@@ -436,6 +436,14 @@ def _ptr(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def _dev(p):  # a device address (e.g. a torch tensor's data_ptr()), or None for a NULL pointer
+    return None if p is None else C.c_void_p(p)
+
+
+def _batch(a, dtype):  # a host batch as a contiguous `dtype` array, or None for a NULL pointer
+    return None if a is None else np.ascontiguousarray(a, dtype)
+
+
 def pack_dense(dist, mat, blend, out=None):
     """Host helper: the reference's PackForSave bytes for dense [z,y,x] volumes (numpy uint8 array).  No GPU needed."""
     L = load_library()
@@ -602,7 +610,7 @@ class Mesh:
     def select_cut_rc(self, lod_camera, lod_factor, views, lists_out=None, count=None):
         """vxb_mesh_select_cut's return code: `lod_camera` and `views` ([views, 6, 4] plane coefficients or a View array) may be
         None for NULL pointers, `lists_out` (a DrawLists array) None for a NULL out; `count` defaults to len(views)."""
-        cam = np.ascontiguousarray(lod_camera, np.float32) if lod_camera is not None else None
+        cam = _batch(lod_camera, np.float32)
         if views is not None and not isinstance(views, C.Array):
             views = make_views(views)
         n = (0 if views is None else len(views)) if count is None else count
@@ -623,7 +631,7 @@ class Mesh:
     def raycast_rc(self, rays, hits=None):
         """vxb_mesh_raycast's return code for a RAY_DTYPE array; the hits go to `hits` (a RAY_HIT_DTYPE array, or None for a
         NULL pointer)."""
-        rays = np.ascontiguousarray(rays, RAY_DTYPE) if rays is not None else None
+        rays = _batch(rays, RAY_DTYPE)
         return self.L.vxb_mesh_raycast(self.h, _ptr(rays), 0 if rays is None else len(rays), _ptr(hits))
 
     def raycast(self, origins, directions=None, t_min=0.0, t_max=np.inf):
@@ -631,22 +639,20 @@ class Mesh:
         (Y-up) coordinates, or `origins` is a RAY_DTYPE array and `directions` None.  Returns a RAY_HIT_DTYPE array."""
         rays = np.ascontiguousarray(origins if directions is None else make_rays(origins, directions, t_min, t_max), RAY_DTYPE)
         hits = np.zeros(len(rays), RAY_HIT_DTYPE)
-        self.ctx._check(self.L.vxb_mesh_raycast(self.h, _ptr(rays), len(rays), _ptr(hits)), "vxb_mesh_raycast")
+        self.ctx._check(self.raycast_rc(rays, hits), "vxb_mesh_raycast")
         return hits
 
     def raycast_device(self, rays_ptr, count, hits_ptr):
         """vxb_mesh_raycast_device: `count` vxb_ray at the device address `rays_ptr`, hits to `hits_ptr` (e.g. torch tensors'
         data_ptr()); enqueued on the context's stream, returns without waiting."""
-        self.ctx._check(self.L.vxb_mesh_raycast_device(self.h, None if rays_ptr is None else C.c_void_p(rays_ptr), count,
-                                                       None if hits_ptr is None else C.c_void_p(hits_ptr)), "vxb_mesh_raycast_device")
+        self.ctx._check(self.L.vxb_mesh_raycast_device(self.h, _dev(rays_ptr), count, _dev(hits_ptr)), "vxb_mesh_raycast_device")
 
     def raycast_cut_rc(self, lod_camera, lod_factor, rays, hits=None, count=None):
         """vxb_mesh_raycast_cut's return code: `lod_camera` and `rays` (a RAY_DTYPE array) may be None for NULL pointers, `hits`
         (a CUT_HIT_DTYPE array) None for a NULL pointer; `count` defaults to len(rays)."""
-        cam = np.ascontiguousarray(lod_camera, np.float32) if lod_camera is not None else None
-        rays = np.ascontiguousarray(rays, RAY_DTYPE) if rays is not None else None
+        rays = _batch(rays, RAY_DTYPE)
         n = (0 if rays is None else len(rays)) if count is None else count
-        return self.L.vxb_mesh_raycast_cut(self.h, _ptr(cam), lod_factor, _ptr(rays), n, _ptr(hits))
+        return self.L.vxb_mesh_raycast_cut(self.h, _ptr(_batch(lod_camera, np.float32)), lod_factor, _ptr(rays), n, _ptr(hits))
 
     def raycast_cut(self, lod_camera, lod_factor, origins, directions=None, t_min=0.0, t_max=np.inf):
         """Casts rays against the triangles vxb_mesh_select_cut's cut of (lod_camera, lod_factor) draws (vxb_mesh_raycast_cut):
@@ -659,15 +665,13 @@ class Mesh:
     def raycast_cut_device(self, lod_camera, lod_factor, rays_ptr, count, hits_ptr):
         """vxb_mesh_raycast_cut_device: `count` vxb_ray at the device address `rays_ptr`, hits to `hits_ptr`; enqueued on the
         context's stream (the first cast after an apply waits for it once)."""
-        cam = np.ascontiguousarray(lod_camera, np.float32) if lod_camera is not None else None
-        self.ctx._check(self.L.vxb_mesh_raycast_cut_device(self.h, _ptr(cam), lod_factor, None if rays_ptr is None else C.c_void_p(rays_ptr),
-                                                           count, None if hits_ptr is None else C.c_void_p(hits_ptr)),
-                        "vxb_mesh_raycast_cut_device")
+        self.ctx._check(self.L.vxb_mesh_raycast_cut_device(self.h, _ptr(_batch(lod_camera, np.float32)), lod_factor, _dev(rays_ptr),
+                                                           count, _dev(hits_ptr)), "vxb_mesh_raycast_cut_device")
 
     def sphere_cast_rc(self, radius, rays, hits=None, count=None):
         """vxb_mesh_sphere_cast's return code for a RAY_DTYPE array (or None for a NULL pointer); the hits go to `hits` (a
         SPHERE_HIT_DTYPE array, or None for a NULL pointer); `count` defaults to len(rays)."""
-        rays = np.ascontiguousarray(rays, RAY_DTYPE) if rays is not None else None
+        rays = _batch(rays, RAY_DTYPE)
         n = (0 if rays is None else len(rays)) if count is None else count
         return self.L.vxb_mesh_sphere_cast(self.h, radius, _ptr(rays), n, _ptr(hits))
 
@@ -677,19 +681,20 @@ class Mesh:
         `directions` None.  Returns a SPHERE_HIT_DTYPE array."""
         rays = np.ascontiguousarray(origins if directions is None else make_rays(origins, directions, t_min, t_max), RAY_DTYPE)
         hits = np.zeros(len(rays), SPHERE_HIT_DTYPE)
-        self.ctx._check(self.L.vxb_mesh_sphere_cast(self.h, radius, _ptr(rays), len(rays), _ptr(hits)), "vxb_mesh_sphere_cast")
+        self.ctx._check(self.sphere_cast_rc(radius, rays, hits), "vxb_mesh_sphere_cast")
         return hits
 
     def sphere_cast_device(self, radius, rays_ptr, count, hits_ptr):
         """vxb_mesh_sphere_cast_device: `count` vxb_ray at the device address `rays_ptr`, hits to `hits_ptr`; enqueued on the
         context's stream, returns without waiting."""
-        self.ctx._check(self.L.vxb_mesh_sphere_cast_device(self.h, radius, None if rays_ptr is None else C.c_void_p(rays_ptr), count,
-                                                           None if hits_ptr is None else C.c_void_p(hits_ptr)), "vxb_mesh_sphere_cast_device")
+        self.ctx._check(self.L.vxb_mesh_sphere_cast_device(self.h, radius, _dev(rays_ptr), count, _dev(hits_ptr)),
+                        "vxb_mesh_sphere_cast_device")
 
     def closest_points_rc(self, max_distance, points, hits=None, count=None):
         """vxb_mesh_closest_point's return code for [count, 3] float32 points (or None for a NULL pointer); the hits go to
         `hits` (a CLOSEST_HIT_DTYPE array, or None for a NULL pointer); `count` defaults to len(points)."""
-        pts = np.ascontiguousarray(points, np.float32).reshape(-1, 3) if points is not None else None
+        pts = _batch(points, np.float32)
+        pts = None if pts is None else pts.reshape(-1, 3)
         n = (0 if pts is None else len(pts)) if count is None else count
         return self.L.vxb_mesh_closest_point(self.h, max_distance, _ptr(pts), n, _ptr(hits))
 
@@ -698,20 +703,19 @@ class Mesh:
         coordinates), vxb_mesh_closest_point.  Returns a CLOSEST_HIT_DTYPE array."""
         pts = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
         hits = np.zeros(len(pts), CLOSEST_HIT_DTYPE)
-        self.ctx._check(self.L.vxb_mesh_closest_point(self.h, max_distance, _ptr(pts), len(pts), _ptr(hits)), "vxb_mesh_closest_point")
+        self.ctx._check(self.closest_points_rc(max_distance, pts, hits), "vxb_mesh_closest_point")
         return hits
 
     def closest_points_device(self, max_distance, points_ptr, count, hits_ptr):
         """vxb_mesh_closest_point_device: `count` points (3 floats each) at the device address `points_ptr`, hits to
         `hits_ptr`; enqueued on the context's stream, returns without waiting."""
-        self.ctx._check(self.L.vxb_mesh_closest_point_device(self.h, max_distance, None if points_ptr is None else C.c_void_p(points_ptr),
-                                                             count, None if hits_ptr is None else C.c_void_p(hits_ptr)),
+        self.ctx._check(self.L.vxb_mesh_closest_point_device(self.h, max_distance, _dev(points_ptr), count, _dev(hits_ptr)),
                         "vxb_mesh_closest_point_device")
 
     def capsule_cast_rc(self, sweeps, hits=None, count=None):
         """vxb_mesh_capsule_cast's return code for a CAPSULE_SWEEP_DTYPE array (or None for a NULL pointer); the hits go to
         `hits` (a CAPSULE_HIT_DTYPE array, or None for a NULL pointer); `count` defaults to len(sweeps)."""
-        sweeps = np.ascontiguousarray(sweeps, CAPSULE_SWEEP_DTYPE) if sweeps is not None else None
+        sweeps = _batch(sweeps, CAPSULE_SWEEP_DTYPE)
         n = (0 if sweeps is None else len(sweeps)) if count is None else count
         return self.L.vxb_mesh_capsule_cast(self.h, _ptr(sweeps), n, _ptr(hits))
 
@@ -720,19 +724,19 @@ class Mesh:
         array (make_capsule_sweeps), OUTPUT (Y-up) coordinates.  Returns a CAPSULE_HIT_DTYPE array."""
         sweeps = np.ascontiguousarray(sweeps, CAPSULE_SWEEP_DTYPE)
         hits = np.zeros(len(sweeps), CAPSULE_HIT_DTYPE)
-        self.ctx._check(self.L.vxb_mesh_capsule_cast(self.h, _ptr(sweeps), len(sweeps), _ptr(hits)), "vxb_mesh_capsule_cast")
+        self.ctx._check(self.capsule_cast_rc(sweeps, hits), "vxb_mesh_capsule_cast")
         return hits
 
     def capsule_cast_device(self, sweeps_ptr, count, hits_ptr):
         """vxb_mesh_capsule_cast_device: `count` vxb_capsule_sweep at the device address `sweeps_ptr`, hits to `hits_ptr`;
         enqueued on the context's stream, returns without waiting."""
-        self.ctx._check(self.L.vxb_mesh_capsule_cast_device(self.h, None if sweeps_ptr is None else C.c_void_p(sweeps_ptr), count,
-                                                            None if hits_ptr is None else C.c_void_p(hits_ptr)), "vxb_mesh_capsule_cast_device")
+        self.ctx._check(self.L.vxb_mesh_capsule_cast_device(self.h, _dev(sweeps_ptr), count, _dev(hits_ptr)),
+                        "vxb_mesh_capsule_cast_device")
 
     def closest_to_segment_rc(self, max_distance, segments, hits=None, count=None):
         """vxb_mesh_closest_to_segment's return code for a SEGMENT_DTYPE array (or None for a NULL pointer); the hits go to
         `hits` (a SEGMENT_HIT_DTYPE array, or None for a NULL pointer); `count` defaults to len(segments)."""
-        segments = np.ascontiguousarray(segments, SEGMENT_DTYPE) if segments is not None else None
+        segments = _batch(segments, SEGMENT_DTYPE)
         n = (0 if segments is None else len(segments)) if count is None else count
         return self.L.vxb_mesh_closest_to_segment(self.h, max_distance, _ptr(segments), n, _ptr(hits))
 
@@ -741,23 +745,20 @@ class Mesh:
         OUTPUT, Y-up coordinates), vxb_mesh_closest_to_segment.  Returns a SEGMENT_HIT_DTYPE array."""
         segments = np.ascontiguousarray(segments, SEGMENT_DTYPE)
         hits = np.zeros(len(segments), SEGMENT_HIT_DTYPE)
-        self.ctx._check(self.L.vxb_mesh_closest_to_segment(self.h, max_distance, _ptr(segments), len(segments), _ptr(hits)),
-                        "vxb_mesh_closest_to_segment")
+        self.ctx._check(self.closest_to_segment_rc(max_distance, segments, hits), "vxb_mesh_closest_to_segment")
         return hits
 
     def closest_to_segment_device(self, max_distance, segments_ptr, count, hits_ptr):
         """vxb_mesh_closest_to_segment_device: `count` vxb_segment at the device address `segments_ptr`, hits to `hits_ptr`;
         enqueued on the context's stream, returns without waiting."""
-        self.ctx._check(self.L.vxb_mesh_closest_to_segment_device(self.h, max_distance,
-                                                                  None if segments_ptr is None else C.c_void_p(segments_ptr), count,
-                                                                  None if hits_ptr is None else C.c_void_p(hits_ptr)),
+        self.ctx._check(self.L.vxb_mesh_closest_to_segment_device(self.h, max_distance, _dev(segments_ptr), count, _dev(hits_ptr)),
                         "vxb_mesh_closest_to_segment_device")
 
     def overlap_boxes_rc(self, boxes, offsets, tris=None, capacity=None, count=None):
         """vxb_mesh_overlap_box's return code for a BOX_DTYPE array (or None for a NULL pointer): offsets to `offsets` (a uint64
         array of count + 1, or None), triangles to `tris` (an OVERLAP_TRIANGLE_DTYPE array, or None for a NULL pointer);
         `capacity` defaults to len(tris) (0 without), `count` to len(boxes)."""
-        boxes = np.ascontiguousarray(boxes, BOX_DTYPE) if boxes is not None else None
+        boxes = _batch(boxes, BOX_DTYPE)
         n = (0 if boxes is None else len(boxes)) if count is None else count
         cap = (0 if tris is None else len(tris)) if capacity is None else capacity
         return self.L.vxb_mesh_overlap_box(self.h, _ptr(boxes), n, _ptr(offsets), _ptr(tris), cap)
@@ -777,9 +778,7 @@ class Mesh:
         """vxb_mesh_overlap_box_device: `count` vxb_box at the device address `boxes_ptr`, count + 1 uint64 offsets to
         `offsets_ptr`, at most `capacity` triangles to `tris_ptr` (None: count only); enqueued on the context's stream, returns
         without waiting."""
-        self.ctx._check(self.L.vxb_mesh_overlap_box_device(self.h, None if boxes_ptr is None else C.c_void_p(boxes_ptr), count,
-                                                           None if offsets_ptr is None else C.c_void_p(offsets_ptr),
-                                                           None if tris_ptr is None else C.c_void_p(tris_ptr), capacity),
+        self.ctx._check(self.L.vxb_mesh_overlap_box_device(self.h, _dev(boxes_ptr), count, _dev(offsets_ptr), _dev(tris_ptr), capacity),
                         "vxb_mesh_overlap_box_device")
 
 

@@ -2219,33 +2219,26 @@ struct vxb_mesh
 	uint64_t serial = 0;                        // vxb_context::runSerial of that run
 	uint32_t n = 0;
 	vxb_mesh_info info;
-	// ray casts (vxb_ray.cuh): the level-0 coord_id -> slot map, built for the applied run `mapSerial` on a grid of `mapN`
-	DevBuf<unsigned int> rayMap;
-	bool mapBuilt = false;
-	uint64_t mapSerial = 0;
-	uint32_t mapN = 0;
-	DevBuf<vxb_ray> rayIn;                      // the host variants' device staging (rays and sweeps), grown as needed
-	DevBuf<vxb_ray_hit> rayOut;
-	DevBuf<vxb_sphere_hit> sphereOut;
-	DevBuf<float> pointIn;                      // 3 floats per closest-point query
-	DevBuf<vxb_closest_hit> closestOut;
-	DevBuf<vxb_capsule_sweep> capsuleIn;
-	DevBuf<vxb_capsule_hit> capsuleOut;
-	DevBuf<vxb_segment> segmentIn;
-	DevBuf<vxb_segment_hit> segmentOut;
-	// cut ray casts (vxb_cutray.cuh): the all-level map (bounds slot -> directory slot) and the excursion, measured for the
-	// applied run `cutSerial` on a grid of `cutN`; separate from rayMap, so the level-0 queries never see them
-	DevBuf<unsigned int> cutMap, cutExcursion;
-	bool cutBuilt = false;
-	uint64_t cutSerial = 0;
-	uint32_t cutN = 0;
+	// A map built lazily for one applied run (`serial`) on one grid (`n`); every apply has a new serial.
+	struct LazyMap
+	{
+		DevBuf<unsigned int> buf;
+		bool built = false;
+		uint64_t serial = 0;
+		uint32_t n = 0;
+	};
+	// ray casts and the other level-0 queries (vxb_ray.cuh): the level-0 coord_id -> slot map
+	LazyMap rayMap;
+	// cut ray casts (vxb_cutray.cuh): the all-level map (bounds slot -> directory slot) and the excursion measured with it;
+	// separate from rayMap, so the level-0 queries never see them
+	LazyMap cutMap;
+	DevBuf<unsigned int> cutExcursion;
 	float excursion = 0.f;
-	DevBuf<vxb_cut_hit> cutOut;
-	// box overlap gathers (vxb_overlap.cuh): the per-box counts and the scan's storage, the host variant's staging
+	// the host variants' device staging of queries and hits, shared by every query and grown as needed
+	DevBuf<unsigned char> stageIn, stageOut;
+	// box overlap gathers (vxb_overlap.cuh): the per-box counts and the scan's storage, the host variant's offsets
 	DevBuf<uint64_t> overlapCounts, overlapOffsets;
 	DevBuf<unsigned char> overlapTemp;
-	DevBuf<vxb_box> boxIn;
-	DevBuf<vxb_overlap_triangle> overlapOut;
 };
 
 namespace
@@ -2258,34 +2251,44 @@ void deleteMesh(vxb_mesh* m)
 
 uint64_t grownCapacity(uint64_t live) { return (std::max<uint64_t>(live + live / 2, 1024) + 3) & ~(uint64_t)3; }
 
-// The level-0 map for the applied run (rebuilt after every apply: each one has a new serial), queued on ctx->stream, and the
-// kernels' view of the mesh.
-int ensureMap(vxb_mesh* m, VxbRayMesh& rm)
+// Whether `map` was built for another applied run or grid.  If so, it is readied on ctx->stream for its rebuild: grown to
+// `entries` (a query still queued may read the old map, so the stream drains first) and filled with VXB_RAY_MISS.
+int staleMap(vxb_mesh* m, vxb_mesh::LazyMap& map, size_t entries, bool& stale)
 {
 	vxb_context* ctx = m->ctx;
-	cudaStream_t st = ctx->stream;
-	const uint32_t nb = m->n / 16;
-	if (!m->mapBuilt || m->mapSerial != m->serial || m->mapN != m->n)
+	stale = !map.built || map.serial != m->serial || map.n != m->n;
+	if (!stale) return VXB_OK;
+	if (entries > map.buf.count)
 	{
-		const size_t cells = (size_t)nb * nb * nb;
-		if (cells > m->rayMap.count)
-		{
-			VXB_CUDA(ctx, cudaStreamSynchronize(st)); // a query still queued may read the old map
-			VXB_CUDA(ctx, m->rayMap.ensure(cells));
-		}
-		VXB_CUDA(ctx, cudaMemsetAsync(m->rayMap.p, 0xFF, cells * sizeof(unsigned int), st));
-		const unsigned level0 = m->info.level_blocks[0];
-		if (level0) vxb_ray_map_kernel<<<(level0 + 255) / 256, 256, 0, st>>>(m->dir.p, level0, m->rayMap.p);
-		VXB_CUDA(ctx, cudaGetLastError());
-		m->mapBuilt = true; m->mapSerial = m->serial; m->mapN = m->n;
+		VXB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+		VXB_CUDA(ctx, map.buf.ensure(entries));
 	}
-	rm.dir = m->dir.p; rm.map = m->rayMap.p; rm.verts = m->set[m->active].v.p; rm.idx = m->set[m->active].i.p; rm.nb = (int)nb;
+	VXB_CUDA(ctx, cudaMemsetAsync(map.buf.p, 0xFF, entries * sizeof(unsigned int), ctx->stream));
 	return VXB_OK;
 }
 
-// The all-level map and the excursion for the applied run (rebuilt after every apply), queued on ctx->stream; the excursion
-// is read back, so a rebuild waits for the stream once.  Then the refusal of an excursion beyond the walk's reach, and the
-// kernel's view of the mesh.
+void markBuilt(const vxb_mesh* m, vxb_mesh::LazyMap& map) { map.built = true; map.serial = m->serial; map.n = m->n; }
+
+// The level-0 map for the applied run, queued on ctx->stream, and the kernels' view of the mesh.
+int ensureMap(vxb_mesh* m, VxbRayMesh& rm)
+{
+	const uint32_t nb = m->n / 16;
+	bool stale;
+	const int e = staleMap(m, m->rayMap, (size_t)nb * nb * nb, stale);
+	if (e != VXB_OK) return e;
+	if (stale)
+	{
+		const unsigned level0 = m->info.level_blocks[0];
+		if (level0) vxb_ray_map_kernel<<<(level0 + 255) / 256, 256, 0, m->ctx->stream>>>(m->dir.p, level0, m->rayMap.buf.p);
+		VXB_CUDA(m->ctx, cudaGetLastError());
+		markBuilt(m, m->rayMap);
+	}
+	rm.dir = m->dir.p; rm.map = m->rayMap.buf.p; rm.verts = m->set[m->active].v.p; rm.idx = m->set[m->active].i.p; rm.nb = (int)nb;
+	return VXB_OK;
+}
+
+// The all-level map and the excursion for the applied run, queued on ctx->stream; the excursion is read back, so a rebuild
+// waits for the stream once.  Then the refusal of an excursion beyond the walk's reach, and the kernel's view of the mesh.
 int ensureCutMap(vxb_mesh* m, const char* what, VxbCutRayMesh& c)
 {
 	vxb_context* ctx = m->ctx;
@@ -2294,25 +2297,21 @@ int ensureCutMap(vxb_mesh* m, const char* what, VxbCutRayMesh& c)
 	VxbCutMapArgs a;
 	for (int l = 0; l < VXB_MAX_LEVELS; ++l) a.levelBase[l] = m->bounds.level_base[l];
 	a.nb = (int)nb;
-	if (!m->cutBuilt || m->cutSerial != m->serial || m->cutN != m->n)
+	bool stale;
+	const int e = staleMap(m, m->cutMap, m->bounds.slots, stale);
+	if (e != VXB_OK) return e;
+	if (stale)
 	{
-		const size_t slots = m->bounds.slots;
-		if (slots > m->cutMap.count)
-		{
-			VXB_CUDA(ctx, cudaStreamSynchronize(st)); // a query still queued may read the old map
-			VXB_CUDA(ctx, m->cutMap.ensure(slots));
-		}
 		VXB_CUDA(ctx, m->cutExcursion.ensure(1));
-		VXB_CUDA(ctx, cudaMemsetAsync(m->cutMap.p, 0xFF, slots * sizeof(unsigned int), st));
 		VXB_CUDA(ctx, cudaMemsetAsync(m->cutExcursion.p, 0, sizeof(unsigned int), st));
 		const unsigned blocks = m->info.block_count;
-		if (blocks) vxb_cutray_map_kernel<<<(blocks + 255) / 256, 256, 0, st>>>(m->dir.p, blocks, a, m->boxes.p, m->cutMap.p, m->cutExcursion.p);
+		if (blocks) vxb_cutray_map_kernel<<<(blocks + 255) / 256, 256, 0, st>>>(m->dir.p, blocks, a, m->boxes.p, m->cutMap.buf.p, m->cutExcursion.p);
 		VXB_CUDA(ctx, cudaGetLastError());
 		unsigned bits = 0;
 		VXB_CUDA(ctx, cudaMemcpyAsync(&bits, m->cutExcursion.p, sizeof(bits), cudaMemcpyDeviceToHost, st));
 		VXB_CUDA(ctx, cudaStreamSynchronize(st));
 		memcpy(&m->excursion, &bits, sizeof(bits));
-		m->cutBuilt = true; m->cutSerial = m->serial; m->cutN = m->n;
+		markBuilt(m, m->cutMap);
 	}
 	if (!(m->excursion + VXB_RAY_EPS <= 15.f))
 	{
@@ -2320,7 +2319,7 @@ int ensureCutMap(vxb_mesh* m, const char* what, VxbCutRayMesh& c)
 		snprintf(buf, sizeof(buf), "%s: a block's vertices leave its lattice box by %g voxels; the walk reaches 15 - 1/16", what, (double)m->excursion);
 		return fail(ctx, VXB_ERR_STATE, buf);
 	}
-	c.m.dir = m->dir.p; c.m.map = m->cutMap.p; c.m.verts = m->set[m->active].v.p; c.m.idx = m->set[m->active].i.p; c.m.nb = (int)nb;
+	c.m.dir = m->dir.p; c.m.map = m->cutMap.buf.p; c.m.verts = m->set[m->active].v.p; c.m.idx = m->set[m->active].i.p; c.m.nb = (int)nb;
 	c.tverts = m->set[m->active].tv.p; c.tidx = m->set[m->active].ti.p;
 	c.boxes = m->boxes.p;
 	c.slots = a;
@@ -2337,12 +2336,14 @@ unsigned queryCtas(const vxb_context* ctx, uint32_t count, unsigned threads)
 	return std::min<unsigned>((count + warpsPerCta - 1) / warpsPerCta, (unsigned)std::max(ctx->smCount, 1) * 8);
 }
 
-int enqueueRaycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits)
+// A level-0 query's launch on ctx->stream: `kernel(rm, args...)`, one warp per query over the level-0 map (ensureMap).
+template <class Kernel, class... Args>
+int launchLevel0(vxb_mesh* m, Kernel kernel, unsigned threads, uint32_t count, Args... args)
 {
 	VxbRayMesh rm;
 	const int e = ensureMap(m, rm);
 	if (e != VXB_OK) return e;
-	vxb_raycast_kernel<<<queryCtas(m->ctx, count, VXB_RAY_THREADS), VXB_RAY_THREADS, 0, m->ctx->stream>>>(rm, rays, count, hits);
+	kernel<<<queryCtas(m->ctx, count, threads), threads, 0, m->ctx->stream>>>(rm, args...);
 	VXB_CUDA(m->ctx, cudaGetLastError());
 	return VXB_OK;
 }
@@ -2355,46 +2356,6 @@ int enqueueRaycastCut(vxb_mesh* m, const char* what, const float camera[3], floa
 	for (int k = 0; k < 3; ++k) c.cut.camera[k] = camera[k];
 	c.cut.lod = lodFactor;
 	vxb_raycast_cut_kernel<<<queryCtas(m->ctx, count, VXB_RAY_THREADS), VXB_RAY_THREADS, 0, m->ctx->stream>>>(c, rays, count, hits);
-	VXB_CUDA(m->ctx, cudaGetLastError());
-	return VXB_OK;
-}
-
-int enqueueSphereCast(vxb_mesh* m, float radius, const vxb_ray* rays, uint32_t count, vxb_sphere_hit* hits)
-{
-	VxbRayMesh rm;
-	const int e = ensureMap(m, rm);
-	if (e != VXB_OK) return e;
-	vxb_sphere_cast_kernel<<<queryCtas(m->ctx, count, VXB_COLLIDE_THREADS), VXB_COLLIDE_THREADS, 0, m->ctx->stream>>>(rm, radius, rays, count, hits);
-	VXB_CUDA(m->ctx, cudaGetLastError());
-	return VXB_OK;
-}
-
-int enqueueClosestPoint(vxb_mesh* m, float maxDistance, const float* points, uint32_t count, vxb_closest_hit* hits)
-{
-	VxbRayMesh rm;
-	const int e = ensureMap(m, rm);
-	if (e != VXB_OK) return e;
-	vxb_closest_point_kernel<<<queryCtas(m->ctx, count, VXB_COLLIDE_THREADS), VXB_COLLIDE_THREADS, 0, m->ctx->stream>>>(rm, maxDistance, points, count, hits);
-	VXB_CUDA(m->ctx, cudaGetLastError());
-	return VXB_OK;
-}
-
-int enqueueCapsuleCast(vxb_mesh* m, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits)
-{
-	VxbRayMesh rm;
-	const int e = ensureMap(m, rm);
-	if (e != VXB_OK) return e;
-	vxb_capsule_cast_kernel<<<queryCtas(m->ctx, count, VXB_COLLIDE_THREADS), VXB_COLLIDE_THREADS, 0, m->ctx->stream>>>(rm, sweeps, count, hits);
-	VXB_CUDA(m->ctx, cudaGetLastError());
-	return VXB_OK;
-}
-
-int enqueueClosestSegment(vxb_mesh* m, float maxDistance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits)
-{
-	VxbRayMesh rm;
-	const int e = ensureMap(m, rm);
-	if (e != VXB_OK) return e;
-	vxb_closest_segment_kernel<<<queryCtas(m->ctx, count, VXB_COLLIDE_THREADS), VXB_COLLIDE_THREADS, 0, m->ctx->stream>>>(rm, maxDistance, segments, count, hits);
 	VXB_CUDA(m->ctx, cudaGetLastError());
 	return VXB_OK;
 }
@@ -2438,72 +2399,94 @@ int enqueueOverlap(vxb_mesh* m, const vxb_box* boxes, uint32_t count, uint64_t* 
 	return VXB_OK;
 }
 
-// the host variant's box rule (include/vxb200.h "box overlap gathers"): the index of the first invalid box, or -1
-long long invalidBox(const vxb_box* boxes, uint32_t count)
-{
-	for (uint32_t q = 0; q < count; ++q)
-		for (int i = 0; i < 3; ++i)
-			if (!std::isfinite(boxes[q].min[i]) || !std::isfinite(boxes[q].max[i]) || !(boxes[q].min[i] <= boxes[q].max[i])) return q;
-	return -1;
-}
-
-// the reach rule of the capsule queries (include/vxb200.h), in float as the kernels evaluate it: a finite half axis and
-// max_i |h_i| + extra <= 15
-bool capsuleReach(const float h[3], float extra)
-{
-	if (!std::isfinite(h[0]) || !std::isfinite(h[1]) || !std::isfinite(h[2])) return false;
-	const float hm = std::max(std::max(std::fabs(h[0]), std::fabs(h[1])), std::fabs(h[2]));
-	const float reach = hm + extra;
-	return reach <= VXB_SPHERE_RADIUS_MAX;
-}
-
-// the batch arguments of the collision queries (include/vxb200.h): 0 < radius <= 15, 0 <= max_distance <= 15; NaN fails
-bool validRadius(float r) { return r > 0.f && r <= VXB_SPHERE_RADIUS_MAX; }
-bool validMaxDistance(float d) { return d >= 0.f && d <= VXB_SPHERE_RADIUS_MAX; }
-
-// the index of the first query point with a non-finite coordinate, or -1
-long long invalidPoint(const float* points, uint32_t count)
-{
-	for (uint32_t q = 0; q < count; ++q)
-		if (!std::isfinite(points[3 * q]) || !std::isfinite(points[3 * q + 1]) || !std::isfinite(points[3 * q + 2])) return q;
-	return -1;
-}
-
-// A host variant's round trip on ctx->stream: queries to the staging `in`, the enqueued query, hits back; blocks.
+// A host variant's round trip on ctx->stream: `inBytes` of queries to the staging, the enqueued query, `count` hits back;
+// blocks.
 template <class In, class Out, class Enqueue>
-int hostQuery(vxb_mesh* m, DevBuf<In>& in, size_t inPerQuery, DevBuf<Out>& out, const In* queries, uint32_t count, Out* hits, Enqueue&& enqueue)
+int hostQuery(vxb_mesh* m, const In* queries, size_t inBytes, uint32_t count, Out* hits, Enqueue&& enqueue)
 {
 	vxb_context* ctx = m->ctx;
-	cudaSetDevice(ctx->device);
 	cudaStream_t st = ctx->stream;
-	if (count * inPerQuery > in.count || count > out.count)
+	const size_t outBytes = sizeof(Out) * count;
+	if (inBytes > m->stageIn.count || outBytes > m->stageOut.count)
 	{
 		VXB_CUDA(ctx, cudaStreamSynchronize(st)); // nothing queued may still use the staging being replaced
-		VXB_CUDA(ctx, in.ensure(count * inPerQuery)); VXB_CUDA(ctx, out.ensure(count));
+		VXB_CUDA(ctx, m->stageIn.ensure(inBytes)); VXB_CUDA(ctx, m->stageOut.ensure(outBytes));
 	}
-	VXB_CUDA(ctx, cudaMemcpyAsync(in.p, queries, sizeof(In) * inPerQuery * count, cudaMemcpyHostToDevice, st));
-	const int r = enqueue(in.p, out.p);
+	VXB_CUDA(ctx, cudaMemcpyAsync(m->stageIn.p, queries, inBytes, cudaMemcpyHostToDevice, st));
+	const int r = enqueue((const In*)m->stageIn.p, (Out*)m->stageOut.p);
 	if (r != VXB_OK) return r;
-	VXB_CUDA(ctx, cudaMemcpyAsync(hits, out.p, sizeof(Out) * count, cudaMemcpyDeviceToHost, st));
+	VXB_CUDA(ctx, cudaMemcpyAsync(hits, m->stageOut.p, outBytes, cudaMemcpyDeviceToHost, st));
 	VXB_CUDA(ctx, cudaStreamSynchronize(st));
 	return VXB_OK;
 }
 
-// the host variant's argument rule (include/vxb200.h): the index of the first invalid ray, or -1
-long long invalidRay(const vxb_ray* rays, uint32_t count, const char** why)
+// the batch arguments of the queries (include/vxb200.h): why one is refused, or NULL.  NaN fails.
+const char* radiusFault(float r) { return r > 0.f && r <= VXB_SPHERE_RADIUS_MAX ? nullptr : "radius must be in (0, 15]"; }
+const char* maxDistanceFault(float d) { return d >= 0.f && d <= VXB_SPHERE_RADIUS_MAX ? nullptr : "max_distance must be in [0, 15]"; }
+const char* cutFault(const float camera[3], float lodFactor)
 {
-	for (uint32_t r = 0; r < count; ++r)
+	if (!std::isfinite(lodFactor) || !(lodFactor >= VXB_LOD_FACTOR_MIN)) return "lod_factor must be finite and >= 2";
+	if (camera && (!std::isfinite(camera[0]) || !std::isfinite(camera[1]) || !std::isfinite(camera[2]))) return "non-finite lod_camera component";
+	return nullptr;
+}
+
+// the host variants' ray rule (include/vxb200.h): why the ray is refused, or NULL
+const char* rayFault(const vxb_ray& x)
+{
+	bool finite = true;
+	for (int a = 0; a < 3; ++a) finite = finite && std::isfinite(x.origin[a]) && std::isfinite(x.direction[a]);
+	if (!finite) return "non-finite origin or direction";
+	if (x.direction[0] == 0.f && x.direction[1] == 0.f && x.direction[2] == 0.f) return "zero direction";
+	if (!std::isfinite(x.t_min)) return "t_min is NaN or infinite";
+	if (std::isnan(x.t_max)) return "t_max is NaN";
+	if (x.t_min > x.t_max) return "t_min > t_max";
+	return nullptr;
+}
+
+// A host variant's per-query rule: fault(i) is why query i is refused, or NULL; `noun` names the query in the refusal.  A
+// device variant has none (noun NULL): its queries are in device memory, and the kernels answer an invalid one with a miss.
+template <class Fault> struct Rule { const char* noun; Fault fault; };
+template <class Fault> Rule<Fault> rule(const char* noun, Fault fault) { return { noun, fault }; }
+const Rule<const char* (*)(uint32_t)> deviceRule = { nullptr, nullptr };
+
+// What a query entry checks before its rule (include/vxb200.h)
+struct Entry
+{
+	const char* name;      // the entry point, which starts every message
+	bool null;             // a pointer the call needs when count > 0 is NULL, of ...
+	const char* pointers;  // ... these, as the message names them
+	const char* batch;     // why a batch argument is refused, or NULL
+	bool levels = false;   // the query reads every level and transition mesh: the mesh must be complete
+};
+
+// Every query entry's path, its checks in one order: a NULL pointer (only when count > 0), the batch arguments, nothing
+// applied, an incomplete mesh, count == 0 (VXB_OK), the host variant's per-query rule; then `run`, the staging round trip or
+// the direct enqueue, on the context's device.  Every argument check comes before every state check.
+template <class Fault, class Run>
+int meshQuery(vxb_mesh* m, const Entry& q, uint32_t count, const Rule<Fault>& rule, Run&& run)
+{
+	if (!m) return VXB_ERR_ARGUMENT;
+	vxb_context* ctx = m->ctx;
+	char buf[256];
+	if (count && q.null) { snprintf(buf, sizeof(buf), "%s: NULL %s", q.name, q.pointers); return fail(ctx, VXB_ERR_ARGUMENT, buf); }
+	if (q.batch) { snprintf(buf, sizeof(buf), "%s: %s", q.name, q.batch); return fail(ctx, VXB_ERR_ARGUMENT, buf); }
+	if (!m->content) { snprintf(buf, sizeof(buf), "%s: nothing applied yet", q.name); return fail(ctx, VXB_ERR_STATE, buf); }
+	if (q.levels && !m->complete)
 	{
-		const vxb_ray& x = rays[r];
-		bool finite = true;
-		for (int a = 0; a < 3; ++a) finite = finite && std::isfinite(x.origin[a]) && std::isfinite(x.direction[a]);
-		if (!finite) { *why = "non-finite origin or direction"; return r; }
-		if (x.direction[0] == 0.f && x.direction[1] == 0.f && x.direction[2] == 0.f) { *why = "zero direction"; return r; }
-		if (!std::isfinite(x.t_min)) { *why = "t_min is NaN or infinite"; return r; }
-		if (std::isnan(x.t_max)) { *why = "t_max is NaN"; return r; }
-		if (x.t_min > x.t_max) { *why = "t_min > t_max"; return r; }
+		snprintf(buf, sizeof(buf), "%s: the mesh lacks levels or transition meshes (a run since the last full apply had max_levels "
+			"below the grid's levels or VXB_FLAG_NO_TRANSITIONS)", q.name);
+		return fail(ctx, VXB_ERR_STATE, buf);
 	}
-	return -1;
+	if (!count) return VXB_OK;
+	if (rule.noun)
+		for (uint32_t i = 0; i < count; ++i)
+			if (const char* why = rule.fault(i))
+			{
+				snprintf(buf, sizeof(buf), "%s: %s %u: %s", q.name, rule.noun, i, why);
+				return fail(ctx, VXB_ERR_ARGUMENT, buf);
+			}
+	cudaSetDevice(ctx->device);
+	return run();
 }
 
 // The culled selects' shared body, after the caller's NULL, view-count and state checks: the plane check (a refusal names the
@@ -2873,286 +2856,159 @@ int vxb_mesh_select_cut(vxb_mesh* m, const float camera[3], float lodFactor, con
 
 int vxb_mesh_raycast(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (count && (!rays || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_raycast: NULL rays or hits");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_raycast: nothing applied yet");
-	if (!count) return VXB_OK;
-	const char* why = "";
-	const long long bad = invalidRay(rays, count, &why);
-	if (bad >= 0)
-	{
-		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_raycast: ray %lld: %s", bad, why);
-		return fail(ctx, VXB_ERR_ARGUMENT, buf);
-	}
-	return hostQuery(m, m->rayIn, 1, m->rayOut, rays, count, hits,
-		[&](const vxb_ray* in, vxb_ray_hit* out) { return enqueueRaycast(m, in, count, out); });
+	return meshQuery(m, { "vxb_mesh_raycast", !rays || !hits, "rays or hits", nullptr }, count,
+		rule("ray", [=](uint32_t i) { return rayFault(rays[i]); }), [&] {
+			return hostQuery(m, rays, sizeof(vxb_ray) * count, count, hits, [&](const vxb_ray* in, vxb_ray_hit* out) {
+				return launchLevel0(m, vxb_raycast_kernel, VXB_RAY_THREADS, count, in, count, out); }); });
 }
 
 int vxb_mesh_raycast_device(vxb_mesh* m, const vxb_ray* rays, uint32_t count, vxb_ray_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (count && (!rays || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_raycast_device: NULL rays or hits");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_raycast_device: nothing applied yet");
-	if (!count) return VXB_OK;
-	cudaSetDevice(ctx->device);
-	return enqueueRaycast(m, rays, count, hits);
+	return meshQuery(m, { "vxb_mesh_raycast_device", !rays || !hits, "rays or hits", nullptr }, count, deviceRule,
+		[&] { return launchLevel0(m, vxb_raycast_kernel, VXB_RAY_THREADS, count, rays, count, hits); });
 }
-
-} // extern "C"
-
-namespace
-{
-// the checks of the cut casts (include/vxb200.h "ray queries against the drawn LOD cut"): vxb_mesh_raycast's NULL rule,
-// vxb_mesh_select_cut's lod_factor, lod_camera and state rules
-int cutCastChecks(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, const vxb_ray* rays, uint32_t count, const vxb_cut_hit* hits)
-{
-	vxb_context* ctx = m->ctx;
-	char buf[192];
-	if (count && (!camera || !rays || !hits)) { snprintf(buf, sizeof(buf), "%s: NULL lod_camera, rays or hits", what); return fail(ctx, VXB_ERR_ARGUMENT, buf); }
-	if (!std::isfinite(lodFactor) || !(lodFactor >= VXB_LOD_FACTOR_MIN))
-	{
-		snprintf(buf, sizeof(buf), "%s: lod_factor must be finite and >= 2", what);
-		return fail(ctx, VXB_ERR_ARGUMENT, buf);
-	}
-	if (camera && (!std::isfinite(camera[0]) || !std::isfinite(camera[1]) || !std::isfinite(camera[2])))
-	{
-		snprintf(buf, sizeof(buf), "%s: non-finite lod_camera component", what);
-		return fail(ctx, VXB_ERR_ARGUMENT, buf);
-	}
-	if (!m->content) { snprintf(buf, sizeof(buf), "%s: nothing applied yet", what); return fail(ctx, VXB_ERR_STATE, buf); }
-	if (!m->complete)
-	{
-		snprintf(buf, sizeof(buf), "%s: the mesh lacks levels or transition meshes (a run since the last full apply had max_levels "
-			"below the grid's levels or VXB_FLAG_NO_TRANSITIONS)", what);
-		return fail(ctx, VXB_ERR_STATE, buf);
-	}
-	return VXB_OK;
-}
-}
-
-extern "C"
-{
 
 int vxb_mesh_raycast_cut(vxb_mesh* m, const float camera[3], float lodFactor, const vxb_ray* rays, uint32_t count, vxb_cut_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	const int e = cutCastChecks(m, "vxb_mesh_raycast_cut", camera, lodFactor, rays, count, hits);
-	if (e != VXB_OK || !count) return e;
-	const char* why = "";
-	const long long bad = invalidRay(rays, count, &why);
-	if (bad >= 0)
-	{
-		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_raycast_cut: ray %lld: %s", bad, why);
-		return fail(m->ctx, VXB_ERR_ARGUMENT, buf);
-	}
-	return hostQuery(m, m->rayIn, 1, m->cutOut, rays, count, hits,
-		[&](const vxb_ray* in, vxb_cut_hit* out) { return enqueueRaycastCut(m, "vxb_mesh_raycast_cut", camera, lodFactor, in, count, out); });
+	const char* what = "vxb_mesh_raycast_cut";
+	return meshQuery(m, { what, !camera || !rays || !hits, "lod_camera, rays or hits", cutFault(camera, lodFactor), true }, count,
+		rule("ray", [=](uint32_t i) { return rayFault(rays[i]); }), [&] {
+			return hostQuery(m, rays, sizeof(vxb_ray) * count, count, hits, [&](const vxb_ray* in, vxb_cut_hit* out) {
+				return enqueueRaycastCut(m, what, camera, lodFactor, in, count, out); }); });
 }
 
 int vxb_mesh_raycast_cut_device(vxb_mesh* m, const float camera[3], float lodFactor, const vxb_ray* rays, uint32_t count, vxb_cut_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	const int e = cutCastChecks(m, "vxb_mesh_raycast_cut_device", camera, lodFactor, rays, count, hits);
-	if (e != VXB_OK || !count) return e;
-	cudaSetDevice(m->ctx->device);
-	return enqueueRaycastCut(m, "vxb_mesh_raycast_cut_device", camera, lodFactor, rays, count, hits);
+	const char* what = "vxb_mesh_raycast_cut_device";
+	return meshQuery(m, { what, !camera || !rays || !hits, "lod_camera, rays or hits", cutFault(camera, lodFactor), true }, count,
+		deviceRule, [&] { return enqueueRaycastCut(m, what, camera, lodFactor, rays, count, hits); });
 }
 
 int vxb_mesh_sphere_cast(vxb_mesh* m, float radius, const vxb_ray* rays, uint32_t count, vxb_sphere_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (!validRadius(radius)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_sphere_cast: radius must be in (0, 15]");
-	if (count && (!rays || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_sphere_cast: NULL rays or hits");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_sphere_cast: nothing applied yet");
-	if (!count) return VXB_OK;
-	const char* why = "";
-	const long long bad = invalidRay(rays, count, &why);
-	if (bad >= 0)
-	{
-		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_sphere_cast: sweep %lld: %s", bad, why);
-		return fail(ctx, VXB_ERR_ARGUMENT, buf);
-	}
-	return hostQuery(m, m->rayIn, 1, m->sphereOut, rays, count, hits,
-		[&](const vxb_ray* in, vxb_sphere_hit* out) { return enqueueSphereCast(m, radius, in, count, out); });
+	return meshQuery(m, { "vxb_mesh_sphere_cast", !rays || !hits, "rays or hits", radiusFault(radius) }, count,
+		rule("sweep", [=](uint32_t i) { return rayFault(rays[i]); }), [&] {
+			return hostQuery(m, rays, sizeof(vxb_ray) * count, count, hits, [&](const vxb_ray* in, vxb_sphere_hit* out) {
+				return launchLevel0(m, vxb_sphere_cast_kernel, VXB_COLLIDE_THREADS, count, radius, in, count, out); }); });
 }
 
 int vxb_mesh_sphere_cast_device(vxb_mesh* m, float radius, const vxb_ray* rays, uint32_t count, vxb_sphere_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (!validRadius(radius)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_sphere_cast_device: radius must be in (0, 15]");
-	if (count && (!rays || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_sphere_cast_device: NULL rays or hits");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_sphere_cast_device: nothing applied yet");
-	if (!count) return VXB_OK;
-	cudaSetDevice(ctx->device);
-	return enqueueSphereCast(m, radius, rays, count, hits);
+	return meshQuery(m, { "vxb_mesh_sphere_cast_device", !rays || !hits, "rays or hits", radiusFault(radius) }, count, deviceRule,
+		[&] { return launchLevel0(m, vxb_sphere_cast_kernel, VXB_COLLIDE_THREADS, count, radius, rays, count, hits); });
 }
 
 int vxb_mesh_closest_point(vxb_mesh* m, float maxDistance, const float* points, uint32_t count, vxb_closest_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (!validMaxDistance(maxDistance)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_point: max_distance must be in [0, 15]");
-	if (count && (!points || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_point: NULL points or hits");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_closest_point: nothing applied yet");
-	if (!count) return VXB_OK;
-	const long long bad = invalidPoint(points, count);
-	if (bad >= 0)
-	{
-		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_closest_point: point %lld: non-finite coordinate", bad);
-		return fail(ctx, VXB_ERR_ARGUMENT, buf);
-	}
-	return hostQuery(m, m->pointIn, 3, m->closestOut, points, count, hits,
-		[&](const float* in, vxb_closest_hit* out) { return enqueueClosestPoint(m, maxDistance, in, count, out); });
+	const auto pointFault = [=](uint32_t i) -> const char* {
+		const float* p = points + 3 * (size_t)i;
+		return std::isfinite(p[0]) && std::isfinite(p[1]) && std::isfinite(p[2]) ? nullptr : "non-finite coordinate";
+	};
+	return meshQuery(m, { "vxb_mesh_closest_point", !points || !hits, "points or hits", maxDistanceFault(maxDistance) }, count,
+		rule("point", pointFault), [&] {
+			return hostQuery(m, points, 3 * sizeof(float) * count, count, hits, [&](const float* in, vxb_closest_hit* out) {
+				return launchLevel0(m, vxb_closest_point_kernel, VXB_COLLIDE_THREADS, count, maxDistance, in, count, out); }); });
 }
 
 int vxb_mesh_closest_point_device(vxb_mesh* m, float maxDistance, const float* points, uint32_t count, vxb_closest_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (!validMaxDistance(maxDistance)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_point_device: max_distance must be in [0, 15]");
-	if (count && (!points || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_point_device: NULL points or hits");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_closest_point_device: nothing applied yet");
-	if (!count) return VXB_OK;
-	cudaSetDevice(ctx->device);
-	return enqueueClosestPoint(m, maxDistance, points, count, hits);
+	return meshQuery(m, { "vxb_mesh_closest_point_device", !points || !hits, "points or hits", maxDistanceFault(maxDistance) }, count,
+		deviceRule, [&] { return launchLevel0(m, vxb_closest_point_kernel, VXB_COLLIDE_THREADS, count, maxDistance, points, count, hits); });
 }
 
 int vxb_mesh_capsule_cast(vxb_mesh* m, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (count && (!sweeps || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_capsule_cast: NULL sweeps or hits");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_capsule_cast: nothing applied yet");
-	if (!count) return VXB_OK;
-	for (uint32_t q = 0; q < count; ++q)
-	{
-		const char* why = nullptr;
-		const float r = sweeps[q].radius;
-		invalidRay(&sweeps[q].path, 1, &why);
-		if (!why && !(r > 0.f)) why = "radius must be > 0";
-		if (!why && !capsuleReach(sweeps[q].half_axis, r)) why = "non-finite half axis or radius, or max |half_axis| + radius above 15";
-		if (why)
-		{
-			char buf[192]; snprintf(buf, sizeof(buf), "vxb_mesh_capsule_cast: sweep %u: %s", q, why);
-			return fail(ctx, VXB_ERR_ARGUMENT, buf);
-		}
-	}
-	return hostQuery(m, m->capsuleIn, 1, m->capsuleOut, sweeps, count, hits,
-		[&](const vxb_capsule_sweep* in, vxb_capsule_hit* out) { return enqueueCapsuleCast(m, in, count, out); });
+	const auto sweepFault = [=](uint32_t i) -> const char* {
+		const vxb_capsule_sweep& s = sweeps[i];
+		if (const char* why = rayFault(s.path)) return why;
+		if (!(s.radius > 0.f)) return "radius must be > 0";
+		if (!vxb_capsule_reach(make_float3(s.half_axis[0], s.half_axis[1], s.half_axis[2]), s.radius))
+			return "non-finite half axis or radius, or max |half_axis| + radius above 15";
+		return nullptr;
+	};
+	return meshQuery(m, { "vxb_mesh_capsule_cast", !sweeps || !hits, "sweeps or hits", nullptr }, count, rule("sweep", sweepFault), [&] {
+		return hostQuery(m, sweeps, sizeof(vxb_capsule_sweep) * count, count, hits, [&](const vxb_capsule_sweep* in, vxb_capsule_hit* out) {
+			return launchLevel0(m, vxb_capsule_cast_kernel, VXB_COLLIDE_THREADS, count, in, count, out); }); });
 }
 
 int vxb_mesh_capsule_cast_device(vxb_mesh* m, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (count && (!sweeps || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_capsule_cast_device: NULL sweeps or hits");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_capsule_cast_device: nothing applied yet");
-	if (!count) return VXB_OK;
-	cudaSetDevice(ctx->device);
-	return enqueueCapsuleCast(m, sweeps, count, hits);
+	return meshQuery(m, { "vxb_mesh_capsule_cast_device", !sweeps || !hits, "sweeps or hits", nullptr }, count, deviceRule,
+		[&] { return launchLevel0(m, vxb_capsule_cast_kernel, VXB_COLLIDE_THREADS, count, sweeps, count, hits); });
 }
 
 int vxb_mesh_closest_to_segment(vxb_mesh* m, float maxDistance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (!validMaxDistance(maxDistance)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_to_segment: max_distance must be in [0, 15]");
-	if (count && (!segments || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_to_segment: NULL segments or hits");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_closest_to_segment: nothing applied yet");
-	if (!count) return VXB_OK;
-	for (uint32_t q = 0; q < count; ++q)
-	{
-		const char* why = nullptr;
-		const float* c = segments[q].center;
-		if (!std::isfinite(c[0]) || !std::isfinite(c[1]) || !std::isfinite(c[2])) why = "non-finite centre";
-		else if (!capsuleReach(segments[q].half_axis, maxDistance)) why = "non-finite half axis, or max |half_axis| + max_distance above 15";
-		if (why)
-		{
-			char buf[192]; snprintf(buf, sizeof(buf), "vxb_mesh_closest_to_segment: segment %u: %s", q, why);
-			return fail(ctx, VXB_ERR_ARGUMENT, buf);
-		}
-	}
-	return hostQuery(m, m->segmentIn, 1, m->segmentOut, segments, count, hits,
-		[&](const vxb_segment* in, vxb_segment_hit* out) { return enqueueClosestSegment(m, maxDistance, in, count, out); });
+	const auto segmentFault = [=](uint32_t i) -> const char* {
+		const float* c = segments[i].center;
+		const float* h = segments[i].half_axis;
+		if (!std::isfinite(c[0]) || !std::isfinite(c[1]) || !std::isfinite(c[2])) return "non-finite centre";
+		if (!vxb_capsule_reach(make_float3(h[0], h[1], h[2]), maxDistance)) return "non-finite half axis, or max |half_axis| + max_distance above 15";
+		return nullptr;
+	};
+	return meshQuery(m, { "vxb_mesh_closest_to_segment", !segments || !hits, "segments or hits", maxDistanceFault(maxDistance) }, count,
+		rule("segment", segmentFault), [&] {
+			return hostQuery(m, segments, sizeof(vxb_segment) * count, count, hits, [&](const vxb_segment* in, vxb_segment_hit* out) {
+				return launchLevel0(m, vxb_closest_segment_kernel, VXB_COLLIDE_THREADS, count, maxDistance, in, count, out); }); });
 }
 
 int vxb_mesh_closest_to_segment_device(vxb_mesh* m, float maxDistance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (!validMaxDistance(maxDistance)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_to_segment_device: max_distance must be in [0, 15]");
-	if (count && (!segments || !hits)) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_closest_to_segment_device: NULL segments or hits");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_closest_to_segment_device: nothing applied yet");
-	if (!count) return VXB_OK;
-	cudaSetDevice(ctx->device);
-	return enqueueClosestSegment(m, maxDistance, segments, count, hits);
+	return meshQuery(m, { "vxb_mesh_closest_to_segment_device", !segments || !hits, "segments or hits", maxDistanceFault(maxDistance) },
+		count, deviceRule,
+		[&] { return launchLevel0(m, vxb_closest_segment_kernel, VXB_COLLIDE_THREADS, count, maxDistance, segments, count, hits); });
 }
 
+// The host gather: count and scan, then the total decides the fill: the triangles are only written when they fit.
 int vxb_mesh_overlap_box(vxb_mesh* m, const vxb_box* boxes, uint32_t count, uint64_t* offsets, vxb_overlap_triangle* tris, uint64_t capacity)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (count && (!boxes || !offsets || (!tris && capacity))) return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_overlap_box: NULL boxes, offsets or tris");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_overlap_box: nothing applied yet");
-	if (!count) return VXB_OK;
-	const long long bad = invalidBox(boxes, count);
-	if (bad >= 0)
-	{
-		char buf[160]; snprintf(buf, sizeof(buf), "vxb_mesh_overlap_box: box %lld: non-finite component or min > max", bad);
-		return fail(ctx, VXB_ERR_ARGUMENT, buf);
-	}
-	cudaSetDevice(ctx->device);
-	cudaStream_t st = ctx->stream;
-	const uint64_t entries = (uint64_t)count + 1;
-	if (count > m->boxIn.count || entries > m->overlapOffsets.count)
-	{
-		VXB_CUDA(ctx, cudaStreamSynchronize(st)); // nothing queued may still use the staging being replaced
-		VXB_CUDA(ctx, m->boxIn.ensure(count)); VXB_CUDA(ctx, m->overlapOffsets.ensure(entries));
-	}
-	VXB_CUDA(ctx, cudaMemcpyAsync(m->boxIn.p, boxes, sizeof(vxb_box) * count, cudaMemcpyHostToDevice, st));
-	// count and scan, then the total decides the fill: the triangles are only written when they fit
-	int r = enqueueOverlap(m, m->boxIn.p, count, m->overlapOffsets.p, nullptr, 0);
-	if (r != VXB_OK) return r;
-	uint64_t total = 0;
-	VXB_CUDA(ctx, cudaMemcpyAsync(&total, m->overlapOffsets.p + count, sizeof(total), cudaMemcpyDeviceToHost, st));
-	VXB_CUDA(ctx, cudaStreamSynchronize(st));
-	if (tris && total <= capacity && total)
-	{
-		if (total > m->overlapOut.count) VXB_CUDA(ctx, m->overlapOut.ensure(total)); // the stream is idle here
-		VxbOverlapMesh om;
-		r = overlapView(m, om);   // the map is built: this queues nothing
+	const char* what = "vxb_mesh_overlap_box";
+	return meshQuery(m, { what, !boxes || !offsets || (!tris && capacity), "boxes, offsets or tris", nullptr }, count,
+		rule("box", [=](uint32_t i) { return vxb_box_valid(boxes[i]) ? nullptr : "non-finite component or min > max"; }), [&]() -> int {
+		vxb_context* ctx = m->ctx;
+		cudaStream_t st = ctx->stream;
+		const uint64_t entries = (uint64_t)count + 1;
+		if (sizeof(vxb_box) * count > m->stageIn.count || entries > m->overlapOffsets.count)
+		{
+			VXB_CUDA(ctx, cudaStreamSynchronize(st)); // nothing queued may still use the staging being replaced
+			VXB_CUDA(ctx, m->stageIn.ensure(sizeof(vxb_box) * count)); VXB_CUDA(ctx, m->overlapOffsets.ensure(entries));
+		}
+		const vxb_box* in = (const vxb_box*)m->stageIn.p;
+		VXB_CUDA(ctx, cudaMemcpyAsync(m->stageIn.p, boxes, sizeof(vxb_box) * count, cudaMemcpyHostToDevice, st));
+		int r = enqueueOverlap(m, in, count, m->overlapOffsets.p, nullptr, 0);
 		if (r != VXB_OK) return r;
-		vxb_overlap_kernel<true><<<queryCtas(ctx, count, VXB_OVERLAP_THREADS), VXB_OVERLAP_THREADS, 0, st>>>(om, m->boxIn.p, count,
-			m->overlapOffsets.p, m->overlapOut.p, total);
-		VXB_CUDA(ctx, cudaGetLastError());
-		VXB_CUDA(ctx, cudaMemcpyAsync(tris, m->overlapOut.p, sizeof(vxb_overlap_triangle) * total, cudaMemcpyDeviceToHost, st));
-	}
-	VXB_CUDA(ctx, cudaMemcpyAsync(offsets, m->overlapOffsets.p, sizeof(uint64_t) * entries, cudaMemcpyDeviceToHost, st));
-	VXB_CUDA(ctx, cudaStreamSynchronize(st));
-	if (tris && total > capacity)
-	{
-		char buf[192];
-		snprintf(buf, sizeof(buf), "vxb_mesh_overlap_box: %llu triangles exceed the capacity of %llu; offsets are written",
-			(unsigned long long)total, (unsigned long long)capacity);
-		return fail(ctx, VXB_ERR_CAPACITY, buf);
-	}
-	return VXB_OK;
+		uint64_t total = 0;
+		VXB_CUDA(ctx, cudaMemcpyAsync(&total, m->overlapOffsets.p + count, sizeof(total), cudaMemcpyDeviceToHost, st));
+		VXB_CUDA(ctx, cudaStreamSynchronize(st));
+		if (tris && total <= capacity && total)
+		{
+			const size_t bytes = sizeof(vxb_overlap_triangle) * total;
+			if (bytes > m->stageOut.count) VXB_CUDA(ctx, m->stageOut.ensure(bytes)); // the stream is idle here
+			VxbOverlapMesh om;
+			r = overlapView(m, om);   // the map is built: this queues nothing
+			if (r != VXB_OK) return r;
+			vxb_overlap_kernel<true><<<queryCtas(ctx, count, VXB_OVERLAP_THREADS), VXB_OVERLAP_THREADS, 0, st>>>(om, in, count,
+				m->overlapOffsets.p, (vxb_overlap_triangle*)m->stageOut.p, total);
+			VXB_CUDA(ctx, cudaGetLastError());
+			VXB_CUDA(ctx, cudaMemcpyAsync(tris, m->stageOut.p, bytes, cudaMemcpyDeviceToHost, st));
+		}
+		VXB_CUDA(ctx, cudaMemcpyAsync(offsets, m->overlapOffsets.p, sizeof(uint64_t) * entries, cudaMemcpyDeviceToHost, st));
+		VXB_CUDA(ctx, cudaStreamSynchronize(st));
+		if (tris && total > capacity)
+		{
+			char buf[192];
+			snprintf(buf, sizeof(buf), "%s: %llu triangles exceed the capacity of %llu; offsets are written", what,
+				(unsigned long long)total, (unsigned long long)capacity);
+			return fail(ctx, VXB_ERR_CAPACITY, buf);
+		}
+		return VXB_OK;
+	});
 }
 
 int vxb_mesh_overlap_box_device(vxb_mesh* m, const vxb_box* boxes, uint32_t count, uint64_t* offsets, vxb_overlap_triangle* tris, uint64_t capacity)
 {
-	if (!m) return VXB_ERR_ARGUMENT;
-	vxb_context* ctx = m->ctx;
-	if (count && (!boxes || !offsets || (!tris && capacity)))
-		return fail(ctx, VXB_ERR_ARGUMENT, "vxb_mesh_overlap_box_device: NULL boxes, offsets or tris");
-	if (!m->content) return fail(ctx, VXB_ERR_STATE, "vxb_mesh_overlap_box_device: nothing applied yet");
-	if (!count) return VXB_OK;
-	cudaSetDevice(ctx->device);
-	return enqueueOverlap(m, boxes, count, offsets, tris, capacity);
+	return meshQuery(m, { "vxb_mesh_overlap_box_device", !boxes || !offsets || (!tris && capacity), "boxes, offsets or tris", nullptr },
+		count, deviceRule, [&] { return enqueueOverlap(m, boxes, count, offsets, tris, capacity); });
 }
 
 } // extern "C"

@@ -14,12 +14,14 @@
 #if defined(__CUDACC__)
 #define VXB_FN __device__ __forceinline__
 #define VXB_FN_BIG __device__ __forceinline__ // the per-vertex helpers: inlined, a call would pass the vertex through local memory
+#define VXB_HD __host__ __device__ __forceinline__ // a query rule the host pre-check and the kernels both evaluate
 #define VXB_SQRT(x) __fsqrt_rn(x)
 #define VXB_DIV(a, b) __fdiv_rn((a), (b))
 #else
 #include <cmath>
 #define VXB_FN inline
 #define VXB_FN_BIG inline
+#define VXB_HD inline
 #define VXB_SQRT(x) std::sqrt(x)
 #define VXB_DIV(a, b) ((a) / (b))
 #endif

@@ -3,15 +3,7 @@
 //
 //   sweeps          vxb_ray_walk with the block boxes grown by r + VXB_RAY_EPS; the proof of the walk, extended to that
 //                   growth, is at the top of vxb_ray.cuh.
-//   closest points  no walk: a triangle within max_distance of the query lies in a block whose box is within max_distance
-//                   of the query (a level-0 triangle lies in the closed box of its block), and the float test below skips
-//                   a block only when its box is farther than max_distance + VXB_RAY_EPS (the float box distance is within
-//                   a few ulps of the true one; an accepted triangle is within max_distance plus rounding).  Such a block
-//                   lies within max_distance + eps <= 15 + 1/16 < 16 of the query along every axis.  Along an axis where the
-//                   query lies inside the grid, its index is that of the query's block +-1.  Along an axis where the query
-//                   lies outside (below 0 or above n), only the first or last block of the axis is that close, and that is
-//                   the clamped index.  So the 27 neighbours of the clamped block hold every block that can contribute, for
-//                   queries inside and outside the grid box alike.
+//   closest points  no walk: the 27 neighbours of the query's clamped block (vxb_point_candidate, with the proof).
 //   capsules        the same two routes with the reach |h_i| + r (sweeps: the walk grown by max_i |h_i| + r + eps) or
 //                   |h_i| + max_distance (segments: the per-axis box gap instead of the distance); see "capsules" below.
 #pragma once
@@ -162,16 +154,11 @@ __global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_sphere_cast_kernel(co
 		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
 		bool bStarted = false;
 		vxb_ray_walk(m, ray, r + VXB_RAY_EPS, bt, [&](const unsigned s) {
-			const vxb_block_record* rec = m.dir + s;
-			const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
-			for (unsigned k = lane; k < tris; k += 32)
-			{
-				float3 a, b, c;
-				vxb_ray_triangle(m, vo, io, k, a, b, c);
+			vxb_slot_triangles(m, s, [&](unsigned k, const float3& a, const float3& b, const float3& c) {
 				bool started;
 				const float t = vxb_sweep_triangle(o, d, c0, r, rr, dd, tMin, tMax, a, b, c, started);
 				if (t < CUDART_INF_F && vxb_ray_before(t, s, k, bt, bs, bk)) { bt = t; bs = s; bk = k; bStarted = started; }
-			}
+			});
 		});
 		if (lane == vxb_ray_winner(bt, bs, bk))
 		{
@@ -199,6 +186,42 @@ __global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_sphere_cast_kernel(co
 	}
 }
 
+// The point neighbourhood of the closest-point and closest-to-segment queries: this lane's candidate slot, neighbour k = lane
+// (< 27) of the block of p clamped into the grid, when `ok` (the same for the whole warp) holds, the block lies in the grid,
+// `near(bx, by, bz)` accepts it and the map has a block there.
+//   closest points  a triangle within max_distance of the query lies in a block whose box is within max_distance of the
+//                   query (a level-0 triangle lies in the closed box of its block), and `near` rejects a block only when its
+//                   box is farther than max_distance + VXB_RAY_EPS (the float box distance is within a few ulps of the true
+//                   one; an accepted triangle is within max_distance plus rounding).  Such a block lies within max_distance +
+//                   eps <= 15 + 1/16 < 16 of the query along every axis.  Along an axis where the query lies inside the grid,
+//                   its index is that of the query's block +-1.  Along an axis where the query lies outside (below 0 or above
+//                   n), only the first or last block of the axis is that close, and that is the clamped index.  So the 27
+//                   neighbours of the clamped block hold every block that can contribute, for queries inside and outside the
+//                   grid box alike.
+//   segments        the same with the per-axis gap: `near` rejects a block only when its box is farther than |h_i| +
+//                   max_distance + eps from the centre along some axis, and the reach rule keeps that below 16.
+template <class Near>
+VXB_FN bool vxb_point_candidate(const VxbRayMesh& m, const float3 p, bool ok, Near&& near, unsigned& slot)
+{
+	const unsigned lane = threadIdx.x & 31;
+	const int nb = m.nb;
+	bool cand = false;
+	slot = VXB_RAY_MISS;
+	if (ok && lane < 27)
+	{
+		const float top = (float)(nb - 1);
+		const int bx = (int)fminf(fmaxf(floorf(p.x * 0.0625f), 0.f), top) + (int)(lane % 3) - 1;
+		const int by = (int)fminf(fmaxf(floorf(p.y * 0.0625f), 0.f), top) + (int)((lane / 3) % 3) - 1;
+		const int bz = (int)fminf(fmaxf(floorf(p.z * 0.0625f), 0.f), top) + (int)(lane / 9) - 1;
+		if (bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb && near(bx, by, bz))
+		{
+			slot = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
+			cand = slot != VXB_RAY_MISS;
+		}
+	}
+	return cand;
+}
+
 // One warp per query point, persistent over the batch: lane k < 27 takes neighbour k of the query's block (clamped into the
 // grid), the warp then tests the candidate blocks' triangles strided over the lanes.  Points and hits in OUTPUT (Y-up)
 // coordinates.
@@ -207,53 +230,29 @@ __global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_closest_point_kernel(
 {
 	const unsigned lane = threadIdx.x & 31;
 	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
-	const int nb = m.nb;
 	const float md2 = maxDistance * maxDistance, reach = maxDistance + VXB_RAY_EPS;
-	const int ox = (int)(lane % 3) - 1, oy = (int)((lane / 3) % 3) - 1, oz = (int)(lane / 9) - 1;
 	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
 	{
 		const float3 p = make_float3(points[3 * q], points[3 * q + 1], points[3 * q + 2]);
 		float bd = CUDART_INF_F, bu = 0.f, bv = 0.f;   // this lane's nearest triangle
 		float3 bp = make_float3(0.f, 0.f, 0.f);
 		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		bool cand = false;
-		unsigned slot = VXB_RAY_MISS;
-		if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && lane < 27)
-		{
-			const float top = (float)(nb - 1);
-			const int bx = (int)fminf(fmaxf(floorf(p.x * 0.0625f), 0.f), top) + ox;
-			const int by = (int)fminf(fmaxf(floorf(p.y * 0.0625f), 0.f), top) + oy;
-			const int bz = (int)fminf(fmaxf(floorf(p.z * 0.0625f), 0.f), top) + oz;
-			if (bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb)
-			{
-				const float gx = fmaxf(fmaxf((float)(16 * bx) - p.x, p.x - (float)(16 * bx + 16)), 0.f);
-				const float gy = fmaxf(fmaxf((float)(16 * by) - p.y, p.y - (float)(16 * by + 16)), 0.f);
-				const float gz = fmaxf(fmaxf((float)(16 * bz) - p.z, p.z - (float)(16 * bz + 16)), 0.f);
-				if (VXB_SQRT((gx * gx + gy * gy) + gz * gz) <= reach)
-				{
-					slot = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
-					cand = slot != VXB_RAY_MISS;
-				}
-			}
-		}
-		unsigned todo = __ballot_sync(0xFFFFFFFFu, cand);
-		while (todo)
-		{
-			const unsigned src = __ffs(todo) - 1;
-			todo &= todo - 1;
-			const unsigned s = __shfl_sync(0xFFFFFFFFu, slot, src);
-			const vxb_block_record* rec = m.dir + s;
-			const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
-			for (unsigned k = lane; k < tris; k += 32)
-			{
-				float3 a, b, c, x;
+		unsigned slot;
+		const bool cand = vxb_point_candidate(m, p, isfinite(p.x) && isfinite(p.y) && isfinite(p.z), [&](int bx, int by, int bz) {
+			const float gx = fmaxf(fmaxf((float)(16 * bx) - p.x, p.x - (float)(16 * bx + 16)), 0.f);
+			const float gy = fmaxf(fmaxf((float)(16 * by) - p.y, p.y - (float)(16 * by + 16)), 0.f);
+			const float gz = fmaxf(fmaxf((float)(16 * bz) - p.z, p.z - (float)(16 * bz + 16)), 0.f);
+			return VXB_SQRT((gx * gx + gy * gy) + gz * gz) <= reach;
+		}, slot);
+		vxb_warp_each(cand, slot, [&](const unsigned s) {
+			vxb_slot_triangles(m, s, [&](unsigned k, const float3& a, const float3& b, const float3& c) {
+				float3 x;
 				float u, v;
-				vxb_ray_triangle(m, vo, io, k, a, b, c);
 				vxb_closest_on_triangle(p, a, b, c, x, u, v);
 				const float d2 = vxb_dist2(p, x);
 				if (d2 <= md2 && vxb_ray_before(d2, s, k, bd, bs, bk)) { bd = d2; bs = s; bk = k; bu = u; bv = v; bp = x; }
-			}
-		}
+			});
+		});
 		if (lane == vxb_ray_winner(bd, bs, bk))
 		{
 			vxb_closest_hit h;
@@ -410,8 +409,9 @@ VXB_FN float vxb_capsule_triangle(const float3 o, const float3 d, const float3 c
 	return t;
 }
 
-// the reach of a capsule shape (include/vxb200.h): a finite half axis and max_i |h_i| + extra <= VXB_SPHERE_RADIUS_MAX
-VXB_FN bool vxb_capsule_reach(const float3 h, float extra)
+// the reach of a capsule shape (include/vxb200.h), in float for the host pre-check and the kernels alike: a finite half axis
+// and max_i |h_i| + extra <= VXB_SPHERE_RADIUS_MAX
+VXB_HD bool vxb_capsule_reach(const float3 h, float extra)
 {
 	const float hm = fmaxf(fmaxf(fabsf(h.x), fabsf(h.y)), fabsf(h.z));
 	return isfinite(h.x) && isfinite(h.y) && isfinite(h.z) && hm + extra <= VXB_SPHERE_RADIUS_MAX;
@@ -461,17 +461,12 @@ __global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_capsule_cast_kernel(c
 		bool bStarted = false;
 		if (r > 0.f && vxb_capsule_reach(h, r))   // the same for the whole warp
 			vxb_ray_walk(m, ray, fmaxf(fmaxf(g.x, g.y), g.z), bt, [&](const unsigned s) {
-				const vxb_block_record* rec = m.dir + s;
-				const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
-				for (unsigned k = lane; k < tris; k += 32)
-				{
-					float3 a, b, c;
-					vxb_ray_triangle(m, vo, io, k, a, b, c);
-					if (!vxb_path_meets_box(ray, g, a, b, c)) continue;
+				vxb_slot_triangles(m, s, [&](unsigned k, const float3& a, const float3& b, const float3& c) {
+					if (!vxb_path_meets_box(ray, g, a, b, c)) return;
 					bool started;
 					const float t = vxb_capsule_triangle(o, d, c0, h, r, rr, dd, tMin, tMax, a, b, c, started);
 					if (t < CUDART_INF_F && vxb_ray_before(t, s, k, bt, bs, bk)) { bt = t; bs = s; bk = k; bStarted = started; }
-				}
+				});
 			});
 		if (lane == vxb_ray_winner(bt, bs, bk))
 		{
@@ -511,7 +506,6 @@ __global__ void __launch_bounds__(VXB_COLLIDE_THREADS, 1) vxb_closest_segment_ke
 {
 	const unsigned lane = threadIdx.x & 31;
 	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
-	const int nb = m.nb;
 	const float md2 = maxDistance * maxDistance;
 	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
 	{
@@ -522,43 +516,24 @@ __global__ void __launch_bounds__(VXB_COLLIDE_THREADS, 1) vxb_closest_segment_ke
 			fabsf(h.z) + maxDistance + VXB_RAY_EPS);
 		float bd = CUDART_INF_F;   // this lane's nearest triangle
 		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		bool cand = false;
-		unsigned slot = VXB_RAY_MISS;
-		if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && vxb_capsule_reach(h, maxDistance) && lane < 27)
-		{
-			const float top = (float)(nb - 1);
-			const int bx = (int)fminf(fmaxf(floorf(p.x * 0.0625f), 0.f), top) + (int)(lane % 3) - 1;
-			const int by = (int)fminf(fmaxf(floorf(p.y * 0.0625f), 0.f), top) + (int)((lane / 3) % 3) - 1;
-			const int bz = (int)fminf(fmaxf(floorf(p.z * 0.0625f), 0.f), top) + (int)(lane / 9) - 1;
-			if (bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb &&
-				!((float)(16 * bx) - p.x > g.x || p.x - (float)(16 * bx + 16) > g.x) &&
+		unsigned slot;
+		const bool ok = isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && vxb_capsule_reach(h, maxDistance);
+		const bool cand = vxb_point_candidate(m, p, ok, [&](int bx, int by, int bz) {
+			return !((float)(16 * bx) - p.x > g.x || p.x - (float)(16 * bx + 16) > g.x) &&
 				!((float)(16 * by) - p.y > g.y || p.y - (float)(16 * by + 16) > g.y) &&
-				!((float)(16 * bz) - p.z > g.z || p.z - (float)(16 * bz + 16) > g.z))
-			{
-				slot = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
-				cand = slot != VXB_RAY_MISS;
-			}
-		}
-		unsigned todo = __ballot_sync(0xFFFFFFFFu, cand);
-		while (todo)
-		{
-			const unsigned src = __ffs(todo) - 1;
-			todo &= todo - 1;
-			const unsigned s = __shfl_sync(0xFFFFFFFFu, slot, src);
-			const vxb_block_record* rec = m.dir + s;
-			const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
-			for (unsigned k = lane; k < tris; k += 32)
-			{
-				float3 a, b, c, x;
-				float u, v, w;
-				vxb_ray_triangle(m, vo, io, k, a, b, c);
+				!((float)(16 * bz) - p.z > g.z || p.z - (float)(16 * bz + 16) > g.z);
+		}, slot);
+		vxb_warp_each(cand, slot, [&](const unsigned s) {
+			vxb_slot_triangles(m, s, [&](unsigned k, const float3& a, const float3& b, const float3& c) {
 				if (fminf(fminf(a.x, b.x), c.x) - p.x > g.x || p.x - fmaxf(fmaxf(a.x, b.x), c.x) > g.x ||
 					fminf(fminf(a.y, b.y), c.y) - p.y > g.y || p.y - fmaxf(fmaxf(a.y, b.y), c.y) > g.y ||
-					fminf(fminf(a.z, b.z), c.z) - p.z > g.z || p.z - fmaxf(fmaxf(a.z, b.z), c.z) > g.z) continue;
+					fminf(fminf(a.z, b.z), c.z) - p.z > g.z || p.z - fmaxf(fmaxf(a.z, b.z), c.z) > g.z) return;
+				float3 x;
+				float u, v, w;
 				const float d2 = vxb_segment_triangle(p, h, a, b, c, x, u, v, w);
 				if (d2 <= md2 && vxb_ray_before(d2, s, k, bd, bs, bk)) { bd = d2; bs = s; bk = k; }
-			}
-		}
+			});
+		});
 		if (lane == vxb_ray_winner(bd, bs, bk))
 		{
 			vxb_segment_hit x;

@@ -29,8 +29,9 @@ struct VxbOverlapMesh
 	unsigned base0;         // vxb_mesh_bounds.level_base[0]
 };
 
-// the rule of the host variant: finite components and min_i <= max_i (NaN fails)
-VXB_FN bool vxb_box_valid(const vxb_box& b)
+// the box rule (include/vxb200.h), which the host variant checks and the kernels answer with 0 triangles: finite components
+// and min_i <= max_i (NaN fails)
+VXB_HD bool vxb_box_valid(const vxb_box& b)
 {
 	bool ok = true;
 	for (int i = 0; i < 3; ++i) ok = ok && isfinite(b.min[i]) && isfinite(b.max[i]) && b.min[i] <= b.max[i];
@@ -111,13 +112,7 @@ VXB_FN void vxb_overlap_walk(const VxbOverlapMesh& om, const vxb_box& b, Block&&
 			if (mn.x <= b.max[0] && mx.x >= b.min[0] && mn.y <= b.max[1] && mx.y >= b.min[1] && mn.z <= b.max[2] && mx.z >= b.min[2])
 				slot = __ldg(&om.m.map[cid]);
 		}
-		unsigned todo = __ballot_sync(0xFFFFFFFFu, slot != VXB_RAY_MISS);
-		while (todo)
-		{
-			const unsigned src = __ffs(todo) - 1;
-			todo &= todo - 1;
-			block(__shfl_sync(0xFFFFFFFFu, slot, src));
-		}
+		vxb_warp_each(slot != VXB_RAY_MISS, slot, block);
 	}
 }
 

@@ -171,6 +171,36 @@ VXB_FN unsigned vxb_ray_winner(float t, unsigned s, unsigned k)
 	return __ffs(__ballot_sync(0xFFFFFFFFu, s == ws && k == wk)) - 1;
 }
 
+// The slot hand-off: `block(slot)` is called by the whole warp (every lane takes part) once for each lane that has `take`,
+// with that lane's slot, in lane order.  Returns whether any lane had one.
+template <class Block>
+VXB_FN bool vxb_warp_each(bool take, unsigned slot, Block&& block)
+{
+	unsigned todo = __ballot_sync(0xFFFFFFFFu, take);
+	const bool any = todo != 0;
+	while (todo)
+	{
+		const unsigned src = __ffs(todo) - 1;
+		todo &= todo - 1;
+		block(__shfl_sync(0xFFFFFFFFu, slot, src));
+	}
+	return any;
+}
+
+// f(k, a, b, c) for each triangle k of level-0 slot s with its positions, strided over the lanes (k = lane, lane + 32, ...)
+template <class F>
+VXB_FN void vxb_slot_triangles(const VxbRayMesh& m, unsigned s, F&& f)
+{
+	const vxb_block_record* rec = m.dir + s;
+	const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
+	for (unsigned k = threadIdx.x & 31; k < tris; k += 32)
+	{
+		float3 a, b, c;
+		vxb_ray_triangle(m, vo, io, k, a, b, c);
+		f(k, a, b, c);
+	}
+}
+
 // The conservative block walk of the proof at the top, for one segment per warp (every lane calls it with the same ray),
 // with the candidate step as a parameter: lane k < 27 calls `cand(bx, by, bz, T0, T1, t0, t1, last, slot)` for neighbour k
 // of the cell [t0, t1) when that block lies in the grid; it returns whether there is a directory slot to test there, and
@@ -216,14 +246,7 @@ VXB_FN void vxb_ray_walk_by(const int nb, const vxb_ray& ray, const float grow, 
 			const unsigned peers = __match_any_sync(0xFFFFFFFFu, slot);   // every lane takes part (lanes without a slot hold VXB_RAY_MISS)
 			take = take && (peers & ((1u << lane) - 1u)) == 0;
 		}
-		unsigned todo = __ballot_sync(0xFFFFFFFFu, take);
-		const bool tested = todo != 0;
-		while (todo)
-		{
-			const unsigned src = __ffs(todo) - 1;
-			todo &= todo - 1;
-			block(__shfl_sync(0xFFFFFFFFu, slot, src));
-		}
+		const bool tested = vxb_warp_each(take, slot, block);
 		if (last) break;
 		if (tested)
 		{
@@ -278,18 +301,13 @@ __global__ void __launch_bounds__(VXB_RAY_THREADS) vxb_raycast_kernel(const VxbR
 		float bt = CUDART_INF_F, bu = 0.f, bv = 0.f;   // this lane's best hit
 		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
 		vxb_ray_walk(m, ray, VXB_RAY_EPS, bt, [&](const unsigned s) {
-			const vxb_block_record* rec = m.dir + s;
-			const unsigned tris = __ldg(&rec->index_count) / 3, vo = __ldg(&rec->vertex_offset), io = __ldg(&rec->index_offset);
-			for (unsigned k = lane; k < tris; k += 32)
-			{
-				float3 p0, p1, p2;
-				vxb_ray_triangle(m, vo, io, k, p0, p1, p2);
+			vxb_slot_triangles(m, s, [&](unsigned k, const float3& p0, const float3& p1, const float3& p2) {
 				float t, u, v;
 				if (vxb_ray_mt(px, py, pz, dx, dy, dz, tMin, tMax, p0, p1, p2, t, u, v) && vxb_ray_before(t, s, k, bt, bs, bk))
 				{
 					bt = t; bs = s; bk = k; bu = u; bv = v;
 				}
-			}
+			});
 		});
 		// ---- the winner by the tie rule; its lane writes the hit ----
 		if (lane == vxb_ray_winner(bt, bs, bk))
