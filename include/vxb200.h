@@ -793,6 +793,73 @@ int vxb_mesh_closest_to_segment(vxb_mesh* mesh, float max_distance, const vxb_se
 int vxb_mesh_capsule_cast_device(vxb_mesh* mesh, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits);
 int vxb_mesh_closest_to_segment_device(vxb_mesh* mesh, float max_distance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits);
 
+/* ---- collision queries against the drawn LOD cut: sphere sweeps and closest points on what the renderer shows -------------
+ * The collision queries above answer about the level-0 surface; where the renderer draws coarser blocks the drawn surface
+ * differs from it by up to a cell of the drawn level.  vxb_mesh_sphere_cast_cut and vxb_mesh_closest_point_cut answer about
+ * the triangles the renderer draws for the cut of (lod_camera, lod_factor), so that a camera boom stops at the hill the
+ * player sees and a marker snapped to the surface sits on the drawn triangles.
+ *   The drawn set   vxb_mesh_raycast_cut's: the cut of (lod_camera, lod_factor) as vxb_mesh_select_cut makes it (view culling
+ *                   plays no part), each cut block's regular triangles and the transition meshes its block_adj names, every
+ *                   vertex at the position the vertex shader selects (sec when its mask is non-zero and covered by
+ *                   block_adj, pos otherwise).
+ *   The tests       vxb_mesh_sphere_cast's sweep (start in contact, the offset face, the three edge cylinders, the three
+ *                   vertex spheres) and vxb_mesh_closest_point's closest point (Ericson's routine, dd <= m*m inclusive),
+ *                   unchanged, on the selected positions.  center, point, u, v and the blended normal are computed as there,
+ *                   on the drawn triangle's nrm (both positions share it).
+ *   The hit         Least t (sweeps) or dd (points); ties go to the lower slot, then to the lower part (the regular mesh
+ *                   before transition face 0, ..., face 5), then to the lower triangle: vxb_mesh_raycast_cut's rule.  A pure
+ *                   function of the mesh (content and order), of (lod_camera, lod_factor) and of the query: not of the
+ *                   launch, the variant or the rest of the batch.  A miss is the level-0 query's miss with level and face 0.
+ *   At lod_factor = 1e30 the cut is all of level 0 with block_adj = 0, so the first 64 bytes (sweeps) or 48 bytes (points) of
+ *                   every hit equal vxb_mesh_sphere_cast's or vxb_mesh_closest_point's, with level = 0 and face = 0xFFFFFFFF
+ *                   on a hit.
+ *   The reach       The walk rests on the measured boxes and the excursion e as vxb_mesh_raycast_cut's does, with every box
+ *                   grown by the query's reach R (the radius r for sweeps, max_distance m for points): a block within reach
+ *                   of a query point then stays within e + R + 1/16 < 16 voxels of it, one of the 27 neighbours of its block.
+ *                   The first cut query after an apply (of any of the three kinds) rebuilds the all-level map, measures e
+ *                   and waits for the stream once.
+ * Refusals (`hits` untouched), arguments first: VXB_ERR_ARGUMENT for a NULL pointer with count > 0, a bad lod_factor or
+ * lod_camera (as vxb_mesh_raycast_cut), a radius outside 0 < r <= 15 or a max_distance outside 0 <= m <= 15 (as the
+ * collision queries); VXB_ERR_STATE before the first apply and for a mesh without every level and transition mesh (as
+ * vxb_mesh_select_cut); then, after the map, VXB_ERR_STATE when e + 1/16 > 15 (as vxb_mesh_raycast_cut) or when e + R > 15
+ * in float (vxb_last_error names e and R).  count = 0 does nothing.  The HOST variants also refuse an invalid sweep (the ray
+ * rules) or a point with a non-finite coordinate, naming its index; on the DEVICE variants such a query is a miss. */
+typedef struct vxb_sphere_cut_hit
+{
+	float t;                /* as vxb_sphere_hit: the first 64 bytes are its fields */
+	uint32_t slot;          /* mesh directory slot of the drawn block; VXB_RAY_MISS */
+	uint32_t block_id;
+	uint32_t triangle;      /* k: indices [part offset + 3k, +3) of the part `face` names (as vxb_cut_hit) */
+	float center[3];
+	float point[3];         /* the closest point of the drawn triangle to `center` */
+	float normal[3];
+	float u, v;
+	uint32_t flags;         /* VXB_SPHERE_STARTED_IN_CONTACT */
+	uint32_t level;         /* the hit block's level */
+	uint32_t face;          /* 0xFFFFFFFF: the regular mesh; f: the transition mesh of face f (TransitionFaceId order) */
+} vxb_sphere_cut_hit;                                                       /* 72 bytes; the first 64 are vxb_sphere_hit's */
+typedef struct vxb_closest_cut_hit
+{
+	float distance;         /* as vxb_closest_hit: the first 48 bytes are its fields */
+	uint32_t slot;
+	uint32_t block_id;
+	uint32_t triangle;
+	float point[3];         /* the closest point of the drawn surface within max_distance */
+	float normal[3];
+	float u, v;
+	uint32_t level, face;   /* as vxb_sphere_cut_hit */
+} vxb_closest_cut_hit;                                                     /* 56 bytes; the first 48 are vxb_closest_hit's */
+/* HOST memory; block until the hits are written.  `points` is count x 3 floats. */
+int vxb_mesh_sphere_cast_cut(vxb_mesh* mesh, const float lod_camera[3], float lod_factor, float radius,
+                             const vxb_ray* rays, uint32_t count, vxb_sphere_cut_hit* hits);
+int vxb_mesh_closest_point_cut(vxb_mesh* mesh, const float lod_camera[3], float lod_factor, float max_distance,
+                               const float* points, uint32_t count, vxb_closest_cut_hit* hits);
+/* DEVICE memory; enqueued on vxb_stream(ctx) like vxb_mesh_raycast_cut_device (the first cut query after an apply waits). */
+int vxb_mesh_sphere_cast_cut_device(vxb_mesh* mesh, const float lod_camera[3], float lod_factor, float radius,
+                                    const vxb_ray* rays, uint32_t count, vxb_sphere_cut_hit* hits);
+int vxb_mesh_closest_point_cut_device(vxb_mesh* mesh, const float lod_camera[3], float lod_factor, float max_distance,
+                                      const float* points, uint32_t count, vxb_closest_cut_hit* hits);
+
 /* ---- box overlap gathers: the level-0 triangles in axis-aligned boxes, for a client's physics mid-phase and navmesh tiles --
  * Every other query returns one answer per query; vxb_mesh_overlap_box returns, per box, every triangle that overlaps it, so
  * that a physics engine runs its own narrowphase for its own shapes (processAllTriangles-style callbacks), a navmesh builder

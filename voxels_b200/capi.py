@@ -194,6 +194,11 @@ SPHERE_HIT_DTYPE = np.dtype([("t", "<f4"), ("slot", "<u4"), ("block_id", "<u4"),
 CLOSEST_HIT_DTYPE = np.dtype([("distance", "<f4"), ("slot", "<u4"), ("block_id", "<u4"), ("triangle", "<u4"), ("point", "<f4", 3),
                               ("normal", "<f4", 3), ("u", "<f4"), ("v", "<f4")])
 assert SPHERE_HIT_DTYPE.itemsize == 64 and CLOSEST_HIT_DTYPE.itemsize == 48
+# vxb_sphere_cut_hit / vxb_closest_cut_hit (include/vxb200.h "collision queries against the drawn LOD cut"): the level-0 hits,
+# then level and face
+SPHERE_CUT_HIT_DTYPE = np.dtype(SPHERE_HIT_DTYPE.descr + [("level", "<u4"), ("face", "<u4")])
+CLOSEST_CUT_HIT_DTYPE = np.dtype(CLOSEST_HIT_DTYPE.descr + [("level", "<u4"), ("face", "<u4")])
+assert SPHERE_CUT_HIT_DTYPE.itemsize == 72 and CLOSEST_CUT_HIT_DTYPE.itemsize == 56
 
 # vxb_capsule_sweep / vxb_segment / vxb_capsule_hit / vxb_segment_hit (include/vxb200.h "capsule queries")
 CAPSULE_SWEEP_DTYPE = np.dtype([("path", RAY_DTYPE), ("half_axis", "<f4", 3), ("radius", "<f4")])
@@ -384,6 +389,10 @@ def load_library():
         "vxb_mesh_sphere_cast_device": (C.c_int, [vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_closest_point": (C.c_int, [vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_closest_point_device": (C.c_int, [vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_sphere_cast_cut": (C.c_int, [vp, vp, C.c_float, C.c_float, vp, u32, vp]),
+        "vxb_mesh_sphere_cast_cut_device": (C.c_int, [vp, vp, C.c_float, C.c_float, vp, u32, vp]),
+        "vxb_mesh_closest_point_cut": (C.c_int, [vp, vp, C.c_float, C.c_float, vp, u32, vp]),
+        "vxb_mesh_closest_point_cut_device": (C.c_int, [vp, vp, C.c_float, C.c_float, vp, u32, vp]),
         "vxb_mesh_capsule_cast": (C.c_int, [vp, vp, u32, vp]),
         "vxb_mesh_capsule_cast_device": (C.c_int, [vp, vp, u32, vp]),
         "vxb_mesh_closest_to_segment": (C.c_int, [vp, C.c_float, vp, u32, vp]),
@@ -414,6 +423,8 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_mesh_select_lod_views", "vxb_mesh_select_cut", "vxb_mesh_raycast", "vxb_mesh_raycast_device",
                     "vxb_mesh_raycast_cut", "vxb_mesh_raycast_cut_device",
                     "vxb_mesh_sphere_cast", "vxb_mesh_sphere_cast_device", "vxb_mesh_closest_point", "vxb_mesh_closest_point_device",
+                    "vxb_mesh_sphere_cast_cut", "vxb_mesh_sphere_cast_cut_device", "vxb_mesh_closest_point_cut",
+                    "vxb_mesh_closest_point_cut_device",
                     "vxb_mesh_capsule_cast", "vxb_mesh_capsule_cast_device", "vxb_mesh_closest_to_segment",
                     "vxb_mesh_closest_to_segment_device", "vxb_mesh_overlap_box", "vxb_mesh_overlap_box_device"]
 
@@ -711,6 +722,52 @@ class Mesh:
         `hits_ptr`; enqueued on the context's stream, returns without waiting."""
         self.ctx._check(self.L.vxb_mesh_closest_point_device(self.h, max_distance, _dev(points_ptr), count, _dev(hits_ptr)),
                         "vxb_mesh_closest_point_device")
+
+    def sphere_cast_cut_rc(self, lod_camera, lod_factor, radius, rays, hits=None, count=None):
+        """vxb_mesh_sphere_cast_cut's return code: `lod_camera` and `rays` (a RAY_DTYPE array) may be None for NULL pointers,
+        `hits` (a SPHERE_CUT_HIT_DTYPE array) None for a NULL pointer; `count` defaults to len(rays)."""
+        rays = _batch(rays, RAY_DTYPE)
+        n = (0 if rays is None else len(rays)) if count is None else count
+        return self.L.vxb_mesh_sphere_cast_cut(self.h, _ptr(_batch(lod_camera, np.float32)), lod_factor, radius, _ptr(rays), n, _ptr(hits))
+
+    def sphere_cast_cut(self, lod_camera, lod_factor, radius, origins, directions=None, t_min=0.0, t_max=np.inf):
+        """Sweeps a sphere of `radius` voxels along each segment against the triangles vxb_mesh_select_cut's cut of (lod_camera,
+        lod_factor) draws (vxb_mesh_sphere_cast_cut): `origins` / `directions` as for sphere_cast.  Returns a
+        SPHERE_CUT_HIT_DTYPE array."""
+        rays = np.ascontiguousarray(origins if directions is None else make_rays(origins, directions, t_min, t_max), RAY_DTYPE)
+        hits = np.zeros(len(rays), SPHERE_CUT_HIT_DTYPE)
+        self.ctx._check(self.sphere_cast_cut_rc(lod_camera, lod_factor, radius, rays, hits), "vxb_mesh_sphere_cast_cut")
+        return hits
+
+    def sphere_cast_cut_device(self, lod_camera, lod_factor, radius, rays_ptr, count, hits_ptr):
+        """vxb_mesh_sphere_cast_cut_device: `count` vxb_ray at the device address `rays_ptr`, hits to `hits_ptr`; enqueued on
+        the context's stream (the first cut query after an apply waits for it once)."""
+        self.ctx._check(self.L.vxb_mesh_sphere_cast_cut_device(self.h, _ptr(_batch(lod_camera, np.float32)), lod_factor, radius,
+                                                               _dev(rays_ptr), count, _dev(hits_ptr)), "vxb_mesh_sphere_cast_cut_device")
+
+    def closest_points_cut_rc(self, lod_camera, lod_factor, max_distance, points, hits=None, count=None):
+        """vxb_mesh_closest_point_cut's return code: `lod_camera` and `points` ([count, 3] float32) may be None for NULL
+        pointers, `hits` (a CLOSEST_CUT_HIT_DTYPE array) None for a NULL pointer; `count` defaults to len(points)."""
+        pts = _batch(points, np.float32)
+        pts = None if pts is None else pts.reshape(-1, 3)
+        n = (0 if pts is None else len(pts)) if count is None else count
+        return self.L.vxb_mesh_closest_point_cut(self.h, _ptr(_batch(lod_camera, np.float32)), lod_factor, max_distance, _ptr(pts), n,
+                                                 _ptr(hits))
+
+    def closest_points_cut(self, lod_camera, lod_factor, points, max_distance):
+        """The nearest drawn surface point of the cut of (lod_camera, lod_factor) within `max_distance` voxels of each of the
+        [count, 3] `points` (OUTPUT, Y-up coordinates), vxb_mesh_closest_point_cut.  Returns a CLOSEST_CUT_HIT_DTYPE array."""
+        pts = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
+        hits = np.zeros(len(pts), CLOSEST_CUT_HIT_DTYPE)
+        self.ctx._check(self.closest_points_cut_rc(lod_camera, lod_factor, max_distance, pts, hits), "vxb_mesh_closest_point_cut")
+        return hits
+
+    def closest_points_cut_device(self, lod_camera, lod_factor, max_distance, points_ptr, count, hits_ptr):
+        """vxb_mesh_closest_point_cut_device: `count` points (3 floats each) at the device address `points_ptr`, hits to
+        `hits_ptr`; enqueued on the context's stream (the first cut query after an apply waits for it once)."""
+        self.ctx._check(self.L.vxb_mesh_closest_point_cut_device(self.h, _ptr(_batch(lod_camera, np.float32)), lod_factor,
+                                                                 max_distance, _dev(points_ptr), count, _dev(hits_ptr)),
+                        "vxb_mesh_closest_point_cut_device")
 
     def capsule_cast_rc(self, sweeps, hits=None, count=None):
         """vxb_mesh_capsule_cast's return code for a CAPSULE_SWEEP_DTYPE array (or None for a NULL pointer); the hits go to

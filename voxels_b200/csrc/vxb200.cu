@@ -45,6 +45,8 @@ static_assert(sizeof(vxb_capsule_sweep) == 48 && sizeof(vxb_segment) == 24 && si
 	"capsule layouts");
 static_assert(sizeof(vxb_view) == 96 && sizeof(vxb_mesh_bounds) == 64 && VXB_MAX_LEVELS == 12, "view and bounds layouts");
 static_assert(sizeof(vxb_cut_hit) == 56 && offsetof(vxb_cut_hit, level) == 48, "vxb_cut_hit layout");
+static_assert(sizeof(vxb_sphere_cut_hit) == 72 && offsetof(vxb_sphere_cut_hit, level) == 64 && sizeof(vxb_closest_cut_hit) == 56 &&
+	offsetof(vxb_closest_cut_hit, level) == 48, "cut collision layouts");
 static_assert(sizeof(vxb_box) == 24 && sizeof(vxb_overlap_triangle) == 48, "overlap layouts");
 
 namespace
@@ -2288,8 +2290,9 @@ int ensureMap(vxb_mesh* m, VxbRayMesh& rm)
 }
 
 // The all-level map and the excursion for the applied run, queued on ctx->stream; the excursion is read back, so a rebuild
-// waits for the stream once.  Then the refusal of an excursion beyond the walk's reach, and the kernel's view of the mesh.
-int ensureCutMap(vxb_mesh* m, const char* what, VxbCutRayMesh& c)
+// waits for the stream once.  Then the refusals of an excursion beyond the walk's reach, alone and with the query's reach
+// `reach` (the sweep radius or max_distance; 0 for rays), and the kernel's view of the mesh.
+int ensureCutMap(vxb_mesh* m, const char* what, float reach, VxbCutRayMesh& c)
 {
 	vxb_context* ctx = m->ctx;
 	cudaStream_t st = ctx->stream;
@@ -2317,6 +2320,13 @@ int ensureCutMap(vxb_mesh* m, const char* what, VxbCutRayMesh& c)
 	{
 		char buf[192];
 		snprintf(buf, sizeof(buf), "%s: a block's vertices leave its lattice box by %g voxels; the walk reaches 15 - 1/16", what, (double)m->excursion);
+		return fail(ctx, VXB_ERR_STATE, buf);
+	}
+	if (!(m->excursion + reach <= 15.f))
+	{
+		char buf[224];
+		snprintf(buf, sizeof(buf), "%s: a block's vertices leave its lattice box by %g voxels (e) and the query reaches %g (R); "
+			"e + R must be at most 15", what, (double)m->excursion, (double)reach);
 		return fail(ctx, VXB_ERR_STATE, buf);
 	}
 	c.m.dir = m->dir.p; c.m.map = m->cutMap.buf.p; c.m.verts = m->set[m->active].v.p; c.m.idx = m->set[m->active].i.p; c.m.nb = (int)nb;
@@ -2348,16 +2358,38 @@ int launchLevel0(vxb_mesh* m, Kernel kernel, unsigned threads, uint32_t count, A
 	return VXB_OK;
 }
 
-int enqueueRaycastCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, const vxb_ray* rays, uint32_t count, vxb_cut_hit* hits)
+// A cut query's launch on ctx->stream: `kernel(c, args...)`, one warp per query over the all-level map (ensureCutMap, with
+// the query's reach) and the cut of (camera, lodFactor).
+template <class Kernel, class... Args>
+int launchCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, float reach, Kernel kernel, unsigned threads,
+	uint32_t count, Args... args)
 {
 	VxbCutRayMesh c;
-	const int e = ensureCutMap(m, what, c);
+	const int e = ensureCutMap(m, what, reach, c);
 	if (e != VXB_OK) return e;
 	for (int k = 0; k < 3; ++k) c.cut.camera[k] = camera[k];
 	c.cut.lod = lodFactor;
-	vxb_raycast_cut_kernel<<<queryCtas(m->ctx, count, VXB_RAY_THREADS), VXB_RAY_THREADS, 0, m->ctx->stream>>>(c, rays, count, hits);
+	kernel<<<queryCtas(m->ctx, count, threads), threads, 0, m->ctx->stream>>>(c, args...);
 	VXB_CUDA(m->ctx, cudaGetLastError());
 	return VXB_OK;
+}
+
+int enqueueRaycastCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, const vxb_ray* rays, uint32_t count, vxb_cut_hit* hits)
+{
+	return launchCut(m, what, camera, lodFactor, 0.f, vxb_raycast_cut_kernel, VXB_RAY_THREADS, count, rays, count, hits);
+}
+
+int enqueueSphereCastCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, float radius, const vxb_ray* rays,
+	uint32_t count, vxb_sphere_cut_hit* hits)
+{
+	return launchCut(m, what, camera, lodFactor, radius, vxb_sphere_cast_cut_kernel, VXB_COLLIDE_THREADS, count, radius, rays, count, hits);
+}
+
+int enqueueClosestPointCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, float maxDistance, const float* points,
+	uint32_t count, vxb_closest_cut_hit* hits)
+{
+	return launchCut(m, what, camera, lodFactor, maxDistance, vxb_closest_point_cut_kernel, VXB_COLLIDE_THREADS, count, maxDistance,
+		points, count, hits);
 }
 
 // the gather kernels' view of the mesh: the level-0 map (ensureMap) and the level-0 bounds
@@ -2428,6 +2460,15 @@ const char* cutFault(const float camera[3], float lodFactor)
 	if (!std::isfinite(lodFactor) || !(lodFactor >= VXB_LOD_FACTOR_MIN)) return "lod_factor must be finite and >= 2";
 	if (camera && (!std::isfinite(camera[0]) || !std::isfinite(camera[1]) || !std::isfinite(camera[2]))) return "non-finite lod_camera component";
 	return nullptr;
+}
+// the first of two batch-argument faults, or NULL
+const char* firstFault(const char* a, const char* b) { return a ? a : b; }
+
+// the host variants' point rule (include/vxb200.h): why point i is refused, or NULL
+const char* pointFault(const float* points, uint32_t i)
+{
+	const float* p = points + 3 * (size_t)i;
+	return std::isfinite(p[0]) && std::isfinite(p[1]) && std::isfinite(p[2]) ? nullptr : "non-finite coordinate";
 }
 
 // the host variants' ray rule (include/vxb200.h): why the ray is refused, or NULL
@@ -2900,12 +2941,8 @@ int vxb_mesh_sphere_cast_device(vxb_mesh* m, float radius, const vxb_ray* rays, 
 
 int vxb_mesh_closest_point(vxb_mesh* m, float maxDistance, const float* points, uint32_t count, vxb_closest_hit* hits)
 {
-	const auto pointFault = [=](uint32_t i) -> const char* {
-		const float* p = points + 3 * (size_t)i;
-		return std::isfinite(p[0]) && std::isfinite(p[1]) && std::isfinite(p[2]) ? nullptr : "non-finite coordinate";
-	};
 	return meshQuery(m, { "vxb_mesh_closest_point", !points || !hits, "points or hits", maxDistanceFault(maxDistance) }, count,
-		rule("point", pointFault), [&] {
+		rule("point", [=](uint32_t i) { return pointFault(points, i); }), [&] {
 			return hostQuery(m, points, 3 * sizeof(float) * count, count, hits, [&](const float* in, vxb_closest_hit* out) {
 				return launchLevel0(m, vxb_closest_point_kernel, VXB_COLLIDE_THREADS, count, maxDistance, in, count, out); }); });
 }
@@ -2914,6 +2951,44 @@ int vxb_mesh_closest_point_device(vxb_mesh* m, float maxDistance, const float* p
 {
 	return meshQuery(m, { "vxb_mesh_closest_point_device", !points || !hits, "points or hits", maxDistanceFault(maxDistance) }, count,
 		deviceRule, [&] { return launchLevel0(m, vxb_closest_point_kernel, VXB_COLLIDE_THREADS, count, maxDistance, points, count, hits); });
+}
+
+int vxb_mesh_sphere_cast_cut(vxb_mesh* m, const float camera[3], float lodFactor, float radius, const vxb_ray* rays, uint32_t count,
+	vxb_sphere_cut_hit* hits)
+{
+	const char* what = "vxb_mesh_sphere_cast_cut";
+	return meshQuery(m, { what, !camera || !rays || !hits, "lod_camera, rays or hits", firstFault(cutFault(camera, lodFactor), radiusFault(radius)),
+		true }, count, rule("sweep", [=](uint32_t i) { return rayFault(rays[i]); }), [&] {
+			return hostQuery(m, rays, sizeof(vxb_ray) * count, count, hits, [&](const vxb_ray* in, vxb_sphere_cut_hit* out) {
+				return enqueueSphereCastCut(m, what, camera, lodFactor, radius, in, count, out); }); });
+}
+
+int vxb_mesh_sphere_cast_cut_device(vxb_mesh* m, const float camera[3], float lodFactor, float radius, const vxb_ray* rays, uint32_t count,
+	vxb_sphere_cut_hit* hits)
+{
+	const char* what = "vxb_mesh_sphere_cast_cut_device";
+	return meshQuery(m, { what, !camera || !rays || !hits, "lod_camera, rays or hits", firstFault(cutFault(camera, lodFactor), radiusFault(radius)),
+		true }, count, deviceRule, [&] { return enqueueSphereCastCut(m, what, camera, lodFactor, radius, rays, count, hits); });
+}
+
+int vxb_mesh_closest_point_cut(vxb_mesh* m, const float camera[3], float lodFactor, float maxDistance, const float* points, uint32_t count,
+	vxb_closest_cut_hit* hits)
+{
+	const char* what = "vxb_mesh_closest_point_cut";
+	return meshQuery(m, { what, !camera || !points || !hits, "lod_camera, points or hits",
+		firstFault(cutFault(camera, lodFactor), maxDistanceFault(maxDistance)), true }, count,
+		rule("point", [=](uint32_t i) { return pointFault(points, i); }), [&] {
+			return hostQuery(m, points, 3 * sizeof(float) * count, count, hits, [&](const float* in, vxb_closest_cut_hit* out) {
+				return enqueueClosestPointCut(m, what, camera, lodFactor, maxDistance, in, count, out); }); });
+}
+
+int vxb_mesh_closest_point_cut_device(vxb_mesh* m, const float camera[3], float lodFactor, float maxDistance, const float* points,
+	uint32_t count, vxb_closest_cut_hit* hits)
+{
+	const char* what = "vxb_mesh_closest_point_cut_device";
+	return meshQuery(m, { what, !camera || !points || !hits, "lod_camera, points or hits",
+		firstFault(cutFault(camera, lodFactor), maxDistanceFault(maxDistance)), true }, count, deviceRule,
+		[&] { return enqueueClosestPointCut(m, what, camera, lodFactor, maxDistance, points, count, hits); });
 }
 
 int vxb_mesh_capsule_cast(vxb_mesh* m, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits)
