@@ -1,6 +1,6 @@
 // Per-block and flat kernels of the polygonizer (included by vxb200.cu after vxb_kernels.cuh).
 //
-//   vxb_block_kernel<MODE>  one pass per block: tile -> non-trivial cells, consistency page or material votes, statistics,
+//   vxb_block_kernel<0|1|2> one pass per block: tile -> non-trivial cells, consistency page or material votes, statistics,
 //                           then the decide passes (vxb_decide_cells) and the arena reservation.  Level 0 makes the block's
 //                           vertices and triangles itself; levels >= 1 write cell records + the vertex work list.
 //   vxb_big_block_kernel    the decide passes of the blocks too large for the shared-memory path of vxb_block_kernel.
@@ -68,23 +68,18 @@ __device__ __forceinline__ unsigned vxb_rank_of(const unsigned int* nt32, const 
 // axis, as 19 x 19 rows of 48 bytes (the TMA box starts on a 16-byte boundary one 16-byte group before the block).
 #define VXB_DTILE_PITCH 48
 #define VXB_DTILE_BYTES (19 * 19 * VXB_DTILE_PITCH)
-// Capacities of the shared-memory path of vxb_block_kernel<MODE>: non-trivial cells of a block (larger blocks go to
+// Capacities of the shared-memory path of vxb_block_kernel<0|1|2>: non-trivial cells of a block (larger blocks go to
 // vxb_big_block_kernel) and new vertices of a level-0 block generated inside the CTA (more => the flat kernels).
 template <int MODE> struct VxbBlockCaps { static constexpr int CAP = 1024, VL = (MODE == 0 ? 2048 : 8), NBUF = (MODE == 0 ? 1 : 2); }; // level 0: one tile buffer => 4 CTAs per SM
 
 // ------------------------------------------------------------------------------------------------
-// vxb_block_kernel<MODE>: everything that needs the block as a unit, in ONE pass over its sample tile
+// vxb_block_kernel<0|1|2>: everything that needs the block as a unit, in ONE pass over its sample tile
 //   tile -> case codes -> non-trivial bits; consistency page (level 0) or majority votes of the non-trivial cells and of
 //   every transition-face cell into the level's material page (CalculateMaterialForCellCache :753-838, called from :1568
 //   and :1859) - the only cross-level dependency; statistics; then, for blocks with non-trivial cells: ordered compaction,
 //   materials, owned reuse slots, new-vs-reuse decisions, block scans -> vertex / triangle bases, arena reservation.
-//   MODE 0  level 0 from its work list: halo tile by one TMA load into one tile buffer; the new vertices and the triangles
-//           are produced right here from shared memory (no per-cell records in global memory).
-//   MODE 1  one level from its work list (17^3 tile: TMA for level 0 / the even lattice of level 1, strided gather else);
-//           writes 16-byte cell records + the vertex work list for the flat per-vertex / per-cell kernels.
-//   MODE 2  all coarse levels [coarseLo, computed) in ONE launch: items = blocks in level order; a block first waits for
-//           the done flags of its eight children (they were taken earlier from the same cursor, so they are running or
-//           done: no deadlock), applies the block-walk test itself, then works like MODE 1.
+//   Three kernels, one body each (<0> level 0, <1> one level below the coarse ones, <2> all coarse levels), over the
+//   shared phases below.
 // ------------------------------------------------------------------------------------------------
 template <int MODE>
 struct __align__(128) VxbBlockSmem
@@ -263,359 +258,304 @@ __device__ __forceinline__ void vxb_write_block_rec(const VxbDev& d, unsigned sl
 	if (level > 0 && level != d.lastLevel && d.transitions) d.transList[atomicAdd(&d.counters->transBlocks, 1u)] = slot;
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(VXB_THREADS, VXB_OCC) vxb_block_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB, const VxbDev d, const int levelArg)
+// ---- the phases of vxb_block_kernel<0|1|2> that more than one of them runs ----
+
+template <class Smem>
+__device__ __forceinline__ void vxb_block_prologue(Smem& s)
 {
-	constexpr int PITCH = (MODE == 0) ? VXB_DTILE_PITCH : VXB_TILE_PITCH;
-	constexpr int ROWS = (MODE == 0) ? 19 : 17;
-	typedef VxbBlockSmem<MODE> Smem;
-	constexpr int CAP_C = Smem::Caps::CAP, VL_CAP = Smem::Caps::VL, NBUF = Smem::Caps::NBUF;
-	extern __shared__ __align__(128) unsigned char smemRaw[];
-	Smem& s = *reinterpret_cast<Smem*>(smemRaw);
 	const int tid = threadIdx.x;
-	const VxbGrid g = d.grid;
-	unsigned phaseBits = 0; // mbarrier phase of each tile buffer, bit = buffer
 	if (tid == 0) { vxb_mbar_init(&s.mbar[0], 1); vxb_mbar_init(&s.mbar[1], 1); }
 	if (tid < 16) s.hist[tid] = 0;
 	if (tid < 8) s.used[tid] = 0;
 	for (int i = tid; i < 256; i += VXB_THREADS) { s.tabClass[i] = vxbGRegularCellClass[i]; s.tabCell[i] = vxbGRegularCellData[i]; }
 	for (int i = tid; i < 3072; i += VXB_THREADS) s.tabVert[i] = vxbGRegularVertexData[i];
-	unsigned statNonTrivial = 0;
+}
 
-	// ---- work source ----
-	unsigned workCount;
-	const unsigned* worklist = nullptr;
-	unsigned* cursor;
-	if (MODE == 2)
+// the CTA's statistics, once per CTA
+template <class Smem>
+__device__ __forceinline__ void vxb_block_epilogue(const Smem& s, const VxbDev& d, unsigned statNonTrivial)
+{
+	const int tid = threadIdx.x;
+	__syncthreads();
+	if (tid < 16 && s.hist[tid]) atomicAdd(&d.counters->perCase[tid], s.hist[tid]);
+	if (tid < 8 && s.used[tid]) atomicOr(&d.counters->usedMaterials[tid], s.used[tid]);
+	if (tid == 0 && statNonTrivial) atomicAdd(&d.counters->nonTrivial, statNonTrivial);
+}
+
+// block coordinates of entry `item` of a level's work list (coordIds, x fastest; blocks per axis: a power of two)
+__device__ __forceinline__ void vxb_work_block(const VxbDev& d, const unsigned* worklist, unsigned item, int level, int& bx, int& by, int& bz)
+{
+	const int nbl = (d.n >> 4) >> level, sh = __ffs(nbl) - 1;
+	const unsigned c = worklist[item];
+	bx = c & (nbl - 1); by = (c >> sh) & (nbl - 1); bz = c >> (2 * sh);
+}
+
+// thread 0 takes the next item from the cursor into s.item and clears the per-item flags; the caller's barrier publishes them
+template <class Smem>
+__device__ __forceinline__ void vxb_take_item(Smem& s, unsigned* cursor)
+{
+	if (threadIdx.x == 0) { s.item = atomicAdd(cursor, 1u); s.hasChild = 0; s.pageReady = 0; s.take = 1; s.removed = 0; }
+}
+
+// tile -> non-trivial bits (s.nt32) and their exclusive prefix per word (s.wpre); returns the block's non-trivial cells
+template <int PITCH, int ROWS, class Smem>
+__device__ __forceinline__ unsigned vxb_count_cells(Smem& s, const signed char* tile)
+{
+	const int tid = threadIdx.x;
+	vxb_classify_bits<PITCH, ROWS>(tile, s.rowSign, s.nt32);
+	__syncthreads();
+	unsigned ntc;
+	const unsigned cnt = (tid < 128) ? __popc(s.nt32[tid]) : 0u; // one word per thread
+	const unsigned ex = vxb_block_scan(cnt, s.warpSums, ntc);
+	if (tid < 128) s.wpre[tid] = ex;
+	__syncthreads();
+	return ntc;
+}
+
+// A block with ntc > 0 non-trivial cells: the level's page (level 0: consistency bits; above: the material page), the
+// compact list (inCap), the emission index (emitMine; thread 0 counts the cells in statNonTrivial), the statistics
+// (PerCaseCellsCount :1574) and, above level 0, the material of every non-trivial cell (:1568): majority vote of its 8
+// children, stored in the level's page.  An in-capacity level-0 block takes its histogram in pass A instead.
+template <int PITCH, int ROWS, class Smem>
+__device__ __forceinline__ void vxb_block_cells(Smem& s, const signed char* tile, const VxbDev& d, int level, unsigned coordId,
+	int bx, int by, int bz, unsigned ntc, bool inCap, bool emitMine, unsigned& statNonTrivial)
+{
+	const int tid = threadIdx.x, m = 1 << level;
+	if (level == 0)
 	{
-		if (tid == 0)
+		if (tid < 128)
 		{
-			unsigned acc = 0;
-			for (int l = d.coarseLo; l < d.computed; ++l)
-			{
-				const int nbl = (d.n >> 4) >> l;
-				const int nx = d.ranged ? d.rangeMax[l][0] - d.rangeMin[l][0] : nbl, ny = d.ranged ? d.rangeMax[l][1] - d.rangeMin[l][1] : nbl, nz = d.ranged ? d.rangeMax[l][2] - d.rangeMin[l][2] : nbl;
-				acc += (nx > 0 && ny > 0 && nz > 0) ? (unsigned)nx * ny * nz : 0u;
-				s.levelEnd[l - d.coarseLo] = acc;
-			}
+			unsigned* page = d.consPages + (size_t)coordId * 128;
+			// bits are only ever set (:757); a full run has cleared consValid, and this block is the only one that sets its flag
+			page[tid] = (d.incremental && d.consValid[coordId]) ? (page[tid] | s.nt32[tid]) : s.nt32[tid];
 		}
-		__syncthreads();
-		workCount = (d.computed > d.coarseLo) ? s.levelEnd[d.computed - d.coarseLo - 1] : 0u;
-		cursor = &d.counters->coarseCursor;
 	}
+	else if (!d.cacheValid[level][coordId]) vxb_init_cache_page(d, level, coordId);
+	if (inCap) vxb_compact_cells(s.nt32, s.wpre, s.list);
+	__syncthreads();
+	if (tid == 0)
+	{
+		if (level == 0) d.consValid[coordId] = 1; else d.cacheValid[level][coordId] = 1;
+		s.pageReady = 1;
+		if (emitMine)
+		{
+			const unsigned idx = d.workBase[level] + atomicAdd(&d.counters->emitCount[level], 1u);
+			d.emitList[idx] = ((unsigned)level << 28) | coordId;
+			s.emitIdx = idx;
+			statNonTrivial += ntc;
+		}
+	}
+	auto cellWork = [&](int c) {
+		signed char v[8];
+		vxb_tile_samples<PITCH, ROWS>(tile, c, v);
+		if (emitMine) atomicAdd(&s.hist[s.tabClass[vxb_case_code(v)]], 1u);
+		if (level > 0)
+		{
+			const VxbVoteSource voteSrc = vxb_vote_source(d, level);
+			const int vote = vxb_vote_cell(voteSrc, (bx * 16 + (c & 15)) * m, (by * 16 + ((c >> 4) & 15)) * m, (bz * 16 + (c >> 8)) * m);
+			if (vote >= 0) d.cachePages[level][(size_t)coordId * 4096 + c] = (unsigned short)vote;
+		}
+	};
+	if (inCap) { if (level > 0) for (unsigned i = tid; i < ntc; i += VXB_THREADS) cellWork(s.list[i]); }
 	else
 	{
-		workCount = d.counters->workCount[levelArg];
-		worklist = d.worklist + d.workBase[levelArg];
-		cursor = &d.counters->workCursor[levelArg];
+		for (int r = tid; r < 256; r += VXB_THREADS)
+		{
+			unsigned bits = reinterpret_cast<const unsigned short*>(s.nt32)[r];
+			while (bits) { const int x = __ffs(bits) - 1; bits &= bits - 1; cellWork(r * 16 + x); }
+		}
 	}
-
-	// block coordinates of a work item (MODE 2: also its level)
-	auto decode = [&](unsigned item, int& level, int& bx, int& by, int& bz) {
-		if (MODE == 2)
-		{
-			int q = 0;
-			while (item >= s.levelEnd[q]) ++q;
-			level = d.coarseLo + q;
-			unsigned r = item - (q ? s.levelEnd[q - 1] : 0u);
-			const int nbl = (d.n >> 4) >> level;
-			const int x0 = d.ranged ? d.rangeMin[level][0] : 0, y0 = d.ranged ? d.rangeMin[level][1] : 0, z0 = d.ranged ? d.rangeMin[level][2] : 0;
-			const int nx = d.ranged ? d.rangeMax[level][0] - x0 : nbl, ny = d.ranged ? d.rangeMax[level][1] - y0 : nbl;
-			bx = x0 + (int)(r % nx); by = y0 + (int)((r / nx) % ny); bz = z0 + (int)(r / ((unsigned)nx * ny));
-		}
-		else
-		{
-			level = levelArg;
-			const int nbl = (d.n >> 4) >> level, sh = __ffs(nbl) - 1; // a power of two
-			const unsigned c = worklist[item];
-			bx = c & (nbl - 1); by = (c >> sh) & (nbl - 1); bz = c >> (2 * sh);
-		}
-	};
-	// tile of the block: issue (thread 0; asynchronous when TMA applies) ...
-	auto issue = [&](int buf, int level, int bx, int by, int bz) {
-		if (MODE == 0)
-		{
-			if (tid == 0)
-			{
-				// the tile starts one sample before the block (x: 16 samples, a 16-byte aligned start); on the low grid edge
-				// the box starts at a negative coordinate and TMA zero-fills what lies outside the volume
-				vxb_fence_proxy_async();
-				vxb_mbar_expect_tx(&s.mbar[buf], VXB_DTILE_BYTES);
-				vxb_tma_load_3d(s.tiles[buf], &tmapA, bx * 16 - 16, by * 16 - 1, bz * 16 - 1, &s.mbar[buf]);
-			}
-		}
-		else if (MODE == 1) vxb_tile_issue(s.tiles[buf], &s.mbar[buf], &tmapA, &tmapB, d, level, bx, by, bz);
-	};
-
-	// MODE 0 takes its items two ahead: the cursor's round trip for the item after next overlaps a whole block (the other
-	// modes keep the register it costs)
-	constexpr bool AHEAD = MODE == 0;
-	if (tid == 0) { s.item = atomicAdd(cursor, 1u); if (AHEAD) s.ahead = atomicAdd(cursor, 1u); }
 	__syncthreads();
-	unsigned item = s.item, aheadItem = AHEAD ? s.ahead : 0u;
-	int buf = 0;
-	if (item < workCount) { int l, x, y, z; decode(item, l, x, y, z); issue(0, l, x, y, z); }
+	if (!inCap && emitMine) vxb_save_nt(d, s.emitIdx, s.nt32, s.wpre);
+}
+
+// A mid-level block (levels >= 1 below the last): every cell of every transition face votes too, trivial ones included
+// (:1859) - observable at the next level.  Ends without a barrier.
+template <class Smem>
+__device__ __forceinline__ void vxb_face_votes(Smem& s, const VxbDev& d, int level, int nb, unsigned coordId, int bx, int by, int bz)
+{
+	const int tid = threadIdx.x, m = 1 << level;
+	const VxbVoteSource voteSrc = vxb_vote_source(d, level);
+	if (tid < 8)
+	{
+		const int cnb = nb * 2;
+		const size_t cb = ((size_t)(bz * 2 + (tid >> 2)) * cnb + (by * 2 + ((tid >> 1) & 1))) * cnb + (bx * 2 + (tid & 1));
+		const bool valid = (level == 1) ? __ldcg(d.consValid + cb) : __ldcg(d.cacheValid[level - 1] + cb);
+		if (valid) atomicOr(&s.hasChild, 1u);
+	}
 	__syncthreads();
+	if (!s.hasChild) return;
+	// an all-{EMPTY,0} page is indistinguishable from no page, so it can be created before the votes
+	if (!s.pageReady)
+	{
+		if (!d.cacheValid[level][coordId]) vxb_init_cache_page(d, level, coordId);
+		__syncthreads();
+		if (tid == 0) { d.cacheValid[level][coordId] = 1; s.pageReady = 1; }
+	}
+	for (int fc = tid; fc < 256; fc += VXB_THREADS)
+	{
+		const int row = fc >> 4, col = fc & 15;
+		// most face cells have no child with a material: test all six faces first (independent loads, all in flight
+		// together), then run the vote only where it can succeed
+		unsigned candidates = 0;
+#pragma unroll
+		for (int face = 0; face < 6; ++face)
+		{
+			int axis, ua, va;
+			vxb_face_axes(face, axis, ua, va);
+			const int bc = (axis == 0) ? bx : (axis == 1 ? by : bz);
+			const bool outside = face < 3 ? (bc == 0) : (bc == nb - 1); // neighbour block outside the grid (:1829-1835)
+			const int edge = (face >= 3) ? 15 : 0;
+			const int lx = axis == 0 ? edge : col, ly = axis == 1 ? edge : (axis == 2 ? row : col), lz = axis == 2 ? edge : row;
+			if (vxb_vote_candidate(voteSrc, (bx * 16 + lx) * m, (by * 16 + ly) * m, (bz * 16 + lz) * m) && !outside) candidates |= 1u << face;
+		}
+		while (candidates)
+		{
+			const int face = __ffs(candidates) - 1;
+			candidates &= candidates - 1;
+			int axis, ua, va;
+			vxb_face_axes(face, axis, ua, va);
+			// local[axis] = edge, local[ua] = col, local[va] = row, written with selects (an indexed array would be local memory)
+			const int edge = (face >= 3) ? 15 : 0;
+			const int local[3] = { axis == 0 ? edge : col, axis == 1 ? edge : (axis == 2 ? row : col), axis == 2 ? edge : row };
+			const int vote = vxb_vote_cell(voteSrc, (bx * 16 + local[0]) * m, (by * 16 + local[1]) * m, (bz * 16 + local[2]) * m);
+			if (vote >= 0) d.cachePages[level][(size_t)coordId * 4096 + local[2] * 256 + local[1] * 16 + local[0]] = (unsigned short)vote;
+		}
+	}
+}
+
+// The block's ranges of the arenas and its directory slot: four independent atomics from four warps, one round trip instead
+// of four in a row.  `cells`: the block writes cell records (else cellBase = 0).  A block that does not fit writes nothing;
+// the run is repeated with larger arenas.  (The caller tests the fit: returned from here, the test compiles worse.)
+template <class Smem>
+__device__ __forceinline__ void vxb_reserve(Smem& s, const VxbDev& d, unsigned ntc, unsigned nverts, unsigned ntris, bool cells,
+	unsigned& voff, unsigned& ioff, unsigned& cellBase, unsigned& slot)
+{
+	const int tid = threadIdx.x;
+	if (tid == 0) s.voff = atomicAdd(&d.counters->vertices, nverts);
+	if (tid == 32) s.ioff = atomicAdd(&d.counters->indices, ntris * 3);
+	if (tid == 64 && cells) s.cellBase = atomicAdd(&d.counters->cells, ntc);
+	if (tid == 96) s.slot = atomicAdd(&d.counters->records, 1u);
+	__syncthreads();
+	voff = s.voff; ioff = s.ioff; cellBase = cells ? s.cellBase : 0u; slot = s.slot;
+}
+
+// levels >= 1: the decide passes over the compact list -> cell records + vertex work list for the flat kernels, the block's
+// non-trivial bits for vxb_triangle_kernel, and its directory record
+template <class Smem>
+__device__ __forceinline__ void vxb_emit_cell_records(Smem& s, const signed char* tile, const VxbDev& d, int level, unsigned coordId,
+	int bx, int by, int bz, unsigned ntc)
+{
+	unsigned nverts, ntris, voff, ioff, cellBase, slot;
+	vxb_decide_cells<VXB_TILE_PITCH, 17, true>(s, tile, d, level, coordId, bx, by, bz, ntc, nverts, ntris);
+	vxb_reserve(s, d, ntc, nverts, ntris, true, voff, ioff, cellBase, slot);
+	const bool fits = (unsigned long long)voff + nverts <= d.vcap && (unsigned long long)ioff + ntris * 3ull <= d.icap
+		&& (unsigned long long)cellBase + ntc <= d.ccap && slot < d.rcap;
+	if (fits)
+	{
+		vxb_write_cell_records(s, d, ntc, voff, cellBase, slot);
+		vxb_save_nt(d, s.emitIdx, s.nt32, s.wpre);
+	}
+	if (fits && threadIdx.x == 0) vxb_write_block_rec(d, slot, level, coordId, s.emitIdx, voff, ioff, cellBase, ntc, nverts, ntris, 0u);
+}
+
+template <int MODE>
+__global__ void vxb_block_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB, const VxbDev d, const int levelArg);
+
+// Level 0 from its work list: the halo tile by one TMA load (tmapA: the 48 x 19 x 19 box of the distance volume) into one
+// tile buffer; the new vertices and the triangles are produced right here from shared memory (no per-cell records in
+// global memory).  Blocks over the capacities go to vxb_big_block_kernel + the flat kernels.
+template <>
+__global__ void __launch_bounds__(VXB_THREADS, VXB_OCC) vxb_block_kernel<0>(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap, const VxbDev d, const int)
+{
+	extern __shared__ __align__(128) unsigned char smemRaw[];
+	VxbBlockSmem<0>& s = *reinterpret_cast<VxbBlockSmem<0>*>(smemRaw);
+	const int tid = threadIdx.x;
+	const VxbGrid g = d.grid;
+	const int nb = d.n / 16;
+	unsigned phase = 0, statNonTrivial = 0;
+	vxb_block_prologue(s);
+	const unsigned workCount = d.counters->workCount[0];
+	const unsigned* const worklist = d.worklist + d.workBase[0];
+	unsigned* const cursor = &d.counters->workCursor[0];
+	// thread 0 requests the halo tile of item `it`.  The tile starts one sample before the block (x: 16 samples, a 16-byte
+	// aligned start); on the low grid edge the box starts at a negative coordinate and TMA zero-fills what lies outside.
+	auto issue = [&](unsigned it) {
+		if (tid != 0) return;
+		int x, y, z;
+		vxb_work_block(d, worklist, it, 0, x, y, z);
+		vxb_fence_proxy_async();
+		vxb_mbar_expect_tx(&s.mbar[0], VXB_DTILE_BYTES);
+		vxb_tma_load_3d(s.tiles[0], &tmapA, x * 16 - 16, y * 16 - 1, z * 16 - 1, &s.mbar[0]);
+	};
+
+	// items are taken two ahead: the cursor's round trip for the item after next overlaps a whole block
+	if (tid == 0) { s.item = atomicAdd(cursor, 1u); s.ahead = atomicAdd(cursor, 1u); }
+	__syncthreads();
+	unsigned item = s.item, aheadItem = s.ahead;
+	if (item < workCount) issue(item);
 
 	while (item < workCount)
 	{
+		const unsigned nextItem = aheadItem;
 		unsigned ahead = 0; // thread 0: the item after next, published in s.ahead at the end of this block
-		if (tid == 0) { if (AHEAD) ahead = atomicAdd(cursor, 1u); else s.item = atomicAdd(cursor, 1u); s.hasChild = 0; s.pageReady = 0; s.take = 1; s.removed = 0; }
-		__syncthreads();
-		const unsigned nextItem = AHEAD ? aheadItem : s.item;
-		bool nextIssued = false; // NBUF == 1: the next tile is requested as soon as this one is not read any more
-		if (nextItem < workCount && MODE != 2 && NBUF == 2) { int l, x, y, z; decode(nextItem, l, x, y, z); issue(buf ^ 1, l, x, y, z); nextIssued = true; }
-		int level, bx, by, bz;
-		decode(item, level, bx, by, bz);
-		const int m = 1 << level, nb = d.n / 16 / m;
+		if (tid == 0) { ahead = atomicAdd(cursor, 1u); s.removed = 0; }
+		bool nextIssued = false; // one tile buffer: the next tile is requested as soon as this one is not read any more
+		int bx, by, bz;
+		vxb_work_block(d, worklist, item, 0, bx, by, bz);
 		const unsigned coordId = ((unsigned)bz * nb + by) * nb + bx;
-		const bool midLevel = level > 0 && level != d.lastLevel;
-		signed char* const tileRaw = s.tiles[(MODE == 2 || NBUF == 1) ? 0 : buf];
+		signed char* const tileRaw = s.tiles[0];
+		const int hsx = bx * 16 - 16, hsy = by * 16 - 1, hsz = bz * 16 - 1; // first coordinate held by the halo tile
 
-		if (MODE == 2)
+		vxb_mbar_wait(&s.mbar[0], phase);
+		phase ^= 1u;
+		// grid edges: TMA zero-fills outside the volume, the reference clamps the coordinate to [0, n-1] (:1037-1047, :1198).
+		// One axis after the other, so that edge and corner entries copy values already fixed on the earlier axes.
+		const int lastX = d.n - 1 - hsx, lastY = d.n - 1 - hsy, lastZ = d.n - 1 - hsz; // tile index of coordinate n-1
+		if (bx == 0 || bx == nb - 1)
 		{
-			// warp 0: wait for the children of this run (blocks of the previous coarse level inside the run's range), one lane
-			// each, then the block walk test (vxb_coarse_block_needed) with one lane per child-level neighbour
-			if (tid < 32)
-			{
-				const int cnb = nb * 2, cl = level - 1;
-				if (level > d.coarseLo && tid < 8)
-				{
-					const int cx = bx * 2 + (tid & 1), cy = by * 2 + ((tid >> 1) & 1), cz = bz * 2 + (tid >> 2);
-					const bool inRun = !(d.ranged && (cx < d.rangeMin[cl][0] || cx >= d.rangeMax[cl][0] || cy < d.rangeMin[cl][1] || cy >= d.rangeMax[cl][1] || cz < d.rangeMin[cl][2] || cz >= d.rangeMax[cl][2]));
-					if (inRun)
-					{
-						const volatile unsigned char* flag = d.coarseDone + d.coarseBase[cl] + ((size_t)cz * cnb + cy) * cnb + cx;
-						unsigned spins = 0;
-						while (!*flag) { __nanosleep(32); if (++spins > (1u << 24)) __trap(); }
-					}
-					__threadfence();
-				}
-				__syncwarp();
-				unsigned u = 0, anyChild = 0;
-				if (tid < 27)
-				{
-					const int x = tid % 3, y = (tid / 3) % 3, z = tid / 9;
-					const int cx = min(2 * bx + x, cnb - 1), cy = min(2 * by + y, cnb - 1), cz = min(2 * bz + z, cnb - 1);
-					const size_t cb = ((size_t)cz * cnb + cy) * cnb + cx;
-					u = d.mixInfo[cl][cb];
-					if (x < 2 && y < 2 && z < 2) anyChild = __ldcg(d.cacheValid[cl] + cb);
-				}
-				u = __reduce_or_sync(0xFFFFFFFFu, u);
-				anyChild = __reduce_or_sync(0xFFFFFFFFu, anyChild);
-				if (tid == 0)
-				{
-					s.take = (u == 3u || anyChild != 0u) ? 1u : 0u;
-					if (s.take)
-					{
-						// the block's 17^3 samples: one TMA box of the level's lattice (far-edge entries included, no fix-up)
-						vxb_fence_proxy_async();
-						vxb_mbar_expect_tx(&s.mbar[0], VXB_TILE_BYTES);
-						vxb_tma_load_3d(s.tiles[0], d.coarseMaps + level, bx * 16, by * 16, bz * 16, &s.mbar[0]);
-					}
-				}
-			}
 			__syncthreads();
-			if (!s.take)
+			for (int i = tid; i < 19 * 19; i += VXB_THREADS)
 			{
-				if (tid == 0) { __threadfence(); *(volatile unsigned char*)(d.coarseDone + d.coarseBase[level] + coordId) = 1; }
-				__syncthreads();
-				item = nextItem;
-				continue;
+				signed char* r = tileRaw + i * VXB_DTILE_PITCH;
+				if (bx == 0) r[15] = r[16];
+				if (bx == nb - 1) { r[lastX + 1] = r[lastX]; r[lastX + 2] = r[lastX]; }
 			}
 		}
-
-		// ---- tile ----
-		const signed char* tile; // sample (0, 0, 0) of the block
-		const int hsx = bx * 16 - 16, hsy = by * 16 - 1, hsz = bz * 16 - 1; // MODE 0: first coordinate held by the halo tile
-		if (MODE == 0)
+		if (by == 0 || by == nb - 1)
 		{
-			vxb_mbar_wait(&s.mbar[buf], (phaseBits >> buf) & 1u);
-			phaseBits ^= 1u << buf;
-			// grid edges: TMA zero-fills outside the volume, the reference clamps the coordinate to [0, n-1] (:1037-1047, :1198).
-			// One axis after the other, so that edge and corner entries copy values already fixed on the earlier axes.
-			const int lastX = d.n - 1 - hsx, lastY = d.n - 1 - hsy, lastZ = d.n - 1 - hsz; // tile index of coordinate n-1
-			if (bx == 0 || bx == nb - 1)
+			__syncthreads();
+			for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += VXB_THREADS)
 			{
-				__syncthreads();
-				for (int i = tid; i < 19 * 19; i += VXB_THREADS)
-				{
-					signed char* r = tileRaw + i * VXB_DTILE_PITCH;
-					if (bx == 0) r[15] = r[16];
-					if (bx == nb - 1) { r[lastX + 1] = r[lastX]; r[lastX + 2] = r[lastX]; }
-				}
+				const int z = i / VXB_DTILE_PITCH, x = i % VXB_DTILE_PITCH;
+				signed char* p = tileRaw + z * 19 * VXB_DTILE_PITCH + x;
+				if (by == 0) p[0] = p[VXB_DTILE_PITCH];
+				if (by == nb - 1) for (int q = lastY + 1; q < 19; ++q) p[q * VXB_DTILE_PITCH] = p[lastY * VXB_DTILE_PITCH];
 			}
-			if (by == 0 || by == nb - 1)
-			{
-				__syncthreads();
-				for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += VXB_THREADS)
-				{
-					const int z = i / VXB_DTILE_PITCH, x = i % VXB_DTILE_PITCH;
-					signed char* p = tileRaw + z * 19 * VXB_DTILE_PITCH + x;
-					if (by == 0) p[0] = p[VXB_DTILE_PITCH];
-					if (by == nb - 1) for (int q = lastY + 1; q < 19; ++q) p[q * VXB_DTILE_PITCH] = p[lastY * VXB_DTILE_PITCH];
-				}
-			}
-			if (bz == 0 || bz == nb - 1)
-			{
-				__syncthreads();
-				for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += VXB_THREADS)
-				{
-					const int y = i / VXB_DTILE_PITCH, x = i % VXB_DTILE_PITCH;
-					signed char* p = tileRaw + y * VXB_DTILE_PITCH + x;
-					if (bz == 0) p[0] = p[19 * VXB_DTILE_PITCH];
-					if (bz == nb - 1) for (int q = lastZ + 1; q < 19; ++q) p[q * 19 * VXB_DTILE_PITCH] = p[lastZ * 19 * VXB_DTILE_PITCH];
-				}
-			}
-			tile = tileRaw + (19 + 1) * VXB_DTILE_PITCH + 16;
 		}
-		else if (MODE == 2)
+		if (bz == 0 || bz == nb - 1)
 		{
-			vxb_mbar_wait(&s.mbar[0], phaseBits & 1u);
-			phaseBits ^= 1u;
-			tile = tileRaw;
+			__syncthreads();
+			for (int i = tid; i < 19 * VXB_DTILE_PITCH; i += VXB_THREADS)
+			{
+				const int y = i / VXB_DTILE_PITCH, x = i % VXB_DTILE_PITCH;
+				signed char* p = tileRaw + y * VXB_DTILE_PITCH + x;
+				if (bz == 0) p[0] = p[19 * VXB_DTILE_PITCH];
+				if (bz == nb - 1) for (int q = lastZ + 1; q < 19; ++q) p[q * 19 * VXB_DTILE_PITCH] = p[lastZ * 19 * VXB_DTILE_PITCH];
+			}
 		}
-		else
-		{
-			unsigned ph = (phaseBits >> buf) & 1u;
-			vxb_tile_complete(tileRaw, &s.mbar[buf], ph, d, level, bx, by, bz);
-			phaseBits = (phaseBits & ~(1u << buf)) | (ph << buf);
-			tile = tileRaw;
-		}
+		const signed char* const tile = tileRaw + (19 + 1) * VXB_DTILE_PITCH + 16; // sample (0, 0, 0) of the block
 		__syncthreads();
 
-		vxb_classify_bits<PITCH, ROWS>(tile, s.rowSign, s.nt32);
-		__syncthreads();
-		unsigned ntc;
+		const unsigned ntc = vxb_count_cells<VXB_DTILE_PITCH, 19>(s, tile);
+		const bool inCap = ntc <= (unsigned)VxbBlockCaps<0>::CAP;
+		if (ntc > 0) vxb_block_cells<VXB_DTILE_PITCH, 19>(s, tile, d, 0, coordId, bx, by, bz, ntc, inCap, true, statNonTrivial);
+		if (ntc > 0 && !inCap) { if (tid == 0) d.bigList[atomicAdd(&d.counters->bigCount, 1u)] = s.emitIdx; }
+		else if (ntc > 0)
 		{
-			const unsigned cnt = (tid < 128) ? __popc(s.nt32[tid]) : 0u; // one word per thread
-			const unsigned ex = vxb_block_scan(cnt, s.warpSums, ntc);
-			if (tid < 128) s.wpre[tid] = ex;
-		}
-		__syncthreads();
-		const bool inCap = ntc <= (unsigned)CAP_C;
-		// sharded runs: every rank classifies the coarse levels (the votes feed the next level), one of them emits the block
-		const bool emitMine = MODE != 2 || vxb_coarse_emit_is_mine(d, level, coordId);
-
-		if (ntc > 0)
-		{
-			if (level == 0)
-			{
-				if (tid < 128)
-				{
-					unsigned* page = d.consPages + (size_t)coordId * 128;
-					// bits are only ever set (:757); a full run has cleared consValid, and this block is the only one that sets its flag
-					page[tid] = (d.incremental && d.consValid[coordId]) ? (page[tid] | s.nt32[tid]) : s.nt32[tid];
-				}
-			}
-			else if (!d.cacheValid[level][coordId]) vxb_init_cache_page(d, level, coordId);
-			if (inCap) vxb_compact_cells(s.nt32, s.wpre, s.list);
-			__syncthreads();
-			if (tid == 0)
-			{
-				if (level == 0) d.consValid[coordId] = 1; else d.cacheValid[level][coordId] = 1;
-				s.pageReady = 1;
-				if (emitMine)
-				{
-					const unsigned idx = d.workBase[level] + atomicAdd(&d.counters->emitCount[level], 1u);
-					d.emitList[idx] = ((unsigned)level << 28) | coordId;
-					s.emitIdx = idx;
-					statNonTrivial += ntc;
-				}
-			}
-			// statistics (PerCaseCellsCount :1574) and, above level 0, the material of every non-trivial cell (:1568):
-			// majority vote of its 8 children, stored in the level's page
-			auto cellWork = [&](int c) {
-				signed char v[8];
-				vxb_tile_samples<PITCH, ROWS>(tile, c, v);
-				if (emitMine) atomicAdd(&s.hist[s.tabClass[vxb_case_code(v)]], 1u);
-				if (level > 0)
-				{
-					const VxbVoteSource voteSrc = vxb_vote_source(d, level);
-					const int vote = vxb_vote_cell(voteSrc, (bx * 16 + (c & 15)) * m, (by * 16 + ((c >> 4) & 15)) * m, (bz * 16 + (c >> 8)) * m);
-					if (vote >= 0) d.cachePages[level][(size_t)coordId * 4096 + c] = (unsigned short)vote;
-				}
-			};
-			if (inCap) { if (level > 0) for (unsigned i = tid; i < ntc; i += VXB_THREADS) cellWork(s.list[i]); } // level 0: the histogram is taken in pass A
-			else
-			{
-				for (int r = tid; r < 256; r += VXB_THREADS)
-				{
-					unsigned bits = reinterpret_cast<const unsigned short*>(s.nt32)[r];
-					while (bits) { const int x = __ffs(bits) - 1; bits &= bits - 1; cellWork(r * 16 + x); }
-				}
-			}
-			__syncthreads();
-			if (!inCap && emitMine) vxb_save_nt(d, s.emitIdx, s.nt32, s.wpre);
-		}
-
-		// every cell of every transition face votes too, trivial ones included (:1859) - observable at the next level
-		if (MODE != 0 && midLevel)
-		{
-			const VxbVoteSource voteSrc = vxb_vote_source(d, level);
-			if (tid < 8)
-			{
-				const int cnb = nb * 2;
-				const size_t cb = ((size_t)(bz * 2 + (tid >> 2)) * cnb + (by * 2 + ((tid >> 1) & 1))) * cnb + (bx * 2 + (tid & 1));
-				const bool valid = (level == 1) ? __ldcg(d.consValid + cb) : __ldcg(d.cacheValid[level - 1] + cb);
-				if (valid) atomicOr(&s.hasChild, 1u);
-			}
-			__syncthreads();
-			if (s.hasChild)
-			{
-				// an all-{EMPTY,0} page is indistinguishable from no page, so it can be created before the votes
-				if (!s.pageReady)
-				{
-					if (!d.cacheValid[level][coordId]) vxb_init_cache_page(d, level, coordId);
-					__syncthreads();
-					if (tid == 0) { d.cacheValid[level][coordId] = 1; s.pageReady = 1; }
-				}
-				for (int fc = tid; fc < 256; fc += VXB_THREADS)
-				{
-				const int row = fc >> 4, col = fc & 15;
-				// most face cells have no child with a material: test all six faces first (independent loads, all in flight
-				// together), then run the vote only where it can succeed
-				unsigned candidates = 0;
-#pragma unroll
-				for (int face = 0; face < 6; ++face)
-				{
-					int axis, ua, va;
-					vxb_face_axes(face, axis, ua, va);
-					const int bc = (axis == 0) ? bx : (axis == 1 ? by : bz);
-					const bool outside = face < 3 ? (bc == 0) : (bc == nb - 1); // neighbour block outside the grid (:1829-1835)
-					const int edge = (face >= 3) ? 15 : 0;
-					const int lx = axis == 0 ? edge : col, ly = axis == 1 ? edge : (axis == 2 ? row : col), lz = axis == 2 ? edge : row;
-					if (vxb_vote_candidate(voteSrc, (bx * 16 + lx) * m, (by * 16 + ly) * m, (bz * 16 + lz) * m) && !outside) candidates |= 1u << face;
-				}
-				while (candidates)
-				{
-					const int face = __ffs(candidates) - 1;
-					candidates &= candidates - 1;
-					int axis, ua, va;
-					vxb_face_axes(face, axis, ua, va);
-					// local[axis] = edge, local[ua] = col, local[va] = row, written with selects (an indexed array would be local memory)
-					const int edge = (face >= 3) ? 15 : 0;
-					const int local[3] = { axis == 0 ? edge : col, axis == 1 ? edge : (axis == 2 ? row : col), axis == 2 ? edge : row };
-					const int vote = vxb_vote_cell(voteSrc, (bx * 16 + local[0]) * m, (by * 16 + local[1]) * m, (bz * 16 + local[2]) * m);
-					if (vote >= 0) d.cachePages[level][(size_t)coordId * 4096 + local[2] * 256 + local[1] * 16 + local[0]] = (unsigned short)vote;
-				}
-				}
-			}
-		}
-		__syncthreads(); // the votes of this block are visible to the CTA (pass A reads the page back)
-		// coarse levels: the parent only needs this block's page, so it is released before the block's own emission work
-		if (MODE == 2 && tid == 0) { __threadfence(); *(volatile unsigned char*)(d.coarseDone + d.coarseBase[level] + coordId) = 1; }
-
-		if (ntc > 0 && !inCap)
-		{
-			if (tid == 0 && emitMine) d.bigList[atomicAdd(&d.counters->bigCount, 1u)] = s.emitIdx;
-		}
-		else if (ntc > 0 && emitMine)
-		{
-			unsigned nverts, ntris;
-			vxb_decide_cells<PITCH, ROWS, true>(s, tile, d, level, coordId, bx, by, bz, ntc, nverts, ntris);
-			const bool inCta = MODE == 0 && nverts <= (unsigned)VL_CAP;
-			if (MODE == 0 && !inCta)
+			unsigned nverts, ntris, voff, ioff, cellBase, slot;
+			vxb_decide_cells<VXB_DTILE_PITCH, 19, true>(s, tile, d, 0, coordId, bx, by, bz, ntc, nverts, ntris);
+			if (nverts > (unsigned)VxbBlockCaps<0>::VL)
 			{
 				// too many vertices for the in-CTA path: hand the block to vxb_big_block_kernel + the flat kernels
 				__syncthreads();
@@ -624,21 +564,10 @@ __global__ void __launch_bounds__(VXB_THREADS, VXB_OCC) vxb_block_kernel(const _
 			}
 			else
 			{
-				// four independent atomics from four warps: one round trip instead of four in a row
-				if (tid == 0) s.voff = atomicAdd(&d.counters->vertices, nverts);
-				if (tid == 32) s.ioff = atomicAdd(&d.counters->indices, ntris * 3);
-				if (tid == 64) s.cellBase = (MODE == 0) ? 0u : atomicAdd(&d.counters->cells, ntc);
-				if (tid == 96) s.slot = atomicAdd(&d.counters->records, 1u);
-				__syncthreads();
-				const unsigned voff = s.voff, ioff = s.ioff, cellBase = s.cellBase, slot = s.slot;
+				vxb_reserve(s, d, ntc, nverts, ntris, false, voff, ioff, cellBase, slot);
 				const bool fits = (unsigned long long)voff + nverts <= d.vcap && (unsigned long long)ioff + ntris * 3ull <= d.icap
 					&& (unsigned long long)cellBase + ntc <= d.ccap && slot < d.rcap;
-				if (fits && MODE != 0)
-				{
-					vxb_write_cell_records(s, d, ntc, voff, cellBase, slot);
-					vxb_save_nt(d, s.emitIdx, s.nt32, s.wpre);
-				}
-				if (fits && MODE == 0)
+				if (fits)
 				{
 					// ---- the block's new vertices, one thread each (:1576-1726), from the halo tile ----
 					for (unsigned i = tid; i < ntc; i += VXB_THREADS)
@@ -681,7 +610,7 @@ __global__ void __launch_bounds__(VXB_THREADS, VXB_OCC) vxb_block_kernel(const _
 						atomicOr(&s.used[matId >> 5], 1u << (matId & 31));
 					}
 					__syncthreads(); // the positions are read back by the degenerate test below
-					if (NBUF == 1 && nextItem < workCount) { int l2, x2, y2, z2; decode(nextItem, l2, x2, y2, z2); issue(0, l2, x2, y2, z2); nextIssued = true; } // the tile is not read any more
+					if (nextItem < workCount) { issue(nextItem); nextIssued = true; } // the tile is not read any more
 					// ---- triangles, one thread per non-trivial cell (:1714-1726 + the degenerate filter of :1300-1321) ----
 					// (the step of vxb_triangle_kernel with the owner records in shared memory; one function shared by the two
 					// gives vxb_triangle_kernel a 40th register)
@@ -740,22 +669,189 @@ __global__ void __launch_bounds__(VXB_THREADS, VXB_OCC) vxb_block_kernel(const _
 					}
 					if (removed) atomicAdd(&s.removed, removed);
 					__syncthreads();
+					if (tid == 0) vxb_write_block_rec(d, slot, 0, coordId, s.emitIdx, voff, ioff, cellBase, ntc, nverts, ntris, s.removed);
 				}
-				if (fits && tid == 0) vxb_write_block_rec(d, slot, level, coordId, s.emitIdx, voff, ioff, cellBase, ntc, nverts, ntris, (MODE == 0) ? s.removed : 0u);
 			}
 		}
-		if (AHEAD && tid == 0) s.ahead = ahead;
+		if (tid == 0) s.ahead = ahead;
 		__syncthreads();
-		if (NBUF == 1 && MODE != 2 && !nextIssued && nextItem < workCount) { int l2, x2, y2, z2; decode(nextItem, l2, x2, y2, z2); issue(0, l2, x2, y2, z2); }
+		if (!nextIssued && nextItem < workCount) issue(nextItem);
 		item = nextItem;
-		if (AHEAD) aheadItem = s.ahead;
-		if (NBUF == 2) buf ^= 1;
+		aheadItem = s.ahead;
 	}
+	vxb_block_epilogue(s, d, statNonTrivial);
+}
 
+// One level below the coarse ones (levelArg) from its work list.  17^3 tile (vxb_tile_issue: TMA on the even lattice of
+// level 1 / the level's lattice, strided gather else), double buffered: the next block's tile lands while this one is
+// worked on.  Writes 16-byte cell records + the vertex work list for the flat per-vertex / per-cell kernels.
+template <>
+__global__ void __launch_bounds__(VXB_THREADS, VXB_OCC) vxb_block_kernel<1>(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB, const VxbDev d, const int levelArg)
+{
+	extern __shared__ __align__(128) unsigned char smemRaw[];
+	VxbBlockSmem<1>& s = *reinterpret_cast<VxbBlockSmem<1>*>(smemRaw);
+	const int tid = threadIdx.x;
+	const int level = levelArg;
+	unsigned phaseBits = 0, statNonTrivial = 0; // mbarrier phase of each tile buffer, bit = buffer
+	vxb_block_prologue(s);
+	const unsigned workCount = d.counters->workCount[level];
+	const unsigned* const worklist = d.worklist + d.workBase[level];
+	unsigned* const cursor = &d.counters->workCursor[level];
+	auto issue = [&](int buf, unsigned it) { int x, y, z; vxb_work_block(d, worklist, it, level, x, y, z); vxb_tile_issue(s.tiles[buf], &s.mbar[buf], &tmapA, &tmapB, d, level, x, y, z); };
+
+	if (tid == 0) s.item = atomicAdd(cursor, 1u);
 	__syncthreads();
-	if (tid < 16 && s.hist[tid]) atomicAdd(&d.counters->perCase[tid], s.hist[tid]);
-	if (tid < 8 && s.used[tid]) atomicOr(&d.counters->usedMaterials[tid], s.used[tid]);
-	if (tid == 0 && statNonTrivial) atomicAdd(&d.counters->nonTrivial, statNonTrivial);
+	unsigned item = s.item;
+	int buf = 0;
+	if (item < workCount) issue(0, item);
+	__syncthreads();
+	while (item < workCount)
+	{
+		vxb_take_item(s, cursor);
+		__syncthreads();
+		const unsigned nextItem = s.item;
+		if (nextItem < workCount) issue(buf ^ 1, nextItem);
+		int bx, by, bz;
+		vxb_work_block(d, worklist, item, level, bx, by, bz);
+		const int nb = d.n / 16 / (1 << level);
+		const unsigned coordId = ((unsigned)bz * nb + by) * nb + bx;
+		const bool midLevel = level > 0 && level != d.lastLevel;
+		const signed char* const tile = s.tiles[buf];
+		unsigned ph = (phaseBits >> buf) & 1u;
+		vxb_tile_complete(s.tiles[buf], &s.mbar[buf], ph, d, level, bx, by, bz);
+		phaseBits = (phaseBits & ~(1u << buf)) | (ph << buf);
+		__syncthreads();
+
+		const unsigned ntc = vxb_count_cells<VXB_TILE_PITCH, 17>(s, tile);
+		const bool inCap = ntc <= (unsigned)VxbBlockCaps<1>::CAP;
+		if (ntc > 0) vxb_block_cells<VXB_TILE_PITCH, 17>(s, tile, d, level, coordId, bx, by, bz, ntc, inCap, true, statNonTrivial);
+		if (midLevel) vxb_face_votes(s, d, level, nb, coordId, bx, by, bz);
+		__syncthreads(); // the votes of this block are visible to the CTA (pass A reads the page back)
+		if (ntc > 0 && !inCap) { if (tid == 0) d.bigList[atomicAdd(&d.counters->bigCount, 1u)] = s.emitIdx; }
+		else if (ntc > 0) vxb_emit_cell_records(s, tile, d, level, coordId, bx, by, bz, ntc);
+		__syncthreads();
+		item = nextItem;
+		buf ^= 1;
+	}
+	vxb_block_epilogue(s, d, statNonTrivial);
+}
+
+// All coarse levels [coarseLo, computed) in ONE launch: items = the blocks in level order from one cursor.  A block waits
+// for its children, applies the block-walk test itself, then works like <1>; it is released to its parent right after its
+// votes.
+template <>
+__global__ void __launch_bounds__(VXB_THREADS, VXB_OCC) vxb_block_kernel<2>(const __grid_constant__ CUtensorMap, const __grid_constant__ CUtensorMap, const VxbDev d, const int)
+{
+	extern __shared__ __align__(128) unsigned char smemRaw[];
+	VxbBlockSmem<2>& s = *reinterpret_cast<VxbBlockSmem<2>*>(smemRaw);
+	const int tid = threadIdx.x;
+	unsigned phase = 0, statNonTrivial = 0;
+	vxb_block_prologue(s);
+	if (tid == 0)
+	{
+		unsigned acc = 0;
+		for (int l = d.coarseLo; l < d.computed; ++l)
+		{
+			const int nbl = (d.n >> 4) >> l;
+			const int nx = d.ranged ? d.rangeMax[l][0] - d.rangeMin[l][0] : nbl, ny = d.ranged ? d.rangeMax[l][1] - d.rangeMin[l][1] : nbl, nz = d.ranged ? d.rangeMax[l][2] - d.rangeMin[l][2] : nbl;
+			acc += (nx > 0 && ny > 0 && nz > 0) ? (unsigned)nx * ny * nz : 0u;
+			s.levelEnd[l - d.coarseLo] = acc; // end of the items of level l
+		}
+	}
+	__syncthreads();
+	const unsigned workCount = (d.computed > d.coarseLo) ? s.levelEnd[d.computed - d.coarseLo - 1] : 0u;
+	unsigned* const cursor = &d.counters->coarseCursor;
+
+	if (tid == 0) s.item = atomicAdd(cursor, 1u);
+	__syncthreads();
+	unsigned item = s.item;
+	__syncthreads();
+	while (item < workCount)
+	{
+		vxb_take_item(s, cursor);
+		__syncthreads();
+		const unsigned nextItem = s.item;
+		int q = 0;
+		while (item >= s.levelEnd[q]) ++q;
+		const int level = d.coarseLo + q, nbl = (d.n >> 4) >> level;
+		const unsigned r = item - (q ? s.levelEnd[q - 1] : 0u);
+		const int x0 = d.ranged ? d.rangeMin[level][0] : 0, y0 = d.ranged ? d.rangeMin[level][1] : 0, z0 = d.ranged ? d.rangeMin[level][2] : 0;
+		const int nx = d.ranged ? d.rangeMax[level][0] - x0 : nbl, ny = d.ranged ? d.rangeMax[level][1] - y0 : nbl;
+		const int bx = x0 + (int)(r % nx), by = y0 + (int)((r / nx) % ny), bz = z0 + (int)(r / ((unsigned)nx * ny));
+		const int nb = d.n / 16 / (1 << level);
+		const unsigned coordId = ((unsigned)bz * nb + by) * nb + bx;
+		const bool midLevel = level > 0 && level != d.lastLevel;
+
+		// warp 0: wait for the children of this run (blocks of the previous coarse level inside the run's range), one lane
+		// each, then the block walk test (vxb_coarse_block_needed) with one lane per child-level neighbour.  The children
+		// were taken earlier from the same cursor, so they are running or done: no deadlock.
+		if (tid < 32)
+		{
+			const int cnb = nb * 2, cl = level - 1;
+			if (level > d.coarseLo && tid < 8)
+			{
+				const int cx = bx * 2 + (tid & 1), cy = by * 2 + ((tid >> 1) & 1), cz = bz * 2 + (tid >> 2);
+				const bool inRun = !(d.ranged && (cx < d.rangeMin[cl][0] || cx >= d.rangeMax[cl][0] || cy < d.rangeMin[cl][1] || cy >= d.rangeMax[cl][1] || cz < d.rangeMin[cl][2] || cz >= d.rangeMax[cl][2]));
+				if (inRun)
+				{
+					const volatile unsigned char* flag = d.coarseDone + d.coarseBase[cl] + ((size_t)cz * cnb + cy) * cnb + cx;
+					unsigned spins = 0;
+					while (!*flag) { __nanosleep(32); if (++spins > (1u << 24)) __trap(); }
+				}
+				__threadfence();
+			}
+			__syncwarp();
+			unsigned u = 0, anyChild = 0;
+			if (tid < 27)
+			{
+				const int x = tid % 3, y = (tid / 3) % 3, z = tid / 9;
+				const int cx = min(2 * bx + x, cnb - 1), cy = min(2 * by + y, cnb - 1), cz = min(2 * bz + z, cnb - 1);
+				const size_t cb = ((size_t)cz * cnb + cy) * cnb + cx;
+				u = d.mixInfo[cl][cb];
+				if (x < 2 && y < 2 && z < 2) anyChild = __ldcg(d.cacheValid[cl] + cb);
+			}
+			u = __reduce_or_sync(0xFFFFFFFFu, u);
+			anyChild = __reduce_or_sync(0xFFFFFFFFu, anyChild);
+			if (tid == 0)
+			{
+				s.take = (u == 3u || anyChild != 0u) ? 1u : 0u;
+				if (s.take)
+				{
+					// the block's 17^3 samples: one TMA box of the level's lattice (far-edge entries included, no fix-up)
+					vxb_fence_proxy_async();
+					vxb_mbar_expect_tx(&s.mbar[0], VXB_TILE_BYTES);
+					vxb_tma_load_3d(s.tiles[0], d.coarseMaps + level, bx * 16, by * 16, bz * 16, &s.mbar[0]);
+				}
+			}
+		}
+		__syncthreads();
+		if (!s.take)
+		{
+			if (tid == 0) { __threadfence(); *(volatile unsigned char*)(d.coarseDone + d.coarseBase[level] + coordId) = 1; }
+			__syncthreads();
+			item = nextItem;
+			continue;
+		}
+		const signed char* const tile = s.tiles[0];
+		vxb_mbar_wait(&s.mbar[0], phase);
+		phase ^= 1u;
+		__syncthreads();
+
+		const unsigned ntc = vxb_count_cells<VXB_TILE_PITCH, 17>(s, tile);
+		const bool inCap = ntc <= (unsigned)VxbBlockCaps<2>::CAP;
+		// sharded runs: every rank classifies the coarse levels (the votes feed the next level), one of them emits the block
+		const bool emitMine = vxb_coarse_emit_is_mine(d, level, coordId);
+		if (ntc > 0) vxb_block_cells<VXB_TILE_PITCH, 17>(s, tile, d, level, coordId, bx, by, bz, ntc, inCap, emitMine, statNonTrivial);
+		if (midLevel) vxb_face_votes(s, d, level, nb, coordId, bx, by, bz);
+		__syncthreads(); // the votes of this block are visible to the CTA (pass A reads the page back)
+		// the parent only needs this block's page, so it is released before the block's own emission work
+		if (tid == 0) { __threadfence(); *(volatile unsigned char*)(d.coarseDone + d.coarseBase[level] + coordId) = 1; }
+		if (ntc > 0 && !inCap) { if (tid == 0 && emitMine) d.bigList[atomicAdd(&d.counters->bigCount, 1u)] = s.emitIdx; }
+		else if (ntc > 0 && emitMine) vxb_emit_cell_records(s, tile, d, level, coordId, bx, by, bz, ntc);
+		__syncthreads();
+		item = nextItem;
+	}
+	vxb_block_epilogue(s, d, statNonTrivial);
 }
 
 // ------------------------------------------------------------------------------------------------
