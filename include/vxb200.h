@@ -860,6 +860,76 @@ int vxb_mesh_sphere_cast_cut_device(vxb_mesh* mesh, const float lod_camera[3], f
 int vxb_mesh_closest_point_cut_device(vxb_mesh* mesh, const float lod_camera[3], float lod_factor, float max_distance,
                                       const float* points, uint32_t count, vxb_closest_cut_hit* hits);
 
+/* ---- capsule queries against the drawn LOD cut: capsule sweeps and closest points to segments on what the renderer shows --
+ * The capsule queries above answer about the level-0 surface; a capsule character standing on a drawn level-l block would
+ * float above the triangles on screen or sink into them by up to 2^l voxels, and its penetration depth r - distance would
+ * be measured against a surface nobody sees.  vxb_mesh_capsule_cast_cut and vxb_mesh_closest_to_segment_cut answer about the
+ * triangles the renderer draws for the cut of (lod_camera, lod_factor).
+ *   The drawn set   vxb_mesh_raycast_cut's (see "collision queries against the drawn LOD cut").
+ *   The tests       vxb_mesh_capsule_cast's sweep (the closest pair at c0; the caps, the parallelograms, the cap and lateral
+ *                   edges, the shifted vertices) and vxb_mesh_closest_to_segment's closest pair, unchanged, on the selected
+ *                   positions.  center, point, axis_point, u, v, s and the blended normal are computed as there, on the
+ *                   drawn triangle's nrm.
+ *   The hit         Least t (sweeps) or dd (segments); ties go to the lower slot, then to the lower part (the regular mesh
+ *                   before transition face 0, ..., face 5), then to the lower triangle: vxb_mesh_raycast_cut's rule.  level
+ *                   and face as in vxb_sphere_cut_hit.  A miss is the level-0 query's miss with level and face 0.
+ *   At lod_factor = 1e30 the first 80 bytes (sweeps) or 64 bytes (segments) of every hit equal vxb_mesh_capsule_cast's or
+ *                   vxb_mesh_closest_to_segment's, with level = 0 and face = 0xFFFFFFFF on a hit.
+ *   The reach       A query's reach R is max_i |h_i| + r for a sweep and max_i |h_i| + max_distance for a segment.  Unlike
+ *                   the sphere cut's radius, R travels with each query, so the cut reach rule is per query: a query is in
+ *                   reach when it passes the level-0 capsule queries' rule and, in float and in this order,
+ *                   e + (max_i |h_i| + r) <= 15 (sweeps) or e + (max_i |h_i| + max_distance) <= 15 (segments), e the mesh's
+ *                   excursion.  With h = 0 this is the sphere cut's e + R <= 15.  A contact or closest pair then puts the
+ *                   centre within e + R + 1/16 < 16 voxels of the drawn block's lattice box, one of the 27 neighbours of
+ *                   its block.  The first cut query after an apply (of any kind) rebuilds the all-level map, measures e and
+ *                   waits for the stream once.
+ * Refusals (`hits` untouched), in this order: VXB_ERR_ARGUMENT for a NULL pointer with count > 0, a bad lod_factor or
+ * lod_camera (as vxb_mesh_raycast_cut), and a max_distance outside 0 <= m <= 15; VXB_ERR_STATE before the first apply and
+ * for a mesh without every level and transition mesh (as vxb_mesh_select_cut); count = 0 does nothing; the HOST variants'
+ * per-query rule of vxb_mesh_capsule_cast and vxb_mesh_closest_to_segment (VXB_ERR_ARGUMENT, naming the index); after the
+ * map, VXB_ERR_STATE when e + 1/16 > 15 and, for segments, when e + max_distance > 15; then, HOST variants only,
+ * VXB_ERR_STATE for the first query out of cut reach (vxb_last_error names its index, e and its R).
+ * The DEVICE variants answer an invalid query and a query out of cut reach with a miss and the rest of the batch as usual.
+ * This differs from vxb_mesh_sphere_cast_cut_device, whose one radius serves the whole batch, so that there the whole call
+ * is refused. */
+typedef struct vxb_capsule_cut_hit
+{
+	float t;                /* as vxb_capsule_hit: the first 80 bytes are its fields */
+	uint32_t slot;          /* mesh directory slot of the drawn block; VXB_RAY_MISS */
+	uint32_t block_id;
+	uint32_t triangle;      /* k: indices [part offset + 3k, +3) of the part `face` names (as vxb_cut_hit) */
+	float center[3];
+	float point[3];         /* the contact point on the drawn triangle */
+	float axis_point[3];    /* center + s * half_axis */
+	float normal[3];
+	float u, v, s;
+	uint32_t flags;         /* VXB_SPHERE_STARTED_IN_CONTACT */
+	uint32_t level;         /* the hit block's level */
+	uint32_t face;          /* 0xFFFFFFFF: the regular mesh; f: the transition mesh of face f (TransitionFaceId order) */
+} vxb_capsule_cut_hit;                                                     /* 88 bytes; the first 80 are vxb_capsule_hit's */
+typedef struct vxb_segment_cut_hit
+{
+	float distance;         /* as vxb_segment_hit: the first 64 bytes are its fields */
+	uint32_t slot;
+	uint32_t block_id;
+	uint32_t triangle;
+	float point[3];         /* the closest point of the drawn surface within max_distance of the segment */
+	float axis_point[3];
+	float normal[3];
+	float u, v, s;
+	uint32_t level, face;   /* as vxb_capsule_cut_hit */
+} vxb_segment_cut_hit;                                                     /* 72 bytes; the first 64 are vxb_segment_hit's */
+/* HOST memory; block until the hits are written. */
+int vxb_mesh_capsule_cast_cut(vxb_mesh* mesh, const float lod_camera[3], float lod_factor,
+                              const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_cut_hit* hits);
+int vxb_mesh_closest_to_segment_cut(vxb_mesh* mesh, const float lod_camera[3], float lod_factor, float max_distance,
+                                    const vxb_segment* segments, uint32_t count, vxb_segment_cut_hit* hits);
+/* DEVICE memory; enqueued on vxb_stream(ctx) like vxb_mesh_raycast_cut_device (the first cut query after an apply waits). */
+int vxb_mesh_capsule_cast_cut_device(vxb_mesh* mesh, const float lod_camera[3], float lod_factor,
+                                     const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_cut_hit* hits);
+int vxb_mesh_closest_to_segment_cut_device(vxb_mesh* mesh, const float lod_camera[3], float lod_factor, float max_distance,
+                                           const vxb_segment* segments, uint32_t count, vxb_segment_cut_hit* hits);
+
 /* ---- box overlap gathers: the level-0 triangles in axis-aligned boxes, for a client's physics mid-phase and navmesh tiles --
  * Every other query returns one answer per query; vxb_mesh_overlap_box returns, per box, every triangle that overlaps it, so
  * that a physics engine runs its own narrowphase for its own shapes (processAllTriangles-style callbacks), a navmesh builder

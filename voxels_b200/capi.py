@@ -210,6 +210,11 @@ SEGMENT_HIT_DTYPE = np.dtype([("distance", "<f4"), ("slot", "<u4"), ("block_id",
                               ("axis_point", "<f4", 3), ("normal", "<f4", 3), ("u", "<f4"), ("v", "<f4"), ("s", "<f4")])
 assert CAPSULE_SWEEP_DTYPE.itemsize == 48 and SEGMENT_DTYPE.itemsize == 24
 assert CAPSULE_HIT_DTYPE.itemsize == 80 and SEGMENT_HIT_DTYPE.itemsize == 64
+# vxb_capsule_cut_hit / vxb_segment_cut_hit (include/vxb200.h "capsule queries against the drawn LOD cut"): the level-0 hits,
+# then level and face
+CAPSULE_CUT_HIT_DTYPE = np.dtype(CAPSULE_HIT_DTYPE.descr + [("level", "<u4"), ("face", "<u4")])
+SEGMENT_CUT_HIT_DTYPE = np.dtype(SEGMENT_HIT_DTYPE.descr + [("level", "<u4"), ("face", "<u4")])
+assert CAPSULE_CUT_HIT_DTYPE.itemsize == 88 and SEGMENT_CUT_HIT_DTYPE.itemsize == 72
 
 # vxb_box / vxb_overlap_triangle (include/vxb200.h "box overlap gathers")
 BOX_DTYPE = np.dtype([("min", "<f4", 3), ("max", "<f4", 3)])
@@ -397,6 +402,10 @@ def load_library():
         "vxb_mesh_capsule_cast_device": (C.c_int, [vp, vp, u32, vp]),
         "vxb_mesh_closest_to_segment": (C.c_int, [vp, C.c_float, vp, u32, vp]),
         "vxb_mesh_closest_to_segment_device": (C.c_int, [vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_capsule_cast_cut": (C.c_int, [vp, vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_capsule_cast_cut_device": (C.c_int, [vp, vp, C.c_float, vp, u32, vp]),
+        "vxb_mesh_closest_to_segment_cut": (C.c_int, [vp, vp, C.c_float, C.c_float, vp, u32, vp]),
+        "vxb_mesh_closest_to_segment_cut_device": (C.c_int, [vp, vp, C.c_float, C.c_float, vp, u32, vp]),
         "vxb_mesh_overlap_box": (C.c_int, [vp, vp, u32, vp, vp, u64]),
         "vxb_mesh_overlap_box_device": (C.c_int, [vp, vp, u32, vp, vp, u64]),
         "vxb_host_alloc": (vp, [C.c_size_t]),
@@ -426,7 +435,9 @@ EXPORTED_SYMBOLS = ["vxb_create", "vxb_destroy", "vxb_last_error", "vxb_stream",
                     "vxb_mesh_sphere_cast_cut", "vxb_mesh_sphere_cast_cut_device", "vxb_mesh_closest_point_cut",
                     "vxb_mesh_closest_point_cut_device",
                     "vxb_mesh_capsule_cast", "vxb_mesh_capsule_cast_device", "vxb_mesh_closest_to_segment",
-                    "vxb_mesh_closest_to_segment_device", "vxb_mesh_overlap_box", "vxb_mesh_overlap_box_device"]
+                    "vxb_mesh_closest_to_segment_device", "vxb_mesh_capsule_cast_cut", "vxb_mesh_capsule_cast_cut_device",
+                    "vxb_mesh_closest_to_segment_cut", "vxb_mesh_closest_to_segment_cut_device", "vxb_mesh_overlap_box",
+                    "vxb_mesh_overlap_box_device"]
 
 
 def nccl_unique_id():
@@ -810,6 +821,53 @@ class Mesh:
         enqueued on the context's stream, returns without waiting."""
         self.ctx._check(self.L.vxb_mesh_closest_to_segment_device(self.h, max_distance, _dev(segments_ptr), count, _dev(hits_ptr)),
                         "vxb_mesh_closest_to_segment_device")
+
+    def capsule_cast_cut_rc(self, lod_camera, lod_factor, sweeps, hits=None, count=None):
+        """vxb_mesh_capsule_cast_cut's return code: `lod_camera` and `sweeps` (a CAPSULE_SWEEP_DTYPE array) may be None for NULL
+        pointers, `hits` (a CAPSULE_CUT_HIT_DTYPE array) None for a NULL pointer; `count` defaults to len(sweeps)."""
+        sweeps = _batch(sweeps, CAPSULE_SWEEP_DTYPE)
+        n = (0 if sweeps is None else len(sweeps)) if count is None else count
+        return self.L.vxb_mesh_capsule_cast_cut(self.h, _ptr(_batch(lod_camera, np.float32)), lod_factor, _ptr(sweeps), n, _ptr(hits))
+
+    def capsule_cast_cut(self, lod_camera, lod_factor, sweeps):
+        """Sweeps capsules (a CAPSULE_SWEEP_DTYPE array, make_capsule_sweeps) against the triangles vxb_mesh_select_cut's cut of
+        (lod_camera, lod_factor) draws (vxb_mesh_capsule_cast_cut).  Returns a CAPSULE_CUT_HIT_DTYPE array."""
+        sweeps = np.ascontiguousarray(sweeps, CAPSULE_SWEEP_DTYPE)
+        hits = np.zeros(len(sweeps), CAPSULE_CUT_HIT_DTYPE)
+        self.ctx._check(self.capsule_cast_cut_rc(lod_camera, lod_factor, sweeps, hits), "vxb_mesh_capsule_cast_cut")
+        return hits
+
+    def capsule_cast_cut_device(self, lod_camera, lod_factor, sweeps_ptr, count, hits_ptr):
+        """vxb_mesh_capsule_cast_cut_device: `count` vxb_capsule_sweep at the device address `sweeps_ptr`, hits to `hits_ptr`;
+        enqueued on the context's stream (the first cut query after an apply waits for it once).  A sweep out of reach is a
+        miss."""
+        self.ctx._check(self.L.vxb_mesh_capsule_cast_cut_device(self.h, _ptr(_batch(lod_camera, np.float32)), lod_factor,
+                                                                _dev(sweeps_ptr), count, _dev(hits_ptr)), "vxb_mesh_capsule_cast_cut_device")
+
+    def closest_to_segment_cut_rc(self, lod_camera, lod_factor, max_distance, segments, hits=None, count=None):
+        """vxb_mesh_closest_to_segment_cut's return code: `lod_camera` and `segments` (a SEGMENT_DTYPE array) may be None for
+        NULL pointers, `hits` (a SEGMENT_CUT_HIT_DTYPE array) None for a NULL pointer; `count` defaults to len(segments)."""
+        segments = _batch(segments, SEGMENT_DTYPE)
+        n = (0 if segments is None else len(segments)) if count is None else count
+        return self.L.vxb_mesh_closest_to_segment_cut(self.h, _ptr(_batch(lod_camera, np.float32)), lod_factor, max_distance,
+                                                      _ptr(segments), n, _ptr(hits))
+
+    def closest_to_segment_cut(self, lod_camera, lod_factor, segments, max_distance):
+        """The nearest drawn surface point of the cut of (lod_camera, lod_factor) within `max_distance` voxels of each segment
+        (a SEGMENT_DTYPE array, make_segments), vxb_mesh_closest_to_segment_cut.  Returns a SEGMENT_CUT_HIT_DTYPE array."""
+        segments = np.ascontiguousarray(segments, SEGMENT_DTYPE)
+        hits = np.zeros(len(segments), SEGMENT_CUT_HIT_DTYPE)
+        self.ctx._check(self.closest_to_segment_cut_rc(lod_camera, lod_factor, max_distance, segments, hits),
+                        "vxb_mesh_closest_to_segment_cut")
+        return hits
+
+    def closest_to_segment_cut_device(self, lod_camera, lod_factor, max_distance, segments_ptr, count, hits_ptr):
+        """vxb_mesh_closest_to_segment_cut_device: `count` vxb_segment at the device address `segments_ptr`, hits to
+        `hits_ptr`; enqueued on the context's stream (the first cut query after an apply waits for it once).  A segment out of
+        reach is a miss."""
+        self.ctx._check(self.L.vxb_mesh_closest_to_segment_cut_device(self.h, _ptr(_batch(lod_camera, np.float32)), lod_factor,
+                                                                      max_distance, _dev(segments_ptr), count, _dev(hits_ptr)),
+                        "vxb_mesh_closest_to_segment_cut_device")
 
     def overlap_boxes_rc(self, boxes, offsets, tris=None, capacity=None, count=None):
         """vxb_mesh_overlap_box's return code for a BOX_DTYPE array (or None for a NULL pointer): offsets to `offsets` (a uint64

@@ -47,6 +47,8 @@ static_assert(sizeof(vxb_view) == 96 && sizeof(vxb_mesh_bounds) == 64 && VXB_MAX
 static_assert(sizeof(vxb_cut_hit) == 56 && offsetof(vxb_cut_hit, level) == 48, "vxb_cut_hit layout");
 static_assert(sizeof(vxb_sphere_cut_hit) == 72 && offsetof(vxb_sphere_cut_hit, level) == 64 && sizeof(vxb_closest_cut_hit) == 56 &&
 	offsetof(vxb_closest_cut_hit, level) == 48, "cut collision layouts");
+static_assert(sizeof(vxb_capsule_cut_hit) == 88 && offsetof(vxb_capsule_cut_hit, level) == 80 && sizeof(vxb_segment_cut_hit) == 72 &&
+	offsetof(vxb_segment_cut_hit, level) == 64, "cut capsule layouts");
 static_assert(sizeof(vxb_box) == 24 && sizeof(vxb_overlap_triangle) == 48, "overlap layouts");
 
 namespace
@@ -2335,6 +2337,7 @@ int ensureCutMap(vxb_mesh* m, const char* what, float reach, VxbCutRayMesh& c)
 	c.slots = a;
 	c.top = (int)m->info.levels - 1;
 	c.grow = std::nextafter(m->excursion + VXB_RAY_EPS, INFINITY);
+	c.excursion = m->excursion;
 	memset(&c.cut, 0, sizeof(c.cut));
 	return VXB_OK;
 }
@@ -2359,13 +2362,15 @@ int launchLevel0(vxb_mesh* m, Kernel kernel, unsigned threads, uint32_t count, A
 }
 
 // A cut query's launch on ctx->stream: `kernel(c, args...)`, one warp per query over the all-level map (ensureCutMap, with
-// the query's reach) and the cut of (camera, lodFactor).
-template <class Kernel, class... Args>
-int launchCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, float reach, Kernel kernel, unsigned threads,
-	uint32_t count, Args... args)
+// the batch's reach) and the cut of (camera, lodFactor).  `inReach(e)` runs between the map and the launch: the host capsule
+// variants' per-query reach check against the excursion e (anyReach for every other query).
+template <class InReach, class Kernel, class... Args>
+int launchCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, float reach, InReach&& inReach, Kernel kernel,
+	unsigned threads, uint32_t count, Args... args)
 {
 	VxbCutRayMesh c;
-	const int e = ensureCutMap(m, what, reach, c);
+	int e = ensureCutMap(m, what, reach, c);
+	if (e == VXB_OK) e = inReach(c.excursion);
 	if (e != VXB_OK) return e;
 	for (int k = 0; k < 3; ++k) c.cut.camera[k] = camera[k];
 	c.cut.lod = lodFactor;
@@ -2374,22 +2379,72 @@ int launchCut(vxb_mesh* m, const char* what, const float camera[3], float lodFac
 	return VXB_OK;
 }
 
+int anyReach(float) { return VXB_OK; }
+
 int enqueueRaycastCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, const vxb_ray* rays, uint32_t count, vxb_cut_hit* hits)
 {
-	return launchCut(m, what, camera, lodFactor, 0.f, vxb_raycast_cut_kernel, VXB_RAY_THREADS, count, rays, count, hits);
+	return launchCut(m, what, camera, lodFactor, 0.f, anyReach, vxb_raycast_cut_kernel, VXB_RAY_THREADS, count, rays, count, hits);
 }
 
 int enqueueSphereCastCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, float radius, const vxb_ray* rays,
 	uint32_t count, vxb_sphere_cut_hit* hits)
 {
-	return launchCut(m, what, camera, lodFactor, radius, vxb_sphere_cast_cut_kernel, VXB_COLLIDE_THREADS, count, radius, rays, count, hits);
+	return launchCut(m, what, camera, lodFactor, radius, anyReach, vxb_sphere_cast_cut_kernel, VXB_COLLIDE_THREADS, count, radius, rays, count, hits);
 }
 
 int enqueueClosestPointCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, float maxDistance, const float* points,
 	uint32_t count, vxb_closest_cut_hit* hits)
 {
-	return launchCut(m, what, camera, lodFactor, maxDistance, vxb_closest_point_cut_kernel, VXB_COLLIDE_THREADS, count, maxDistance,
+	return launchCut(m, what, camera, lodFactor, maxDistance, anyReach, vxb_closest_point_cut_kernel, VXB_COLLIDE_THREADS, count, maxDistance,
 		points, count, hits);
+}
+
+// The host capsule cut queries' per-query reach (vxb_capsule_cut_reach) against the excursion e: the first of the `count`
+// queries out of reach is refused with VXB_ERR_STATE, naming its index, e and its reach R.  shape(i, h, extra) gives query
+// i's half axis and its radius or max_distance.  NULL `noun`: the device variants, whose kernels answer such a query with a
+// miss.
+template <class Shape>
+int capsuleCutReach(vxb_mesh* m, const char* what, const char* noun, uint32_t count, float e, Shape&& shape)
+{
+	if (!noun) return VXB_OK;
+	for (uint32_t i = 0; i < count; ++i)
+	{
+		float3 h;
+		float extra;
+		shape(i, h, extra);
+		if (vxb_capsule_cut_reach(h, extra, e)) continue;
+		char buf[256];
+		snprintf(buf, sizeof(buf), "%s: %s %u: a block's vertices leave its lattice box by %g voxels (e) and the %s reaches %g (R); "
+			"e + R must be at most 15", what, noun, i, (double)e, noun, (double)(std::max(std::max(std::fabs(h.x), std::fabs(h.y)), std::fabs(h.z)) + extra));
+		return fail(m->ctx, VXB_ERR_STATE, buf);
+	}
+	return VXB_OK;
+}
+
+// `checked`: the host copy of the queries for the host variant's reach check, NULL for the device variant
+int enqueueCapsuleCastCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, const vxb_capsule_sweep* checked,
+	const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_cut_hit* hits)
+{
+	const auto inReach = [&](float e) {
+		return capsuleCutReach(m, what, checked ? "sweep" : nullptr, count, e, [&](uint32_t i, float3& h, float& extra) {
+			h = make_float3(checked[i].half_axis[0], checked[i].half_axis[1], checked[i].half_axis[2]);
+			extra = checked[i].radius;
+		});
+	};
+	return launchCut(m, what, camera, lodFactor, 0.f, inReach, vxb_capsule_cast_cut_kernel, VXB_COLLIDE_THREADS, count, sweeps, count, hits);
+}
+
+int enqueueClosestToSegmentCut(vxb_mesh* m, const char* what, const float camera[3], float lodFactor, float maxDistance,
+	const vxb_segment* checked, const vxb_segment* segments, uint32_t count, vxb_segment_cut_hit* hits)
+{
+	const auto inReach = [&](float e) {
+		return capsuleCutReach(m, what, checked ? "segment" : nullptr, count, e, [&](uint32_t i, float3& h, float& extra) {
+			h = make_float3(checked[i].half_axis[0], checked[i].half_axis[1], checked[i].half_axis[2]);
+			extra = maxDistance;
+		});
+	};
+	return launchCut(m, what, camera, lodFactor, maxDistance, inReach, vxb_closest_segment_cut_kernel, VXB_COLLIDE_THREADS, count,
+		maxDistance, segments, count, hits);
 }
 
 // the gather kernels' view of the mesh: the level-0 map (ensureMap) and the level-0 bounds
@@ -2991,17 +3046,28 @@ int vxb_mesh_closest_point_cut_device(vxb_mesh* m, const float camera[3], float 
 		[&] { return enqueueClosestPointCut(m, what, camera, lodFactor, maxDistance, points, count, hits); });
 }
 
+// the host variants' capsule rules (include/vxb200.h "capsule queries"): why the query is refused, or NULL
+const char* sweepFault(const vxb_capsule_sweep& s)
+{
+	if (const char* why = rayFault(s.path)) return why;
+	if (!(s.radius > 0.f)) return "radius must be > 0";
+	if (!vxb_capsule_reach(make_float3(s.half_axis[0], s.half_axis[1], s.half_axis[2]), s.radius))
+		return "non-finite half axis or radius, or max |half_axis| + radius above 15";
+	return nullptr;
+}
+const char* segmentFault(const vxb_segment& s, float maxDistance)
+{
+	const float* c = s.center;
+	const float* h = s.half_axis;
+	if (!std::isfinite(c[0]) || !std::isfinite(c[1]) || !std::isfinite(c[2])) return "non-finite centre";
+	if (!vxb_capsule_reach(make_float3(h[0], h[1], h[2]), maxDistance)) return "non-finite half axis, or max |half_axis| + max_distance above 15";
+	return nullptr;
+}
+
 int vxb_mesh_capsule_cast(vxb_mesh* m, const vxb_capsule_sweep* sweeps, uint32_t count, vxb_capsule_hit* hits)
 {
-	const auto sweepFault = [=](uint32_t i) -> const char* {
-		const vxb_capsule_sweep& s = sweeps[i];
-		if (const char* why = rayFault(s.path)) return why;
-		if (!(s.radius > 0.f)) return "radius must be > 0";
-		if (!vxb_capsule_reach(make_float3(s.half_axis[0], s.half_axis[1], s.half_axis[2]), s.radius))
-			return "non-finite half axis or radius, or max |half_axis| + radius above 15";
-		return nullptr;
-	};
-	return meshQuery(m, { "vxb_mesh_capsule_cast", !sweeps || !hits, "sweeps or hits", nullptr }, count, rule("sweep", sweepFault), [&] {
+	return meshQuery(m, { "vxb_mesh_capsule_cast", !sweeps || !hits, "sweeps or hits", nullptr }, count,
+		rule("sweep", [=](uint32_t i) { return sweepFault(sweeps[i]); }), [&] {
 		return hostQuery(m, sweeps, sizeof(vxb_capsule_sweep) * count, count, hits, [&](const vxb_capsule_sweep* in, vxb_capsule_hit* out) {
 			return launchLevel0(m, vxb_capsule_cast_kernel, VXB_COLLIDE_THREADS, count, in, count, out); }); });
 }
@@ -3014,15 +3080,8 @@ int vxb_mesh_capsule_cast_device(vxb_mesh* m, const vxb_capsule_sweep* sweeps, u
 
 int vxb_mesh_closest_to_segment(vxb_mesh* m, float maxDistance, const vxb_segment* segments, uint32_t count, vxb_segment_hit* hits)
 {
-	const auto segmentFault = [=](uint32_t i) -> const char* {
-		const float* c = segments[i].center;
-		const float* h = segments[i].half_axis;
-		if (!std::isfinite(c[0]) || !std::isfinite(c[1]) || !std::isfinite(c[2])) return "non-finite centre";
-		if (!vxb_capsule_reach(make_float3(h[0], h[1], h[2]), maxDistance)) return "non-finite half axis, or max |half_axis| + max_distance above 15";
-		return nullptr;
-	};
 	return meshQuery(m, { "vxb_mesh_closest_to_segment", !segments || !hits, "segments or hits", maxDistanceFault(maxDistance) }, count,
-		rule("segment", segmentFault), [&] {
+		rule("segment", [=](uint32_t i) { return segmentFault(segments[i], maxDistance); }), [&] {
 			return hostQuery(m, segments, sizeof(vxb_segment) * count, count, hits, [&](const vxb_segment* in, vxb_segment_hit* out) {
 				return launchLevel0(m, vxb_closest_segment_kernel, VXB_COLLIDE_THREADS, count, maxDistance, in, count, out); }); });
 }
@@ -3032,6 +3091,44 @@ int vxb_mesh_closest_to_segment_device(vxb_mesh* m, float maxDistance, const vxb
 	return meshQuery(m, { "vxb_mesh_closest_to_segment_device", !segments || !hits, "segments or hits", maxDistanceFault(maxDistance) },
 		count, deviceRule,
 		[&] { return launchLevel0(m, vxb_closest_segment_kernel, VXB_COLLIDE_THREADS, count, maxDistance, segments, count, hits); });
+}
+
+int vxb_mesh_capsule_cast_cut(vxb_mesh* m, const float camera[3], float lodFactor, const vxb_capsule_sweep* sweeps, uint32_t count,
+	vxb_capsule_cut_hit* hits)
+{
+	const char* what = "vxb_mesh_capsule_cast_cut";
+	return meshQuery(m, { what, !camera || !sweeps || !hits, "lod_camera, sweeps or hits", cutFault(camera, lodFactor), true }, count,
+		rule("sweep", [=](uint32_t i) { return sweepFault(sweeps[i]); }), [&] {
+			return hostQuery(m, sweeps, sizeof(vxb_capsule_sweep) * count, count, hits, [&](const vxb_capsule_sweep* in, vxb_capsule_cut_hit* out) {
+				return enqueueCapsuleCastCut(m, what, camera, lodFactor, sweeps, in, count, out); }); });
+}
+
+int vxb_mesh_capsule_cast_cut_device(vxb_mesh* m, const float camera[3], float lodFactor, const vxb_capsule_sweep* sweeps, uint32_t count,
+	vxb_capsule_cut_hit* hits)
+{
+	const char* what = "vxb_mesh_capsule_cast_cut_device";
+	return meshQuery(m, { what, !camera || !sweeps || !hits, "lod_camera, sweeps or hits", cutFault(camera, lodFactor), true }, count,
+		deviceRule, [&] { return enqueueCapsuleCastCut(m, what, camera, lodFactor, nullptr, sweeps, count, hits); });
+}
+
+int vxb_mesh_closest_to_segment_cut(vxb_mesh* m, const float camera[3], float lodFactor, float maxDistance, const vxb_segment* segments,
+	uint32_t count, vxb_segment_cut_hit* hits)
+{
+	const char* what = "vxb_mesh_closest_to_segment_cut";
+	return meshQuery(m, { what, !camera || !segments || !hits, "lod_camera, segments or hits",
+		firstFault(cutFault(camera, lodFactor), maxDistanceFault(maxDistance)), true }, count,
+		rule("segment", [=](uint32_t i) { return segmentFault(segments[i], maxDistance); }), [&] {
+			return hostQuery(m, segments, sizeof(vxb_segment) * count, count, hits, [&](const vxb_segment* in, vxb_segment_cut_hit* out) {
+				return enqueueClosestToSegmentCut(m, what, camera, lodFactor, maxDistance, segments, in, count, out); }); });
+}
+
+int vxb_mesh_closest_to_segment_cut_device(vxb_mesh* m, const float camera[3], float lodFactor, float maxDistance,
+	const vxb_segment* segments, uint32_t count, vxb_segment_cut_hit* hits)
+{
+	const char* what = "vxb_mesh_closest_to_segment_cut_device";
+	return meshQuery(m, { what, !camera || !segments || !hits, "lod_camera, segments or hits",
+		firstFault(cutFault(camera, lodFactor), maxDistanceFault(maxDistance)), true }, count, deviceRule,
+		[&] { return enqueueClosestToSegmentCut(m, what, camera, lodFactor, maxDistance, nullptr, segments, count, hits); });
 }
 
 // The host gather: count and scan, then the total decides the fill: the triangles are only written when they fit.

@@ -39,6 +39,23 @@
 //                of the anchor cell's 27 neighbours lies inside the node, and its covering cut node is this node.
 //   stop         unchanged: the grown box holds every contact's centre, and te is still two rounded operations from a plane.
 // Closest points against the cut need no walk; their proof is with vxb_closest_point_cut_kernel.
+//
+// Capsules against the cut (vxb_capsule_cast_cut_kernel, vxb_closest_segment_cut_kernel).  The reach R' is r for sweeps and
+// max_distance m for segments, and the shape's reach max_i |h_i| + R' travels with each query while e is the mesh's, so the
+// rule is per query (vxb_capsule_cut_reach): e + (max_i |h_i| + R') <= 15 in float; a query that fails it is a miss.
+//   sweeps       the walk above with the clip box grown by e + max_i |h_i| + r + VXB_RAY_EPS and every node's measured box by
+//                max_i |h_i| + r + VXB_RAY_EPS (both rounded up).  A contact puts the centre within |h_i| + r (+ rounding) of
+//                its drawn triangle along axis i (the capsule point paired with the contact is within r of it and within
+//                |h_i| of the centre), hence inside the node's grown box; a sweep that starts in contact has c(t_min) there.
+//                The centre at te then lies within e + max_i |h_i| + r + eps <= 15 + 1/16 < 16 (+ rounding) of the node's
+//                lattice box along every axis, and the 27-neighbour argument of the ray cast holds word for word.  The
+//                per-triangle reject in front of the capsule's tests is the level-0 kernel's (vxb_path_meets_box on the box
+//                grown by |h_i| + r + eps); it never changes a result.
+//   segments     as the closest points, with the per-axis gap: a closest pair within m puts the centre within |h_i| + m (+
+//                rounding) of its drawn triangle along axis i, so of the node's measured box, and the node is kept when its
+//                box lies within |h_i| + m + eps of the centre along every axis.  Its lattice box then lies within e +
+//                max_i |h_i| + m + eps <= 15 + 1/16 < 16 of the centre along every axis: one of the 27 neighbours of the
+//                centre's clamped block lies in it, and its covering cut node is it.
 #pragma once
 
 // The all-level map (bounds slot level_base[l] + coord_id -> directory slot, VXB_RAY_MISS where no block is, after a memset
@@ -82,6 +99,8 @@ struct VxbCutRayMesh
 	VxbCutMapArgs slots;       // level_base and nb
 	int top;                   // the top level
 	float grow;                // e + VXB_RAY_EPS, rounded up: the clip box's growth
+	float excursion;           // e itself, for the capsule queries' per-query reach (vxb_capsule_cut_reach); it fills the
+	                           // padding before `cut`, so the layout the other cut kernels read is unchanged
 	VxbLodArgs cut;            // camera and lod (lod_factor); the list pointers are unused
 };
 
@@ -373,6 +392,178 @@ __global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_closest_point_cut_ker
 				h.level = __ldg(&rec->level);
 			}
 			hits[q] = h;
+		}
+	}
+}
+
+// The cut reach of a capsule query (include/vxb200.h "capsule queries against the drawn LOD cut"), in float for the host
+// check and the kernels alike: the level-0 rule vxb_capsule_reach, then e + (max_i |h_i| + extra) <= 15; extra is the radius
+// of a sweep or the max_distance of a segment, e the mesh's excursion.
+VXB_HD bool vxb_capsule_cut_reach(const float3 h, float extra, float e)
+{
+	const float hm = fmaxf(fmaxf(fabsf(h.x), fabsf(h.y)), fabsf(h.z));
+	return vxb_capsule_reach(h, extra) && e + (hm + extra) <= VXB_SPHERE_RADIUS_MAX;
+}
+
+// One warp per capsule sweep, persistent over the batch: the cut walk with the clip box grown by e + max_i |h_i| + r +
+// VXB_RAY_EPS and every node's measured box by max_i |h_i| + r + VXB_RAY_EPS (both rounded up; "capsules" at the top), then
+// on the drawn triangles the level-0 kernel's per-triangle reject and the capsule's tests (vxb_capsule_triangle).  A sweep
+// out of cut reach is a miss.  Sweeps and hits in OUTPUT (Y-up) coordinates.  (Two CTAs per SM in the launch bounds: ptxas
+// then fits the kernel in 127 registers without a stack frame or spills, the occupancy of vxb_capsule_cast_kernel; with one
+// CTA per SM it takes 136 registers and runs slower, DESIGN.md section 6.)
+__global__ void __launch_bounds__(VXB_COLLIDE_THREADS, 2) vxb_capsule_cast_cut_kernel(const VxbCutRayMesh c,
+	const vxb_capsule_sweep* __restrict__ sweeps, unsigned count, vxb_capsule_cut_hit* __restrict__ hits)
+{
+	const unsigned lane = threadIdx.x & 31;
+	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
+	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
+	{
+		const vxb_capsule_sweep cs = sweeps[q];
+		const vxb_ray& ray = cs.path;
+		const float3 o = make_float3(ray.origin[0], ray.origin[1], ray.origin[2]);
+		const float3 d = make_float3(ray.direction[0], ray.direction[1], ray.direction[2]);
+		const float3 h = make_float3(cs.half_axis[0], cs.half_axis[1], cs.half_axis[2]);
+		const float r = cs.radius, rr = r * r;
+		const float tMin = ray.t_min, tMax = ray.t_max;
+		const float3 c0 = make_float3(o.x + tMin * d.x, o.y + tMin * d.y, o.z + tMin * d.z);
+		const float dd = (d.x * d.x + d.y * d.y) + d.z * d.z;
+		const float3 g = make_float3(fabsf(h.x) + r + VXB_RAY_EPS, fabsf(h.y) + r + VXB_RAY_EPS, fabsf(h.z) + r + VXB_RAY_EPS);
+		const float R = __fadd_ru(fmaxf(fmaxf(fabsf(h.x), fabsf(h.y)), fabsf(h.z)), r);
+		const float gn = __fadd_ru(R, VXB_RAY_EPS), clip = __fadd_ru(c.grow, R);
+		float bt = CUDART_INF_F;   // this lane's first contact
+		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
+		bool bStarted = false;
+		if (r > 0.f && vxb_capsule_cut_reach(h, r, c.excursion))   // the same for the whole warp
+			vxb_ray_walk_by<true>(c.m.nb, ray, clip, bt,
+				[&](int bx, int by, int bz, float T0, float T1, float t0, float t1, bool last, unsigned& slot) {
+					return vxb_cut_candidate(c, ray, gn, bx, by, bz, T0, T1, t0, t1, last, slot);
+				},
+				[&](const unsigned s) {
+					vxb_cut_triangles(c, s, [&](unsigned key, const float3& p0, const float3& p1, const float3& p2) {
+						if (!vxb_path_meets_box(ray, g, p0, p1, p2)) return;
+						bool started;
+						const float t = vxb_capsule_triangle(o, d, c0, h, r, rr, dd, tMin, tMax, p0, p1, p2, started);
+						if (t < CUDART_INF_F && vxb_ray_before(t, s, key, bt, bs, bk)) { bt = t; bs = s; bk = key; bStarted = started; }
+					});
+				});
+		if (lane == vxb_ray_winner(bt, bs, bk))
+		{
+			vxb_capsule_cut_hit x;
+			x.t = CUDART_INF_F; x.slot = VXB_RAY_MISS; x.block_id = 0; x.triangle = 0;
+			x.center[0] = x.center[1] = x.center[2] = 0.f;
+			x.point[0] = x.point[1] = x.point[2] = 0.f;
+			x.axis_point[0] = x.axis_point[1] = x.axis_point[2] = 0.f;
+			x.normal[0] = x.normal[1] = x.normal[2] = 0.f;
+			x.u = 0.f; x.v = 0.f; x.s = 0.f; x.flags = 0; x.level = 0; x.face = 0;
+			if (bs != VXB_RAY_MISS)
+			{
+				const vxb_block_record* rec = c.m.dir + bs;
+				const VxbVertex* verts;
+				unsigned vo;
+				const unsigned* ip;
+				x.face = vxb_cut_hit_part(c, rec, bk, verts, vo, ip);
+				const unsigned adj = vxb_cut_adj(c, rec);
+				const float3 p0 = vxb_cut_vertex(verts, vo, __ldg(ip), adj);
+				const float3 p1 = vxb_cut_vertex(verts, vo, __ldg(ip + 1), adj);
+				const float3 p2 = vxb_cut_vertex(verts, vo, __ldg(ip + 2), adj);
+				const float3 ct = make_float3(o.x + bt * d.x, o.y + bt * d.y, o.z + bt * d.z);
+				float3 pq, px;
+				vxb_pair_fields(ct, h, p0, p1, p2, pq, px, x.u, x.v, x.s);
+				x.point[0] = pq.x; x.point[1] = pq.y; x.point[2] = pq.z;
+				x.axis_point[0] = px.x; x.axis_point[1] = px.y; x.axis_point[2] = px.z;
+				x.t = bt; x.slot = bs; x.block_id = __ldg(&rec->id); x.triangle = bk & 0xFFFFFFu;
+				x.center[0] = ct.x; x.center[1] = ct.y; x.center[2] = ct.z;
+				vxb_blend_normal(verts, vo, ip, x.u, x.v, x.normal);
+				x.flags = bStarted ? VXB_SPHERE_STARTED_IN_CONTACT : 0u;
+				x.level = __ldg(&rec->level);
+			}
+			hits[q] = x;
+		}
+	}
+}
+
+// One warp per segment, persistent over the batch.  Lane k < 27 takes neighbour k of the centre's block clamped into the
+// grid (vxb_point_candidate's arithmetic), finds that block's covering cut node and keeps it when the node's measured box
+// lies within |h_i| + max_distance + VXB_RAY_EPS of the centre along every axis (the proof under "capsules" at the top).
+// Lanes that reach the same node hand it on once (the lowest lane); the warp then runs the level-0 kernel's per-axis reject
+// and the closest pair (vxb_segment_triangle) on each node's drawn triangles, strided over the lanes.  A segment out of cut
+// reach is a miss.  OUTPUT (Y-up) coordinates.  (A minimum of one CTA per SM in the launch bounds, as
+// vxb_closest_segment_kernel.)
+__global__ void __launch_bounds__(VXB_COLLIDE_THREADS, 1) vxb_closest_segment_cut_kernel(const VxbCutRayMesh c, const float maxDistance,
+	const vxb_segment* __restrict__ segments, unsigned count, vxb_segment_cut_hit* __restrict__ hits)
+{
+	const unsigned lane = threadIdx.x & 31;
+	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
+	const float md2 = maxDistance * maxDistance;
+	const int nb = c.m.nb;
+	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
+	{
+		const vxb_segment sg = segments[q];
+		const float3 p = make_float3(sg.center[0], sg.center[1], sg.center[2]);
+		const float3 h = make_float3(sg.half_axis[0], sg.half_axis[1], sg.half_axis[2]);
+		const float3 g = make_float3(fabsf(h.x) + maxDistance + VXB_RAY_EPS, fabsf(h.y) + maxDistance + VXB_RAY_EPS,
+			fabsf(h.z) + maxDistance + VXB_RAY_EPS);
+		float bd = CUDART_INF_F;   // this lane's nearest triangle
+		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
+		unsigned slot = VXB_RAY_MISS;
+		if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && vxb_capsule_cut_reach(h, maxDistance, c.excursion) && lane < 27)
+		{
+			const float top = (float)(nb - 1);
+			const int bx = (int)fminf(fmaxf(floorf(p.x * 0.0625f), 0.f), top) + (int)(lane % 3) - 1;
+			const int by = (int)fminf(fmaxf(floorf(p.y * 0.0625f), 0.f), top) + (int)((lane / 3) % 3) - 1;
+			const int bz = (int)fminf(fmaxf(floorf(p.z * 0.0625f), 0.f), top) + (int)(lane / 9) - 1;
+			if (bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb)
+			{
+				unsigned key;
+				const unsigned s = vxb_cut_node(c, bx, bz, by, key);   // grid (x, y, z) = output (x, z, y)
+				if (s != VXB_RAY_MISS)
+				{
+					const float4 lo = __ldg(&c.boxes[2 * (size_t)key]), hi = __ldg(&c.boxes[2 * (size_t)key + 1]);
+					if (!(lo.x - p.x > g.x || p.x - hi.x > g.x) && !(lo.y - p.y > g.y || p.y - hi.y > g.y) &&
+						!(lo.z - p.z > g.z || p.z - hi.z > g.z)) slot = s;
+				}
+			}
+		}
+		const unsigned peers = __match_any_sync(0xFFFFFFFFu, slot);   // every lane takes part
+		vxb_warp_each(slot != VXB_RAY_MISS && (peers & ((1u << lane) - 1u)) == 0, slot, [&](const unsigned s) {
+			vxb_cut_triangles(c, s, [&](unsigned key, const float3& p0, const float3& p1, const float3& p2) {
+				if (fminf(fminf(p0.x, p1.x), p2.x) - p.x > g.x || p.x - fmaxf(fmaxf(p0.x, p1.x), p2.x) > g.x ||
+					fminf(fminf(p0.y, p1.y), p2.y) - p.y > g.y || p.y - fmaxf(fmaxf(p0.y, p1.y), p2.y) > g.y ||
+					fminf(fminf(p0.z, p1.z), p2.z) - p.z > g.z || p.z - fmaxf(fmaxf(p0.z, p1.z), p2.z) > g.z) return;
+				float3 x;
+				float u, v, w;
+				const float d2 = vxb_segment_triangle(p, h, p0, p1, p2, x, u, v, w);
+				if (d2 <= md2 && vxb_ray_before(d2, s, key, bd, bs, bk)) { bd = d2; bs = s; bk = key; }
+			});
+		});
+		if (lane == vxb_ray_winner(bd, bs, bk))
+		{
+			vxb_segment_cut_hit x;
+			x.distance = CUDART_INF_F; x.slot = VXB_RAY_MISS; x.block_id = 0; x.triangle = 0;
+			x.point[0] = x.point[1] = x.point[2] = 0.f;
+			x.axis_point[0] = x.axis_point[1] = x.axis_point[2] = 0.f;
+			x.normal[0] = x.normal[1] = x.normal[2] = 0.f;
+			x.u = 0.f; x.v = 0.f; x.s = 0.f; x.level = 0; x.face = 0;
+			if (bs != VXB_RAY_MISS)
+			{
+				const vxb_block_record* rec = c.m.dir + bs;
+				const VxbVertex* verts;
+				unsigned vo;
+				const unsigned* ip;
+				x.face = vxb_cut_hit_part(c, rec, bk, verts, vo, ip);
+				const unsigned adj = vxb_cut_adj(c, rec);
+				const float3 p0 = vxb_cut_vertex(verts, vo, __ldg(ip), adj);
+				const float3 p1 = vxb_cut_vertex(verts, vo, __ldg(ip + 1), adj);
+				const float3 p2 = vxb_cut_vertex(verts, vo, __ldg(ip + 2), adj);
+				float3 pq, px;
+				vxb_pair_fields(p, h, p0, p1, p2, pq, px, x.u, x.v, x.s);
+				x.point[0] = pq.x; x.point[1] = pq.y; x.point[2] = pq.z;
+				x.axis_point[0] = px.x; x.axis_point[1] = px.y; x.axis_point[2] = px.z;
+				x.distance = VXB_SQRT(bd); x.slot = bs; x.block_id = __ldg(&rec->id); x.triangle = bk & 0xFFFFFFu;
+				vxb_blend_normal(verts, vo, ip, x.u, x.v, x.normal);
+				x.level = __ldg(&rec->level);
+			}
+			hits[q] = x;
 		}
 	}
 }
