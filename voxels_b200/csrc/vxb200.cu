@@ -35,6 +35,7 @@
 #include "vxb_ray.cuh"
 #include "vxb_collide.cuh"
 #include "vxb_cutray.cuh"
+#include "vxb_query.cuh"
 #include "vxb_overlap.cuh"
 
 static_assert(sizeof(VxbVertex) == 48, "PolygonVertex layout");

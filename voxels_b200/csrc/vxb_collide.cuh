@@ -134,61 +134,10 @@ VXB_FN float vxb_sweep_triangle(const float3 o, const float3 d, const float3 c0,
 	return t;
 }
 
-// One warp per sweep, persistent over the batch: the block walk of the ray casts with boxes grown by r + eps.  Sweeps and hits
-// in OUTPUT (Y-up) coordinates.
-__global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_sphere_cast_kernel(const VxbRayMesh m, const float r, const vxb_ray* __restrict__ rays,
-	unsigned count, vxb_sphere_hit* __restrict__ hits)
-{
-	const unsigned lane = threadIdx.x & 31;
-	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
-	const float rr = r * r;
-	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
-	{
-		const vxb_ray ray = rays[q];
-		const float3 o = make_float3(ray.origin[0], ray.origin[1], ray.origin[2]);
-		const float3 d = make_float3(ray.direction[0], ray.direction[1], ray.direction[2]);
-		const float tMin = ray.t_min, tMax = ray.t_max;
-		const float3 c0 = make_float3(o.x + tMin * d.x, o.y + tMin * d.y, o.z + tMin * d.z);
-		const float dd = (d.x * d.x + d.y * d.y) + d.z * d.z;
-		float bt = CUDART_INF_F;   // this lane's first contact
-		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		bool bStarted = false;
-		vxb_ray_walk(m, ray, r + VXB_RAY_EPS, bt, [&](const unsigned s) {
-			vxb_slot_triangles(m, s, [&](unsigned k, const float3& a, const float3& b, const float3& c) {
-				bool started;
-				const float t = vxb_sweep_triangle(o, d, c0, r, rr, dd, tMin, tMax, a, b, c, started);
-				if (t < CUDART_INF_F && vxb_ray_before(t, s, k, bt, bs, bk)) { bt = t; bs = s; bk = k; bStarted = started; }
-			});
-		});
-		if (lane == vxb_ray_winner(bt, bs, bk))
-		{
-			vxb_sphere_hit h;
-			h.t = CUDART_INF_F; h.slot = VXB_RAY_MISS; h.block_id = 0; h.triangle = 0;
-			h.center[0] = h.center[1] = h.center[2] = 0.f;
-			h.point[0] = h.point[1] = h.point[2] = 0.f;
-			h.normal[0] = h.normal[1] = h.normal[2] = 0.f;
-			h.u = 0.f; h.v = 0.f; h.flags = 0;
-			if (bs != VXB_RAY_MISS)
-			{
-				const vxb_block_record* rec = m.dir + bs;
-				float3 a, b, c, p;
-				vxb_ray_triangle(m, __ldg(&rec->vertex_offset), __ldg(&rec->index_offset), bk, a, b, c);
-				const float3 ct = make_float3(o.x + bt * d.x, o.y + bt * d.y, o.z + bt * d.z);
-				vxb_closest_on_triangle(ct, a, b, c, p, h.u, h.v);
-				h.t = bt; h.slot = bs; h.block_id = __ldg(&rec->id); h.triangle = bk;
-				h.center[0] = ct.x; h.center[1] = ct.y; h.center[2] = ct.z;
-				h.point[0] = p.x; h.point[1] = p.y; h.point[2] = p.z;
-				vxb_ray_blend_normal(m, bs, bk, h.u, h.v, h.normal);
-				h.flags = bStarted ? VXB_SPHERE_STARTED_IN_CONTACT : 0u;
-			}
-			hits[q] = h;
-		}
-	}
-}
-
 // The point neighbourhood of the closest-point and closest-to-segment queries: this lane's candidate slot, neighbour k = lane
-// (< 27) of the block of p clamped into the grid, when `ok` (the same for the whole warp) holds, the block lies in the grid,
-// `near(bx, by, bz)` accepts it and the map has a block there.
+// (< 27) of the block of p clamped into the grid, when `ok` (the same for the whole warp) holds, the block lies in the grid
+// and `at(bx, by, bz, slot)` yields a slot there (the surface's step: its box accepted by the shape's `near`, then its slot;
+// VxbLevel0Surface::point, VxbCutSurface::point).
 //   closest points  a triangle within max_distance of the query lies in a block whose box is within max_distance of the
 //                   query (a level-0 triangle lies in the closed box of its block), and `near` rejects a block only when its
 //                   box is farther than max_distance + VXB_RAY_EPS (the float box distance is within a few ulps of the true
@@ -200,11 +149,10 @@ __global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_sphere_cast_kernel(co
 //                   grid box alike.
 //   segments        the same with the per-axis gap: `near` rejects a block only when its box is farther than |h_i| +
 //                   max_distance + eps from the centre along some axis, and the reach rule keeps that below 16.
-template <class Near>
-VXB_FN bool vxb_point_candidate(const VxbRayMesh& m, const float3 p, bool ok, Near&& near, unsigned& slot)
+template <class At>
+VXB_FN bool vxb_point_candidate(const int nb, const float3 p, bool ok, At&& at, unsigned& slot)
 {
 	const unsigned lane = threadIdx.x & 31;
-	const int nb = m.nb;
 	bool cand = false;
 	slot = VXB_RAY_MISS;
 	if (ok && lane < 27)
@@ -213,63 +161,9 @@ VXB_FN bool vxb_point_candidate(const VxbRayMesh& m, const float3 p, bool ok, Ne
 		const int bx = (int)fminf(fmaxf(floorf(p.x * 0.0625f), 0.f), top) + (int)(lane % 3) - 1;
 		const int by = (int)fminf(fmaxf(floorf(p.y * 0.0625f), 0.f), top) + (int)((lane / 3) % 3) - 1;
 		const int bz = (int)fminf(fmaxf(floorf(p.z * 0.0625f), 0.f), top) + (int)(lane / 9) - 1;
-		if (bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb && near(bx, by, bz))
-		{
-			slot = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
-			cand = slot != VXB_RAY_MISS;
-		}
+		if (bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb) cand = at(bx, by, bz, slot);
 	}
 	return cand;
-}
-
-// One warp per query point, persistent over the batch: lane k < 27 takes neighbour k of the query's block (clamped into the
-// grid), the warp then tests the candidate blocks' triangles strided over the lanes.  Points and hits in OUTPUT (Y-up)
-// coordinates.
-__global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_closest_point_kernel(const VxbRayMesh m, const float maxDistance,
-	const float* __restrict__ points, unsigned count, vxb_closest_hit* __restrict__ hits)
-{
-	const unsigned lane = threadIdx.x & 31;
-	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
-	const float md2 = maxDistance * maxDistance, reach = maxDistance + VXB_RAY_EPS;
-	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
-	{
-		const float3 p = make_float3(points[3 * q], points[3 * q + 1], points[3 * q + 2]);
-		float bd = CUDART_INF_F, bu = 0.f, bv = 0.f;   // this lane's nearest triangle
-		float3 bp = make_float3(0.f, 0.f, 0.f);
-		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		unsigned slot;
-		const bool cand = vxb_point_candidate(m, p, isfinite(p.x) && isfinite(p.y) && isfinite(p.z), [&](int bx, int by, int bz) {
-			const float gx = fmaxf(fmaxf((float)(16 * bx) - p.x, p.x - (float)(16 * bx + 16)), 0.f);
-			const float gy = fmaxf(fmaxf((float)(16 * by) - p.y, p.y - (float)(16 * by + 16)), 0.f);
-			const float gz = fmaxf(fmaxf((float)(16 * bz) - p.z, p.z - (float)(16 * bz + 16)), 0.f);
-			return VXB_SQRT((gx * gx + gy * gy) + gz * gz) <= reach;
-		}, slot);
-		vxb_warp_each(cand, slot, [&](const unsigned s) {
-			vxb_slot_triangles(m, s, [&](unsigned k, const float3& a, const float3& b, const float3& c) {
-				float3 x;
-				float u, v;
-				vxb_closest_on_triangle(p, a, b, c, x, u, v);
-				const float d2 = vxb_dist2(p, x);
-				if (d2 <= md2 && vxb_ray_before(d2, s, k, bd, bs, bk)) { bd = d2; bs = s; bk = k; bu = u; bv = v; bp = x; }
-			});
-		});
-		if (lane == vxb_ray_winner(bd, bs, bk))
-		{
-			vxb_closest_hit h;
-			h.distance = CUDART_INF_F; h.slot = VXB_RAY_MISS; h.block_id = 0; h.triangle = 0;
-			h.point[0] = h.point[1] = h.point[2] = 0.f;
-			h.normal[0] = h.normal[1] = h.normal[2] = 0.f;
-			h.u = 0.f; h.v = 0.f;
-			if (bs != VXB_RAY_MISS)
-			{
-				h.distance = VXB_SQRT(bd); h.slot = bs; h.block_id = __ldg(&m.dir[bs].id); h.triangle = bk;
-				h.point[0] = bp.x; h.point[1] = bp.y; h.point[2] = bp.z;
-				h.u = bu; h.v = bv;
-				vxb_ray_blend_normal(m, bs, bk, bu, bv, h.normal);
-			}
-			hits[q] = h;
-		}
-	}
 }
 
 // ---- capsules (include/vxb200.h "capsule queries") ---------------------------------------------------------------------
@@ -437,124 +331,56 @@ VXB_FN void vxb_pair_fields(const float3 ctr, const float3 h, const float3 a, co
 	x = make_float3(ctr.x + s * h.x, ctr.y + s * h.y, ctr.z + s * h.z);
 }
 
-// One warp per capsule sweep, persistent over the batch: the block walk of the ray casts with boxes grown by max_i |h_i| + r +
-// eps (the proof at the top of vxb_ray.cuh), and the per-triangle reject above.  Sweeps and hits in OUTPUT (Y-up) coordinates.
-__global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_capsule_cast_kernel(const VxbRayMesh m, const vxb_capsule_sweep* __restrict__ sweeps,
-	unsigned count, vxb_capsule_hit* __restrict__ hits)
+// ---- the level-0 surface -----------------------------------------------------------------------------------------------
+//
+// The level-0 triangles as the query bodies (vxb_query.cuh) see them; VxbCutSurface (vxb_cutray.cuh) is the drawn cut's.
+// A surface supplies the candidate blocks (the walk of a swept shape, the 27-neighbour step of a point shape), a block's
+// triangles, the winning triangle, the capsule reach rule and the tail of the hit.  Keys are triangle indices.
+struct VxbLevel0Surface
 {
-	const unsigned lane = threadIdx.x & 31;
-	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
-	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
-	{
-		const vxb_capsule_sweep cs = sweeps[q];
-		const vxb_ray& ray = cs.path;
-		const float3 o = make_float3(ray.origin[0], ray.origin[1], ray.origin[2]);
-		const float3 d = make_float3(ray.direction[0], ray.direction[1], ray.direction[2]);
-		const float3 h = make_float3(cs.half_axis[0], cs.half_axis[1], cs.half_axis[2]);
-		const float r = cs.radius, rr = r * r;
-		const float tMin = ray.t_min, tMax = ray.t_max;
-		const float3 c0 = make_float3(o.x + tMin * d.x, o.y + tMin * d.y, o.z + tMin * d.z);
-		const float dd = (d.x * d.x + d.y * d.y) + d.z * d.z;
-		const float3 g = make_float3(fabsf(h.x) + r + VXB_RAY_EPS, fabsf(h.y) + r + VXB_RAY_EPS, fabsf(h.z) + r + VXB_RAY_EPS);
-		float bt = CUDART_INF_F;   // this lane's first contact
-		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		bool bStarted = false;
-		if (r > 0.f && vxb_capsule_reach(h, r))   // the same for the whole warp
-			vxb_ray_walk(m, ray, fmaxf(fmaxf(g.x, g.y), g.z), bt, [&](const unsigned s) {
-				vxb_slot_triangles(m, s, [&](unsigned k, const float3& a, const float3& b, const float3& c) {
-					if (!vxb_path_meets_box(ray, g, a, b, c)) return;
-					bool started;
-					const float t = vxb_capsule_triangle(o, d, c0, h, r, rr, dd, tMin, tMax, a, b, c, started);
-					if (t < CUDART_INF_F && vxb_ray_before(t, s, k, bt, bs, bk)) { bt = t; bs = s; bk = k; bStarted = started; }
-				});
-			});
-		if (lane == vxb_ray_winner(bt, bs, bk))
-		{
-			vxb_capsule_hit x;
-			x.t = CUDART_INF_F; x.slot = VXB_RAY_MISS; x.block_id = 0; x.triangle = 0;
-			x.center[0] = x.center[1] = x.center[2] = 0.f;
-			x.point[0] = x.point[1] = x.point[2] = 0.f;
-			x.axis_point[0] = x.axis_point[1] = x.axis_point[2] = 0.f;
-			x.normal[0] = x.normal[1] = x.normal[2] = 0.f;
-			x.u = 0.f; x.v = 0.f; x.s = 0.f; x.flags = 0;
-			if (bs != VXB_RAY_MISS)
-			{
-				const vxb_block_record* rec = m.dir + bs;
-				float3 a, b, c;
-				vxb_ray_triangle(m, __ldg(&rec->vertex_offset), __ldg(&rec->index_offset), bk, a, b, c);
-				const float3 ct = make_float3(o.x + bt * d.x, o.y + bt * d.y, o.z + bt * d.z);
-				float3 pq, px;
-				vxb_pair_fields(ct, h, a, b, c, pq, px, x.u, x.v, x.s);
-				x.point[0] = pq.x; x.point[1] = pq.y; x.point[2] = pq.z;
-				x.axis_point[0] = px.x; x.axis_point[1] = px.y; x.axis_point[2] = px.z;
-				x.t = bt; x.slot = bs; x.block_id = __ldg(&rec->id); x.triangle = bk;
-				x.center[0] = ct.x; x.center[1] = ct.y; x.center[2] = ct.z;
-				vxb_ray_blend_normal(m, bs, bk, x.u, x.v, x.normal);
-				x.flags = bStarted ? VXB_SPHERE_STARTED_IN_CONTACT : 0u;
-			}
-			hits[q] = x;
-		}
-	}
-}
+	const VxbRayMesh& m;
 
-// One warp per segment, persistent over the batch: lane k < 27 takes neighbour k of the centre's block (clamped into the
-// grid) and skips it when its box is farther than |h_i| + max_distance + eps along some axis; the warp then tests the
-// candidate blocks' triangles strided over the lanes, with the same per-axis reject per triangle.  OUTPUT (Y-up) coordinates.
-// (A minimum of one CTA per SM in the launch bounds: without it ptxas holds this kernel to 64 registers and spills.)
-__global__ void __launch_bounds__(VXB_COLLIDE_THREADS, 1) vxb_closest_segment_kernel(const VxbRayMesh m, const float maxDistance,
-	const vxb_segment* __restrict__ segments, unsigned count, vxb_segment_hit* __restrict__ hits)
-{
-	const unsigned lane = threadIdx.x & 31;
-	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
-	const float md2 = maxDistance * maxDistance;
-	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
+	// The walk of a shape whose reach splits as hm = max_i |h_i| and r (both 0 for rays, hm = -0 for spheres): the level-0
+	// boxes grown by (hm + r) + VXB_RAY_EPS, which is max_i (|h_i| + r + eps) in float (rounding is monotone).
+	template <class Block>
+	VXB_FN void walk(const vxb_ray& ray, float hm, float r, const float& best, Block&& block) const
 	{
-		const vxb_segment sg = segments[q];
-		const float3 p = make_float3(sg.center[0], sg.center[1], sg.center[2]);
-		const float3 h = make_float3(sg.half_axis[0], sg.half_axis[1], sg.half_axis[2]);
-		const float3 g = make_float3(fabsf(h.x) + maxDistance + VXB_RAY_EPS, fabsf(h.y) + maxDistance + VXB_RAY_EPS,
-			fabsf(h.z) + maxDistance + VXB_RAY_EPS);
-		float bd = CUDART_INF_F;   // this lane's nearest triangle
-		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		unsigned slot;
-		const bool ok = isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && vxb_capsule_reach(h, maxDistance);
-		const bool cand = vxb_point_candidate(m, p, ok, [&](int bx, int by, int bz) {
-			return !((float)(16 * bx) - p.x > g.x || p.x - (float)(16 * bx + 16) > g.x) &&
-				!((float)(16 * by) - p.y > g.y || p.y - (float)(16 * by + 16) > g.y) &&
-				!((float)(16 * bz) - p.z > g.z || p.z - (float)(16 * bz + 16) > g.z);
-		}, slot);
-		vxb_warp_each(cand, slot, [&](const unsigned s) {
-			vxb_slot_triangles(m, s, [&](unsigned k, const float3& a, const float3& b, const float3& c) {
-				if (fminf(fminf(a.x, b.x), c.x) - p.x > g.x || p.x - fmaxf(fmaxf(a.x, b.x), c.x) > g.x ||
-					fminf(fminf(a.y, b.y), c.y) - p.y > g.y || p.y - fmaxf(fmaxf(a.y, b.y), c.y) > g.y ||
-					fminf(fminf(a.z, b.z), c.z) - p.z > g.z || p.z - fmaxf(fmaxf(a.z, b.z), c.z) > g.z) return;
-				float3 x;
-				float u, v, w;
-				const float d2 = vxb_segment_triangle(p, h, a, b, c, x, u, v, w);
-				if (d2 <= md2 && vxb_ray_before(d2, s, k, bd, bs, bk)) { bd = d2; bs = s; bk = k; }
-			});
-		});
-		if (lane == vxb_ray_winner(bd, bs, bk))
-		{
-			vxb_segment_hit x;
-			x.distance = CUDART_INF_F; x.slot = VXB_RAY_MISS; x.block_id = 0; x.triangle = 0;
-			x.point[0] = x.point[1] = x.point[2] = 0.f;
-			x.axis_point[0] = x.axis_point[1] = x.axis_point[2] = 0.f;
-			x.normal[0] = x.normal[1] = x.normal[2] = 0.f;
-			x.u = 0.f; x.v = 0.f; x.s = 0.f;
-			if (bs != VXB_RAY_MISS)
-			{
-				const vxb_block_record* rec = m.dir + bs;
-				float3 a, b, c;
-				vxb_ray_triangle(m, __ldg(&rec->vertex_offset), __ldg(&rec->index_offset), bk, a, b, c);
-				float3 pq, px;
-				vxb_pair_fields(p, h, a, b, c, pq, px, x.u, x.v, x.s);
-				x.point[0] = pq.x; x.point[1] = pq.y; x.point[2] = pq.z;
-				x.axis_point[0] = px.x; x.axis_point[1] = px.y; x.axis_point[2] = px.z;
-				x.distance = VXB_SQRT(bd); x.slot = bs; x.block_id = __ldg(&rec->id); x.triangle = bk;
-				vxb_ray_blend_normal(m, bs, bk, x.u, x.v, x.normal);
-			}
-			hits[q] = x;
-		}
+		vxb_ray_walk(m, ray, (hm + r) + VXB_RAY_EPS, best, block);
 	}
-}
+
+	// the point candidate: the block's lattice box [16 b, 16 b + 16] accepted by `near(lo, hi)`, then its map slot
+	template <class Near>
+	VXB_FN bool point(const float3 p, bool ok, Near&& near, unsigned& slot) const
+	{
+		const int nb = m.nb;
+		return vxb_point_candidate(nb, p, ok, [&](int bx, int by, int bz, unsigned& s) {
+			const float3 lo = make_float3((float)(16 * bx), (float)(16 * by), (float)(16 * bz));
+			const float3 hi = make_float3((float)(16 * bx + 16), (float)(16 * by + 16), (float)(16 * bz + 16));
+			if (!near(lo, hi)) return false;
+			s = __ldg(&m.map[((unsigned)by * nb + (unsigned)bz) * nb + (unsigned)bx]);   // output y = grid z
+			return s != VXB_RAY_MISS;
+		}, slot);
+	}
+
+	template <class F>
+	VXB_FN void triangles(unsigned s, F&& f) const { vxb_slot_triangles(m, s, f); }
+
+	VXB_FN const vxb_block_record* record(unsigned s) const { return m.dir + s; }
+
+	// the positions of the winning triangle k of the block at directory record rec, and its blended normal at (u, v)
+	VXB_FN void corners(const vxb_block_record* rec, unsigned k, float3& p0, float3& p1, float3& p2) const
+	{
+		vxb_ray_triangle(m, __ldg(&rec->vertex_offset), __ldg(&rec->index_offset), k, p0, p1, p2);
+	}
+	VXB_FN void normal(const vxb_block_record* rec, unsigned k, float u, float v, float* out) const
+	{
+		vxb_blend_normal(m.verts, __ldg(&rec->vertex_offset), m.idx + __ldg(&rec->index_offset) + 3 * k, u, v, out);
+	}
+
+	VXB_FN unsigned triangle(unsigned k) const { return k; }
+
+	VXB_FN bool reach(const float3 h, float extra) const { return vxb_capsule_reach(h, extra); }
+
+	template <class Hit>
+	VXB_FN void tail(Hit&, unsigned, unsigned) const {}
+};

@@ -38,7 +38,7 @@
 //                (+ rounding) of the node's lattice box along every axis.  The argument above then holds word for word: one
 //                of the anchor cell's 27 neighbours lies inside the node, and its covering cut node is this node.
 //   stop         unchanged: the grown box holds every contact's centre, and te is still two rounded operations from a plane.
-// Closest points against the cut need no walk; their proof is with vxb_closest_point_cut_kernel.
+// Closest points against the cut need no walk; their proof is with VxbCutSurface::point.
 //
 // Capsules against the cut (vxb_capsule_cast_cut_kernel, vxb_closest_segment_cut_kernel).  The reach R' is r for sweeps and
 // max_distance m for segments, and the shape's reach max_i |h_i| + R' travels with each query while e is the mesh's, so the
@@ -181,219 +181,14 @@ VXB_FN void vxb_cut_triangles(const VxbCutRayMesh& c, const unsigned s, F&& f)
 				__ldg(&rec->trans_index_count[x]) / 3);
 }
 
-// One warp per ray, persistent over the batch.  Rays and hits in OUTPUT (Y-up) coordinates.
-__global__ void __launch_bounds__(VXB_RAY_THREADS) vxb_raycast_cut_kernel(const VxbCutRayMesh c, const vxb_ray* __restrict__ rays, unsigned count,
-	vxb_cut_hit* __restrict__ hits)
-{
-	const unsigned lane = threadIdx.x & 31;
-	const unsigned warps = gridDim.x * (VXB_RAY_THREADS / 32);
-	const VxbRayMesh& m = c.m;
-	for (unsigned r = blockIdx.x * (VXB_RAY_THREADS / 32) + (threadIdx.x >> 5); r < count; r += warps)
-	{
-		const vxb_ray ray = rays[r];
-		const float px = ray.origin[0], py = ray.origin[1], pz = ray.origin[2];
-		const float dx = ray.direction[0], dy = ray.direction[1], dz = ray.direction[2];
-		const float tMin = ray.t_min, tMax = ray.t_max;
-		float bt = CUDART_INF_F, bu = 0.f, bv = 0.f;   // this lane's best hit
-		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		vxb_ray_walk_by<true>(m.nb, ray, c.grow, bt,
-			[&](int bx, int by, int bz, float T0, float T1, float t0, float t1, bool last, unsigned& slot) {
-				return vxb_cut_candidate(c, ray, VXB_RAY_EPS, bx, by, bz, T0, T1, t0, t1, last, slot);
-			},
-			[&](const unsigned s) {
-				vxb_cut_triangles(c, s, [&](unsigned key, const float3& p0, const float3& p1, const float3& p2) {
-					float t, u, v;
-					if (vxb_ray_mt(px, py, pz, dx, dy, dz, tMin, tMax, p0, p1, p2, t, u, v) && vxb_ray_before(t, s, key, bt, bs, bk))
-					{
-						bt = t; bs = s; bk = key; bu = u; bv = v;
-					}
-				});
-			});
-		// ---- the winner by the tie rule; its lane writes the hit ----
-		if (lane == vxb_ray_winner(bt, bs, bk))
-		{
-			vxb_cut_hit h;
-			h.u = 0.f; h.v = 0.f; h.slot = VXB_RAY_MISS; h.block_id = 0; h.triangle = 0;
-			h.t = CUDART_INF_F;
-			h.position[0] = h.position[1] = h.position[2] = 0.f;
-			h.normal[0] = h.normal[1] = h.normal[2] = 0.f;
-			h.level = 0; h.face = 0;
-			if (bs != VXB_RAY_MISS)
-			{
-				const vxb_block_record* rec = m.dir + bs;
-				const unsigned p = bk >> 24, k = bk & 0xFFFFFFu;
-				h.t = bt; h.u = bu; h.v = bv; h.slot = bs; h.block_id = __ldg(&rec->id); h.triangle = k;
-				h.position[0] = px + bt * dx; h.position[1] = py + bt * dy; h.position[2] = pz + bt * dz;
-				h.level = __ldg(&rec->level); h.face = p ? p - 1 : 0xFFFFFFFFu;
-				if (p) vxb_blend_normal(c.tverts, __ldg(&rec->trans_vertex_offset[p - 1]), c.tidx + __ldg(&rec->trans_index_offset[p - 1]) + 3 * k, bu, bv, h.normal);
-				else vxb_blend_normal(m.verts, __ldg(&rec->vertex_offset), m.idx + __ldg(&rec->index_offset) + 3 * k, bu, bv, h.normal);
-			}
-			hits[r] = h;
-		}
-	}
-}
-
-// The winning triangle of a sweep or point hit: triangle key (part << 24 | k) of cut node rec, its part's vertices `verts`
-// from vertex offset vo and its indices at ip (for vxb_blend_normal and vxb_cut_vertex).  Returns the hit's face field.
-VXB_FN unsigned vxb_cut_hit_part(const VxbCutRayMesh& c, const vxb_block_record* rec, unsigned key, const VxbVertex*& verts,
-	unsigned& vo, const unsigned*& ip)
+// The winning triangle of a hit: triangle key (part << 24 | k) of cut node rec, its part's vertices `verts` from vertex offset vo
+// and its indices at ip (for vxb_blend_normal and vxb_cut_vertex).
+VXB_FN void vxb_cut_hit_part(const VxbCutRayMesh& c, const vxb_block_record* rec, unsigned key, const VxbVertex*& verts, unsigned& vo,
+	const unsigned*& ip)
 {
 	const unsigned p = key >> 24, k = key & 0xFFFFFFu;
-	if (p)
-	{
-		verts = c.tverts; vo = __ldg(&rec->trans_vertex_offset[p - 1]); ip = c.tidx + __ldg(&rec->trans_index_offset[p - 1]) + 3 * k;
-		return p - 1;
-	}
-	verts = c.m.verts; vo = __ldg(&rec->vertex_offset); ip = c.m.idx + __ldg(&rec->index_offset) + 3 * k;
-	return 0xFFFFFFFFu;
-}
-
-// One warp per sweep, persistent over the batch: the cut walk with the clip box grown by e + r + VXB_RAY_EPS and every node's
-// measured box by r + VXB_RAY_EPS (both rounded up; "sphere sweeps" at the top), the sphere sweep's tests (vxb_sweep_triangle)
-// on the drawn triangles.  Sweeps and hits in OUTPUT (Y-up) coordinates.  (A minimum of one CTA per SM in the launch bounds:
-// without it ptxas holds this kernel to 64 registers and spills.)
-__global__ void __launch_bounds__(VXB_COLLIDE_THREADS, 1) vxb_sphere_cast_cut_kernel(const VxbCutRayMesh c, const float r,
-	const vxb_ray* __restrict__ rays, unsigned count, vxb_sphere_cut_hit* __restrict__ hits)
-{
-	const unsigned lane = threadIdx.x & 31;
-	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
-	const float rr = r * r;
-	const float g = __fadd_ru(r, VXB_RAY_EPS), clip = __fadd_ru(c.grow, r);
-	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
-	{
-		const vxb_ray ray = rays[q];
-		const float3 o = make_float3(ray.origin[0], ray.origin[1], ray.origin[2]);
-		const float3 d = make_float3(ray.direction[0], ray.direction[1], ray.direction[2]);
-		const float tMin = ray.t_min, tMax = ray.t_max;
-		const float3 c0 = make_float3(o.x + tMin * d.x, o.y + tMin * d.y, o.z + tMin * d.z);
-		const float dd = (d.x * d.x + d.y * d.y) + d.z * d.z;
-		float bt = CUDART_INF_F;   // this lane's first contact
-		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		bool bStarted = false;
-		vxb_ray_walk_by<true>(c.m.nb, ray, clip, bt,
-			[&](int bx, int by, int bz, float T0, float T1, float t0, float t1, bool last, unsigned& slot) {
-				return vxb_cut_candidate(c, ray, g, bx, by, bz, T0, T1, t0, t1, last, slot);
-			},
-			[&](const unsigned s) {
-				vxb_cut_triangles(c, s, [&](unsigned key, const float3& p0, const float3& p1, const float3& p2) {
-					bool started;
-					const float t = vxb_sweep_triangle(o, d, c0, r, rr, dd, tMin, tMax, p0, p1, p2, started);
-					if (t < CUDART_INF_F && vxb_ray_before(t, s, key, bt, bs, bk)) { bt = t; bs = s; bk = key; bStarted = started; }
-				});
-			});
-		if (lane == vxb_ray_winner(bt, bs, bk))
-		{
-			vxb_sphere_cut_hit h;
-			h.t = CUDART_INF_F; h.slot = VXB_RAY_MISS; h.block_id = 0; h.triangle = 0;
-			h.center[0] = h.center[1] = h.center[2] = 0.f;
-			h.point[0] = h.point[1] = h.point[2] = 0.f;
-			h.normal[0] = h.normal[1] = h.normal[2] = 0.f;
-			h.u = 0.f; h.v = 0.f; h.flags = 0; h.level = 0; h.face = 0;
-			if (bs != VXB_RAY_MISS)
-			{
-				const vxb_block_record* rec = c.m.dir + bs;
-				const VxbVertex* verts;
-				unsigned vo;
-				const unsigned* ip;
-				h.face = vxb_cut_hit_part(c, rec, bk, verts, vo, ip);
-				const unsigned adj = vxb_cut_adj(c, rec);
-				const float3 p0 = vxb_cut_vertex(verts, vo, __ldg(ip), adj);
-				const float3 p1 = vxb_cut_vertex(verts, vo, __ldg(ip + 1), adj);
-				const float3 p2 = vxb_cut_vertex(verts, vo, __ldg(ip + 2), adj);
-				const float3 ct = make_float3(o.x + bt * d.x, o.y + bt * d.y, o.z + bt * d.z);
-				float3 x;
-				vxb_closest_on_triangle(ct, p0, p1, p2, x, h.u, h.v);
-				h.t = bt; h.slot = bs; h.block_id = __ldg(&rec->id); h.triangle = bk & 0xFFFFFFu;
-				h.center[0] = ct.x; h.center[1] = ct.y; h.center[2] = ct.z;
-				h.point[0] = x.x; h.point[1] = x.y; h.point[2] = x.z;
-				vxb_blend_normal(verts, vo, ip, h.u, h.v, h.normal);
-				h.flags = bStarted ? VXB_SPHERE_STARTED_IN_CONTACT : 0u;
-				h.level = __ldg(&rec->level);
-			}
-			hits[q] = h;
-		}
-	}
-}
-
-// One warp per query point, persistent over the batch.  Lane k < 27 takes neighbour k of the point's block clamped into the
-// grid (vxb_point_candidate's arithmetic), finds that block's covering cut node and keeps it when the node's measured box is
-// within max_distance + VXB_RAY_EPS of the point.  Lanes that reach the same node hand it on once (the lowest lane); the warp
-// then tests each node's drawn triangles strided over the lanes.  Points and hits in OUTPUT (Y-up) coordinates.
-//   every contributing node is a candidate   a drawn triangle within max_distance m of p (the test accepts it) is within m
-//                   (+ rounding) of a point of the node's measured box, which holds every drawn vertex; the float box distance
-//                   is within a few ulps of the true one, so the node is kept.  Its lattice box then lies within e + m + eps <=
-//                   15 + 1/16 < 16 of p along every axis (the host refuses e + m > 15).  Along an axis where p lies inside the
-//                   grid, the lattice box (a run of whole level-0 blocks) holds a block whose index is that of p's block +-1;
-//                   where p lies outside, it holds the first or last block of the axis, the clamped index.  So one of the 27
-//                   neighbours lies inside the node, and since the cut tiles the grid, that neighbour's covering node is it.
-//   handled once    __match_any_sync over the lanes' slots, the lowest lane of each group hands the node on.
-__global__ void __launch_bounds__(VXB_COLLIDE_THREADS) vxb_closest_point_cut_kernel(const VxbCutRayMesh c, const float maxDistance,
-	const float* __restrict__ points, unsigned count, vxb_closest_cut_hit* __restrict__ hits)
-{
-	const unsigned lane = threadIdx.x & 31;
-	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
-	const float md2 = maxDistance * maxDistance, reach = maxDistance + VXB_RAY_EPS;
-	const int nb = c.m.nb;
-	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
-	{
-		const float3 p = make_float3(points[3 * q], points[3 * q + 1], points[3 * q + 2]);
-		float bd = CUDART_INF_F, bu = 0.f, bv = 0.f;   // this lane's nearest triangle
-		float3 bp = make_float3(0.f, 0.f, 0.f);
-		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		unsigned slot = VXB_RAY_MISS;
-		if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && lane < 27)
-		{
-			const float top = (float)(nb - 1);
-			const int bx = (int)fminf(fmaxf(floorf(p.x * 0.0625f), 0.f), top) + (int)(lane % 3) - 1;
-			const int by = (int)fminf(fmaxf(floorf(p.y * 0.0625f), 0.f), top) + (int)((lane / 3) % 3) - 1;
-			const int bz = (int)fminf(fmaxf(floorf(p.z * 0.0625f), 0.f), top) + (int)(lane / 9) - 1;
-			if (bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb)
-			{
-				unsigned key;
-				const unsigned s = vxb_cut_node(c, bx, bz, by, key);   // grid (x, y, z) = output (x, z, y)
-				if (s != VXB_RAY_MISS)
-				{
-					const float4 lo = __ldg(&c.boxes[2 * (size_t)key]), hi = __ldg(&c.boxes[2 * (size_t)key + 1]);
-					const float gx = fmaxf(fmaxf(lo.x - p.x, p.x - hi.x), 0.f);
-					const float gy = fmaxf(fmaxf(lo.y - p.y, p.y - hi.y), 0.f);
-					const float gz = fmaxf(fmaxf(lo.z - p.z, p.z - hi.z), 0.f);
-					if (VXB_SQRT((gx * gx + gy * gy) + gz * gz) <= reach) slot = s;
-				}
-			}
-		}
-		const unsigned peers = __match_any_sync(0xFFFFFFFFu, slot);   // every lane takes part
-		vxb_warp_each(slot != VXB_RAY_MISS && (peers & ((1u << lane) - 1u)) == 0, slot, [&](const unsigned s) {
-			vxb_cut_triangles(c, s, [&](unsigned key, const float3& p0, const float3& p1, const float3& p2) {
-				float3 x;
-				float u, v;
-				vxb_closest_on_triangle(p, p0, p1, p2, x, u, v);
-				const float d2 = vxb_dist2(p, x);
-				if (d2 <= md2 && vxb_ray_before(d2, s, key, bd, bs, bk)) { bd = d2; bs = s; bk = key; bu = u; bv = v; bp = x; }
-			});
-		});
-		if (lane == vxb_ray_winner(bd, bs, bk))
-		{
-			vxb_closest_cut_hit h;
-			h.distance = CUDART_INF_F; h.slot = VXB_RAY_MISS; h.block_id = 0; h.triangle = 0;
-			h.point[0] = h.point[1] = h.point[2] = 0.f;
-			h.normal[0] = h.normal[1] = h.normal[2] = 0.f;
-			h.u = 0.f; h.v = 0.f; h.level = 0; h.face = 0;
-			if (bs != VXB_RAY_MISS)
-			{
-				const vxb_block_record* rec = c.m.dir + bs;
-				const VxbVertex* verts;
-				unsigned vo;
-				const unsigned* ip;
-				h.face = vxb_cut_hit_part(c, rec, bk, verts, vo, ip);
-				h.distance = VXB_SQRT(bd); h.slot = bs; h.block_id = __ldg(&rec->id); h.triangle = bk & 0xFFFFFFu;
-				h.point[0] = bp.x; h.point[1] = bp.y; h.point[2] = bp.z;
-				h.u = bu; h.v = bv;
-				vxb_blend_normal(verts, vo, ip, bu, bv, h.normal);
-				h.level = __ldg(&rec->level);
-			}
-			hits[q] = h;
-		}
-	}
+	if (p) { verts = c.tverts; vo = __ldg(&rec->trans_vertex_offset[p - 1]); ip = c.tidx + __ldg(&rec->trans_index_offset[p - 1]) + 3 * k; }
+	else { verts = c.m.verts; vo = __ldg(&rec->vertex_offset); ip = c.m.idx + __ldg(&rec->index_offset) + 3 * k; }
 }
 
 // The cut reach of a capsule query (include/vxb200.h "capsule queries against the drawn LOD cut"), in float for the host
@@ -405,165 +200,97 @@ VXB_HD bool vxb_capsule_cut_reach(const float3 h, float extra, float e)
 	return vxb_capsule_reach(h, extra) && e + (hm + extra) <= VXB_SPHERE_RADIUS_MAX;
 }
 
-// One warp per capsule sweep, persistent over the batch: the cut walk with the clip box grown by e + max_i |h_i| + r +
-// VXB_RAY_EPS and every node's measured box by max_i |h_i| + r + VXB_RAY_EPS (both rounded up; "capsules" at the top), then
-// on the drawn triangles the level-0 kernel's per-triangle reject and the capsule's tests (vxb_capsule_triangle).  A sweep
-// out of cut reach is a miss.  Sweeps and hits in OUTPUT (Y-up) coordinates.  (Two CTAs per SM in the launch bounds: ptxas
-// then fits the kernel in 127 registers without a stack frame or spills, the occupancy of vxb_capsule_cast_kernel; with one
-// CTA per SM it takes 136 registers and runs slower, DESIGN.md section 6.)
-__global__ void __launch_bounds__(VXB_COLLIDE_THREADS, 2) vxb_capsule_cast_cut_kernel(const VxbCutRayMesh c,
-	const vxb_capsule_sweep* __restrict__ sweeps, unsigned count, vxb_capsule_cut_hit* __restrict__ hits)
+// ---- the drawn cut as a surface ------------------------------------------------------------------------------------------
+//
+// The drawn triangles of the cut for the query bodies (vxb_query.cuh), as VxbLevel0Surface is for level 0.  Keys are
+// part << 24 | triangle (vxb_cut_triangles); the hit's tail is the winning node's level and the face of its part.
+struct VxbCutSurface
 {
-	const unsigned lane = threadIdx.x & 31;
-	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
-	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
-	{
-		const vxb_capsule_sweep cs = sweeps[q];
-		const vxb_ray& ray = cs.path;
-		const float3 o = make_float3(ray.origin[0], ray.origin[1], ray.origin[2]);
-		const float3 d = make_float3(ray.direction[0], ray.direction[1], ray.direction[2]);
-		const float3 h = make_float3(cs.half_axis[0], cs.half_axis[1], cs.half_axis[2]);
-		const float r = cs.radius, rr = r * r;
-		const float tMin = ray.t_min, tMax = ray.t_max;
-		const float3 c0 = make_float3(o.x + tMin * d.x, o.y + tMin * d.y, o.z + tMin * d.z);
-		const float dd = (d.x * d.x + d.y * d.y) + d.z * d.z;
-		const float3 g = make_float3(fabsf(h.x) + r + VXB_RAY_EPS, fabsf(h.y) + r + VXB_RAY_EPS, fabsf(h.z) + r + VXB_RAY_EPS);
-		const float R = __fadd_ru(fmaxf(fmaxf(fabsf(h.x), fabsf(h.y)), fabsf(h.z)), r);
-		const float gn = __fadd_ru(R, VXB_RAY_EPS), clip = __fadd_ru(c.grow, R);
-		float bt = CUDART_INF_F;   // this lane's first contact
-		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		bool bStarted = false;
-		if (r > 0.f && vxb_capsule_cut_reach(h, r, c.excursion))   // the same for the whole warp
-			vxb_ray_walk_by<true>(c.m.nb, ray, clip, bt,
-				[&](int bx, int by, int bz, float T0, float T1, float t0, float t1, bool last, unsigned& slot) {
-					return vxb_cut_candidate(c, ray, gn, bx, by, bz, T0, T1, t0, t1, last, slot);
-				},
-				[&](const unsigned s) {
-					vxb_cut_triangles(c, s, [&](unsigned key, const float3& p0, const float3& p1, const float3& p2) {
-						if (!vxb_path_meets_box(ray, g, p0, p1, p2)) return;
-						bool started;
-						const float t = vxb_capsule_triangle(o, d, c0, h, r, rr, dd, tMin, tMax, p0, p1, p2, started);
-						if (t < CUDART_INF_F && vxb_ray_before(t, s, key, bt, bs, bk)) { bt = t; bs = s; bk = key; bStarted = started; }
-					});
-				});
-		if (lane == vxb_ray_winner(bt, bs, bk))
-		{
-			vxb_capsule_cut_hit x;
-			x.t = CUDART_INF_F; x.slot = VXB_RAY_MISS; x.block_id = 0; x.triangle = 0;
-			x.center[0] = x.center[1] = x.center[2] = 0.f;
-			x.point[0] = x.point[1] = x.point[2] = 0.f;
-			x.axis_point[0] = x.axis_point[1] = x.axis_point[2] = 0.f;
-			x.normal[0] = x.normal[1] = x.normal[2] = 0.f;
-			x.u = 0.f; x.v = 0.f; x.s = 0.f; x.flags = 0; x.level = 0; x.face = 0;
-			if (bs != VXB_RAY_MISS)
-			{
-				const vxb_block_record* rec = c.m.dir + bs;
-				const VxbVertex* verts;
-				unsigned vo;
-				const unsigned* ip;
-				x.face = vxb_cut_hit_part(c, rec, bk, verts, vo, ip);
-				const unsigned adj = vxb_cut_adj(c, rec);
-				const float3 p0 = vxb_cut_vertex(verts, vo, __ldg(ip), adj);
-				const float3 p1 = vxb_cut_vertex(verts, vo, __ldg(ip + 1), adj);
-				const float3 p2 = vxb_cut_vertex(verts, vo, __ldg(ip + 2), adj);
-				const float3 ct = make_float3(o.x + bt * d.x, o.y + bt * d.y, o.z + bt * d.z);
-				float3 pq, px;
-				vxb_pair_fields(ct, h, p0, p1, p2, pq, px, x.u, x.v, x.s);
-				x.point[0] = pq.x; x.point[1] = pq.y; x.point[2] = pq.z;
-				x.axis_point[0] = px.x; x.axis_point[1] = px.y; x.axis_point[2] = px.z;
-				x.t = bt; x.slot = bs; x.block_id = __ldg(&rec->id); x.triangle = bk & 0xFFFFFFu;
-				x.center[0] = ct.x; x.center[1] = ct.y; x.center[2] = ct.z;
-				vxb_blend_normal(verts, vo, ip, x.u, x.v, x.normal);
-				x.flags = bStarted ? VXB_SPHERE_STARTED_IN_CONTACT : 0u;
-				x.level = __ldg(&rec->level);
-			}
-			hits[q] = x;
-		}
-	}
-}
+	const VxbCutRayMesh& c;
 
-// One warp per segment, persistent over the batch.  Lane k < 27 takes neighbour k of the centre's block clamped into the
-// grid (vxb_point_candidate's arithmetic), finds that block's covering cut node and keeps it when the node's measured box
-// lies within |h_i| + max_distance + VXB_RAY_EPS of the centre along every axis (the proof under "capsules" at the top).
-// Lanes that reach the same node hand it on once (the lowest lane); the warp then runs the level-0 kernel's per-axis reject
-// and the closest pair (vxb_segment_triangle) on each node's drawn triangles, strided over the lanes.  A segment out of cut
-// reach is a miss.  OUTPUT (Y-up) coordinates.  (A minimum of one CTA per SM in the launch bounds, as
-// vxb_closest_segment_kernel.)
-__global__ void __launch_bounds__(VXB_COLLIDE_THREADS, 1) vxb_closest_segment_cut_kernel(const VxbCutRayMesh c, const float maxDistance,
-	const vxb_segment* __restrict__ segments, unsigned count, vxb_segment_cut_hit* __restrict__ hits)
-{
-	const unsigned lane = threadIdx.x & 31;
-	const unsigned warps = gridDim.x * (VXB_COLLIDE_THREADS / 32);
-	const float md2 = maxDistance * maxDistance;
-	const int nb = c.m.nb;
-	for (unsigned q = blockIdx.x * (VXB_COLLIDE_THREADS / 32) + (threadIdx.x >> 5); q < count; q += warps)
+	// The cut walk of a shape whose reach splits as hm = max_i |h_i| and r (both 0 for rays, hm = -0 for spheres): with R = hm + r
+	// rounded up, the clip box grown by e + R + VXB_RAY_EPS and every node's measured box by R + VXB_RAY_EPS (both rounded up;
+	// the proofs at the top).  For rays R = 0, and for spheres R = r, so their growths are c.grow and VXB_RAY_EPS, r + eps.
+	template <class Block>
+	VXB_FN void walk(const vxb_ray& ray, float hm, float r, const float& best, Block&& block) const
 	{
-		const vxb_segment sg = segments[q];
-		const float3 p = make_float3(sg.center[0], sg.center[1], sg.center[2]);
-		const float3 h = make_float3(sg.half_axis[0], sg.half_axis[1], sg.half_axis[2]);
-		const float3 g = make_float3(fabsf(h.x) + maxDistance + VXB_RAY_EPS, fabsf(h.y) + maxDistance + VXB_RAY_EPS,
-			fabsf(h.z) + maxDistance + VXB_RAY_EPS);
-		float bd = CUDART_INF_F;   // this lane's nearest triangle
-		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		unsigned slot = VXB_RAY_MISS;
-		if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && vxb_capsule_cut_reach(h, maxDistance, c.excursion) && lane < 27)
+		const float R = __fadd_ru(hm, r);
+		const float g = __fadd_ru(R, VXB_RAY_EPS);
+		vxb_ray_walk_by<true>(c.m.nb, ray, __fadd_ru(c.grow, R), best,
+			[&](int bx, int by, int bz, float T0, float T1, float t0, float t1, bool last, unsigned& slot) {
+				return vxb_cut_candidate(c, ray, g, bx, by, bz, T0, T1, t0, t1, last, slot);
+			},
+			block);
+	}
+
+	// The point candidate: lane k < 27 takes neighbour k of the point's block clamped into the grid (vxb_point_candidate),
+	// finds that block's covering cut node and keeps it when `near(lo, hi)` accepts the node's measured box.  Lanes that reach
+	// the same node hand it on once (the lowest lane).  For a closest-point query within max_distance m:
+	//   every contributing node is a candidate   a drawn triangle within max_distance m of p (the test accepts it) is within m
+	//                   (+ rounding) of a point of the node's measured box, which holds every drawn vertex; the float box distance
+	//                   is within a few ulps of the true one, so the node is kept.  Its lattice box then lies within e + m + eps <=
+	//                   15 + 1/16 < 16 of p along every axis (the host refuses e + m > 15).  Along an axis where p lies inside the
+	//                   grid, the lattice box (a run of whole level-0 blocks) holds a block whose index is that of p's block +-1;
+	//                   where p lies outside, it holds the first or last block of the axis, the clamped index.  So one of the 27
+	//                   neighbours lies inside the node, and since the cut tiles the grid, that neighbour's covering node is it.
+	//   handled once    __match_any_sync over the lanes' slots, the lowest lane of each group hands the node on.
+	template <class Near>
+	VXB_FN bool point(const float3 p, bool ok, Near&& near, unsigned& slot) const
+	{
+		vxb_point_candidate(c.m.nb, p, ok, [&](int bx, int by, int bz, unsigned& s) {
+			unsigned key;
+			const unsigned n = vxb_cut_node(c, bx, bz, by, key);   // grid (x, y, z) = output (x, z, y)
+			if (n == VXB_RAY_MISS) return false;
+			const float4 lo = __ldg(&c.boxes[2 * (size_t)key]), hi = __ldg(&c.boxes[2 * (size_t)key + 1]);
+			if (!near(make_float3(lo.x, lo.y, lo.z), make_float3(hi.x, hi.y, hi.z))) return false;
+			s = n;
+			return true;
+		}, slot);
+		const unsigned lane = threadIdx.x & 31;
+		const unsigned peers = __match_any_sync(0xFFFFFFFFu, slot);   // every lane takes part (lanes without a node hold VXB_RAY_MISS)
+		return slot != VXB_RAY_MISS && (peers & ((1u << lane) - 1u)) == 0;
+	}
+
+	template <class F>
+	VXB_FN void triangles(unsigned s, F&& f) const { vxb_cut_triangles(c, s, f); }
+
+	VXB_FN const vxb_block_record* record(unsigned s) const { return c.m.dir + s; }
+
+	// the positions of the winning triangle key (part << 24 | k) of the cut node at directory record rec as the renderer draws
+	// them, and its blended normal at (u, v)
+	VXB_FN void corners(const vxb_block_record* rec, unsigned key, float3& p0, float3& p1, float3& p2) const
+	{
+		const VxbVertex* verts;
+		unsigned vo;
+		const unsigned* ip;
+		vxb_cut_hit_part(c, rec, key, verts, vo, ip);
+		const unsigned adj = vxb_cut_adj(c, rec);
+		p0 = vxb_cut_vertex(verts, vo, __ldg(ip), adj);
+		p1 = vxb_cut_vertex(verts, vo, __ldg(ip + 1), adj);
+		p2 = vxb_cut_vertex(verts, vo, __ldg(ip + 2), adj);
+	}
+	VXB_FN void normal(const vxb_block_record* rec, unsigned key, float u, float v, float* out) const
+	{
+		const VxbVertex* verts;
+		unsigned vo;
+		const unsigned* ip;
+		vxb_cut_hit_part(c, rec, key, verts, vo, ip);
+		vxb_blend_normal(verts, vo, ip, u, v, out);
+	}
+
+	VXB_FN unsigned triangle(unsigned key) const { return key & 0xFFFFFFu; }
+
+	VXB_FN bool reach(const float3 h, float extra) const { return vxb_capsule_cut_reach(h, extra, c.excursion); }
+
+	// level and face (0xFFFFFFFF for the regular part) of a hit, 0 and 0 for a miss
+	template <class Hit>
+	VXB_FN void tail(Hit& h, unsigned s, unsigned key) const
+	{
+		h.level = 0; h.face = 0;
+		if (s != VXB_RAY_MISS)
 		{
-			const float top = (float)(nb - 1);
-			const int bx = (int)fminf(fmaxf(floorf(p.x * 0.0625f), 0.f), top) + (int)(lane % 3) - 1;
-			const int by = (int)fminf(fmaxf(floorf(p.y * 0.0625f), 0.f), top) + (int)((lane / 3) % 3) - 1;
-			const int bz = (int)fminf(fmaxf(floorf(p.z * 0.0625f), 0.f), top) + (int)(lane / 9) - 1;
-			if (bx >= 0 && by >= 0 && bz >= 0 && bx < nb && by < nb && bz < nb)
-			{
-				unsigned key;
-				const unsigned s = vxb_cut_node(c, bx, bz, by, key);   // grid (x, y, z) = output (x, z, y)
-				if (s != VXB_RAY_MISS)
-				{
-					const float4 lo = __ldg(&c.boxes[2 * (size_t)key]), hi = __ldg(&c.boxes[2 * (size_t)key + 1]);
-					if (!(lo.x - p.x > g.x || p.x - hi.x > g.x) && !(lo.y - p.y > g.y || p.y - hi.y > g.y) &&
-						!(lo.z - p.z > g.z || p.z - hi.z > g.z)) slot = s;
-				}
-			}
-		}
-		const unsigned peers = __match_any_sync(0xFFFFFFFFu, slot);   // every lane takes part
-		vxb_warp_each(slot != VXB_RAY_MISS && (peers & ((1u << lane) - 1u)) == 0, slot, [&](const unsigned s) {
-			vxb_cut_triangles(c, s, [&](unsigned key, const float3& p0, const float3& p1, const float3& p2) {
-				if (fminf(fminf(p0.x, p1.x), p2.x) - p.x > g.x || p.x - fmaxf(fmaxf(p0.x, p1.x), p2.x) > g.x ||
-					fminf(fminf(p0.y, p1.y), p2.y) - p.y > g.y || p.y - fmaxf(fmaxf(p0.y, p1.y), p2.y) > g.y ||
-					fminf(fminf(p0.z, p1.z), p2.z) - p.z > g.z || p.z - fmaxf(fmaxf(p0.z, p1.z), p2.z) > g.z) return;
-				float3 x;
-				float u, v, w;
-				const float d2 = vxb_segment_triangle(p, h, p0, p1, p2, x, u, v, w);
-				if (d2 <= md2 && vxb_ray_before(d2, s, key, bd, bs, bk)) { bd = d2; bs = s; bk = key; }
-			});
-		});
-		if (lane == vxb_ray_winner(bd, bs, bk))
-		{
-			vxb_segment_cut_hit x;
-			x.distance = CUDART_INF_F; x.slot = VXB_RAY_MISS; x.block_id = 0; x.triangle = 0;
-			x.point[0] = x.point[1] = x.point[2] = 0.f;
-			x.axis_point[0] = x.axis_point[1] = x.axis_point[2] = 0.f;
-			x.normal[0] = x.normal[1] = x.normal[2] = 0.f;
-			x.u = 0.f; x.v = 0.f; x.s = 0.f; x.level = 0; x.face = 0;
-			if (bs != VXB_RAY_MISS)
-			{
-				const vxb_block_record* rec = c.m.dir + bs;
-				const VxbVertex* verts;
-				unsigned vo;
-				const unsigned* ip;
-				x.face = vxb_cut_hit_part(c, rec, bk, verts, vo, ip);
-				const unsigned adj = vxb_cut_adj(c, rec);
-				const float3 p0 = vxb_cut_vertex(verts, vo, __ldg(ip), adj);
-				const float3 p1 = vxb_cut_vertex(verts, vo, __ldg(ip + 1), adj);
-				const float3 p2 = vxb_cut_vertex(verts, vo, __ldg(ip + 2), adj);
-				float3 pq, px;
-				vxb_pair_fields(p, h, p0, p1, p2, pq, px, x.u, x.v, x.s);
-				x.point[0] = pq.x; x.point[1] = pq.y; x.point[2] = pq.z;
-				x.axis_point[0] = px.x; x.axis_point[1] = px.y; x.axis_point[2] = px.z;
-				x.distance = VXB_SQRT(bd); x.slot = bs; x.block_id = __ldg(&rec->id); x.triangle = bk & 0xFFFFFFu;
-				vxb_blend_normal(verts, vo, ip, x.u, x.v, x.normal);
-				x.level = __ldg(&rec->level);
-			}
-			hits[q] = x;
+			const unsigned p = key >> 24;
+			h.level = __ldg(&c.m.dir[s].level); h.face = p ? p - 1 : 0xFFFFFFFFu;
 		}
 	}
-}
+};

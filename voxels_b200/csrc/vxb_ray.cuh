@@ -18,7 +18,7 @@
 //                t >= that.  With the margin 2^-20 |t1|, t1 > best + margin proves t > best for every remaining hit: no hit
 //                can tie or beat the best one, and the walk ends.
 //
-// Sphere sweeps (vxb_collide.cuh) run the same walk with the boxes grown by g = r + VXB_RAY_EPS instead of VXB_RAY_EPS:
+// Sphere sweeps (vxb_sphere_cast_body) run the same walk with the boxes grown by g = r + VXB_RAY_EPS instead of VXB_RAY_EPS:
 //   tested set   a contact the sweep's tests accept puts the centre within r (+ rounding) of its triangle, hence of the
 //                triangle's block, hence inside that block's box grown by r + eps.  A sweep that starts in contact has
 //                c(t_min) there too, so the block's te is the clipped start.  The planes 16 b -+ g are now rounded (g is any
@@ -32,7 +32,7 @@
 //   stop         unchanged: te is still two correctly rounded operations from the (rounded) plane, and a contact inside the
 //                grown box has t >= the true te.
 //
-// Capsule sweeps (half axis h, radius r; vxb_collide.cuh) run it with g = max_i |h_i| + r + VXB_RAY_EPS:
+// Capsule sweeps (half axis h, radius r; vxb_capsule_cast_body) run it with g = max_i |h_i| + r + VXB_RAY_EPS:
 //   tested set   a contact pairs a point c + x h of the capsule's segment (|x| <= 1) with a triangle point within r of it, so
 //                the centre c is within |x h_i| + r <= |h_i| + r <= g - eps (+ rounding) of the triangle along every axis
 //                i, hence inside its block's box grown by g.  A sweep that starts in contact has c(t_min) there too.
@@ -148,13 +148,6 @@ VXB_FN void vxb_blend_normal(const VxbVertex* verts, unsigned vo, const unsigned
 	const float len = VXB_SQRT((nxv * nxv + nyv * nyv) + nzv * nzv);
 	out[0] = out[1] = out[2] = 0.f;
 	if (len > 0.f) { out[0] = VXB_DIV(nxv, len); out[1] = VXB_DIV(nyv, len); out[2] = VXB_DIV(nzv, len); }
-}
-
-// the blended normal of regular triangle k of slot s
-VXB_FN void vxb_ray_blend_normal(const VxbRayMesh& m, unsigned s, unsigned k, float u, float v, float* out)
-{
-	const vxb_block_record* rec = m.dir + s;
-	vxb_blend_normal(m.verts, __ldg(&rec->vertex_offset), m.idx + __ldg(&rec->index_offset) + 3 * k, u, v, out);
 }
 
 // The lane holding the warp's least (t, slot, triangle) by the tie rule (every lane takes part; each candidate is held by
@@ -284,46 +277,4 @@ VXB_FN void vxb_ray_walk(const VxbRayMesh& m, const vxb_ray& ray, const float gr
 			return false;
 		},
 		block);
-}
-
-// One warp per ray, persistent over the batch.  Rays and hits in OUTPUT (Y-up) coordinates.
-__global__ void __launch_bounds__(VXB_RAY_THREADS) vxb_raycast_kernel(const VxbRayMesh m, const vxb_ray* __restrict__ rays, unsigned count,
-	vxb_ray_hit* __restrict__ hits)
-{
-	const unsigned lane = threadIdx.x & 31;
-	const unsigned warps = gridDim.x * (VXB_RAY_THREADS / 32);
-	for (unsigned r = blockIdx.x * (VXB_RAY_THREADS / 32) + (threadIdx.x >> 5); r < count; r += warps)
-	{
-		const vxb_ray ray = rays[r];
-		const float px = ray.origin[0], py = ray.origin[1], pz = ray.origin[2];
-		const float dx = ray.direction[0], dy = ray.direction[1], dz = ray.direction[2];
-		const float tMin = ray.t_min, tMax = ray.t_max;
-		float bt = CUDART_INF_F, bu = 0.f, bv = 0.f;   // this lane's best hit
-		unsigned bs = VXB_RAY_MISS, bk = VXB_RAY_MISS;
-		vxb_ray_walk(m, ray, VXB_RAY_EPS, bt, [&](const unsigned s) {
-			vxb_slot_triangles(m, s, [&](unsigned k, const float3& p0, const float3& p1, const float3& p2) {
-				float t, u, v;
-				if (vxb_ray_mt(px, py, pz, dx, dy, dz, tMin, tMax, p0, p1, p2, t, u, v) && vxb_ray_before(t, s, k, bt, bs, bk))
-				{
-					bt = t; bs = s; bk = k; bu = u; bv = v;
-				}
-			});
-		});
-		// ---- the winner by the tie rule; its lane writes the hit ----
-		if (lane == vxb_ray_winner(bt, bs, bk))
-		{
-			vxb_ray_hit h;
-			h.u = 0.f; h.v = 0.f; h.slot = VXB_RAY_MISS; h.block_id = 0; h.triangle = 0;
-			h.t = CUDART_INF_F;
-			h.position[0] = h.position[1] = h.position[2] = 0.f;
-			h.normal[0] = h.normal[1] = h.normal[2] = 0.f;
-			if (bs != VXB_RAY_MISS)
-			{
-				h.t = bt; h.u = bu; h.v = bv; h.slot = bs; h.block_id = __ldg(&m.dir[bs].id); h.triangle = bk;
-				h.position[0] = px + bt * dx; h.position[1] = py + bt * dy; h.position[2] = pz + bt * dz;
-				vxb_ray_blend_normal(m, bs, bk, bu, bv, h.normal);
-			}
-			hits[r] = h;
-		}
-	}
 }
