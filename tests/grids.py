@@ -68,8 +68,15 @@ RLE_EDGES = {
 }
 
 
+# the block kernels' per-block capacities (tests/test_thresholds_cpu.py, tests/test_gpu_thresholds.py): not in the tables
+# above, so that their golden digests stay as they are
+THRESHOLDS = {
+    "thresholds256": gridgen.thresholds256,
+}
+
+
 def by_name(name):
-    for table in (SMALL, MEDIUM, LARGE, HUGE, RLE_EDGES):
+    for table in (SMALL, MEDIUM, LARGE, HUGE, RLE_EDGES, THRESHOLDS):
         if name in table:
             return table[name]()
     raise KeyError(name)

@@ -11,6 +11,10 @@ and, in the grid built for it (gridgen.skip_quirk), the level-0 skip of a block 
 the surface runs along its faces (TransVoxelImpl.cpp:520).  The patchwork grids must never reach that skip: the
 reference's coarse cells over a skipped block read an uninitialised material, so their output is not defined.
 
+Here a route only has to be reached; the exact edges of the capacities (1023 / 1024 / 1025 cells at levels 0-2, 2047 /
+2048 / 2049 level-0 vertices, both at once, and the flips between them) live in the threshold grid, gridgen.thresholds256,
+whose counts tests/test_thresholds_cpu.py pins.
+
 The grid store's thresholds are pinned the same way: the rle_edges grids reach BF_Empty through the walk of
 vxb_block_info_kernel with both outcomes, the 2048 / 2049-run codec boundary in all three channels, and (only
 rle_edges_skipped) the skip; hostile64_full_range spans the whole int8 range."""
